@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — benchmark of the rasterizer / fusion hot path on the BASELINE.json configs (DESIGN.md §7).
+"""bench.py — benchmark of the rasterizer / fusion hot path on the BASELINE.json configs.
 
   --config K3 (default)  configs[2], the one the metric is quoted on: 1 M Gaussians x 256-ch features, 1920x1080,
                          one view per rank per step, forward + backward (+ gradient exchange at N > 1)
@@ -15,6 +15,10 @@ One JSON line on stdout (rank 0):
   roofline       dominant kernel: algorithmic bytes / CUDA-event duration against the measured HBM peak
   cpu_baseline   the CPU port of the reference algorithm on a bounded sample (rank 0, N = 1)
   --impl reference   times that CPU port alone (rank 0 only), same JSON contract
+  --dump-outputs DIR (K3) after the timed steps, rank 0 writes what the last timed step computed -- the rendered
+                     feature image, the radii and the gradients of the five parameter tensors -- as DIR/<name>.npy
+                     (float32; arrays above DUMP_MAX_ENTRIES entries as a fixed seeded sample of them), so that two
+                     builds run with the same arguments can be compared output for output
 """
 from __future__ import annotations
 
@@ -27,6 +31,7 @@ import subprocess
 import sys
 import tempfile
 import time
+import zlib
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
@@ -55,6 +60,22 @@ CONFIGS = {
 }
 
 
+DUMP_MAX_ENTRIES = 1 << 21   # 8 MB per array, 56 MB for the seven K3 outputs
+
+
+def dump_outputs(torch, path, arrays):
+    """Writes each tensor as <path>/<name>.npy in float32.  A tensor above DUMP_MAX_ENTRIES entries is flattened and
+    sampled at DUMP_MAX_ENTRIES sorted indices drawn from a generator seeded by its name: the same entries on every run."""
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach()
+        if t.numel() > DUMP_MAX_ENTRIES:
+            g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+            idx = torch.randint(0, t.numel(), (DUMP_MAX_ENTRIES,), generator=g).sort().values
+            t = t.reshape(-1)[idx.to(t.device)]
+        np.save(os.path.join(path, name + ".npy"), t.float().cpu().numpy())
+
+
 def env_int(name, default):
     try:
         return int(os.environ.get(name, default))
@@ -69,7 +90,7 @@ def measured_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "MEASURED_PEAKS.json (of measured)"
         except Exception:
             pass
-    return 6650.0, "B200_PROFILING.md fallback (of fallback)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 def build_info():
@@ -105,19 +126,6 @@ def emit_line(line):
     out = _RESULT_OUT or sys.stdout
     out.write(json.dumps(line) + "\n")
     out.flush()
-
-
-def traffic_for(kernel, src_hash):
-    """Measured DRAM bytes per launch (ncu --set full), only when the capture was taken from THIS source tree."""
-    tpath = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    try:
-        t = json.load(open(tpath))
-    except Exception:
-        return None, "no profiles/dram_traffic.json"
-    if t.get("_src_sha256_16") != src_hash:
-        return None, (f"profiles/dram_traffic.json was captured from sources {t.get('_src_sha256_16')}, "
-                      f"not {src_hash}: stale, ignored")
-    return t.get(kernel), t.get("_source")
 
 
 # ------------------------------------------------------------------------------ clocks sampler
@@ -357,7 +365,7 @@ def run_cpu_reference(args, rank, world):
 
 # ------------------------------------------------------------------------------ roofline helpers
 def algorithmic_bytes(P, P_vis, R, C, W, H):
-    """SURVEY.md §8(d) / BASELINE.md §4 compulsory traffic, split by kernel (DESIGN.md §3)."""
+    """Compulsory traffic, split by kernel."""
     px = W * H
     # per kernel: every input read once, every output written once
     alpha = 4 * R + 32 * P_vis + 8 * px                       # ids + splat records in, final_T / n_contrib out
@@ -373,13 +381,13 @@ def algorithmic_bytes(P, P_vis, R, C, W, H):
                 tile_sort=tile_sort, fwd=fwd_total + (4 * px if C <= 4 else 0), bwd=bwd_total)
 
 
-FMA_PEAK_TFLOPS = 70.5   # dependent-free FFMA loop on this pool's B200s (tools/microbench.cu, BASELINE.md §6)
+FMA_PEAK_TFLOPS = 67.0   # H100 SXM data sheet, dense FP32 (not measured; a power-limited card clocks lower)
 
 
 def fma_roofline(C, blended_pairs, per_stage):
-    """fp32 CUDA-core roof of the three C-wide contractions (DESIGN.md §3): achieved = algorithmic flops
+    """fp32 CUDA-core roof of the three C-wide contractions: achieved = algorithmic flops
     (2*C per blended pair and contraction, zero-weight padding not counted) / stage time."""
-    out = {"peak_tflops": FMA_PEAK_TFLOPS, "peak_source": "measured FFMA micro-benchmark (tools/microbench.cu)",
+    out = {"peak_tflops": FMA_PEAK_TFLOPS, "peak_source": "H100 SXM data sheet, dense FP32 (not measured)",
            "algorithmic_flops_per_contraction": 2 * C * blended_pairs, "kernels": {}}
     for k in ("blend_fwd", "blend_bwd", "dfeature"):
         ms = per_stage.get(k)
@@ -495,7 +503,7 @@ class Harness:
 
 
 def view_stats(h, cfg, pc, feats_or_none, cam, bg):
-    """P_vis, R, mean list lengths of one view (reported with every timing, BASELINE.md §3)."""
+    """P_vis, R, mean list lengths of one view (reported with every timing)."""
     torch, _lib = h.torch, h._lib
     from semantic_gaussians_b200.rasterizer import _C_chn, _C_rgbd
     P, C, W, H = cfg["P"], cfg["C"], cfg["W"], cfg["H"]
@@ -524,14 +532,13 @@ def view_stats(h, cfg, pc, feats_or_none, cam, bg):
     return out
 
 
-def roofline_block(per_stage, ab, candidates, src_hash, note=None, config="K3"):
+def roofline_block(per_stage, ab, candidates, note=None):
     peak, peak_src = measured_peaks()
     dom = max(candidates, key=lambda k: per_stage.get(k, 0.0))
     dom_ms = per_stage.get(dom, float("nan"))
     achieved = ab[dom] / (dom_ms * 1e-3) * 1e-9
-    traffic, tsrc = traffic_for(f"{config}.{dom}", src_hash)   # captures are per config: K2 and K3 blend different kernels
     r = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-         "traffic": traffic, "traffic_source": tsrc, "algorithmic_bytes": ab[dom], "kernel_ms": dom_ms,
+         "algorithmic_bytes": ab[dom], "kernel_ms": dom_ms,
          "peak_source": peak_src}
     if note:
         r["note"] = note
@@ -594,6 +601,8 @@ def run_k3(args, rank, world, local_rank):
         # and at every step the `world` ranks render `world` DIFFERENT views
         return (i + rank) % NVIEWS
 
+    last = {}   # --dump-outputs: what the latest device step computed
+
     def step_device(i, exchange=True):
         out = render_chn(cams[view_of(i)], pc, Pipe, bg, num_channels=C, override_color=feats)
         if overlap is not None:
@@ -601,6 +610,9 @@ def run_k3(args, rank, world, local_rank):
         out["render"].backward(dL_fixed)
         if exchange:
             allreduce_grads()
+        if args.dump_outputs:
+            last.update(render=out["render"], radii=out["radii"],
+                        **{"dL_d" + n: p.grad for n, p in zip(("features", "xyz", "scaling", "rotation", "opacity"), params)})
         zero_grads()
 
     cam_dev = Cam()
@@ -702,6 +714,7 @@ def run_k3(args, rank, world, local_rank):
 
     # ---- device-resident timed region (stage tracing + clock sampling), then the same without the exchange
     ms_dev, ms_mine, per_stage, _, clocks, launches = h.profiled(step_device, args.steps)
+    timed_outputs = dict(last)
     rank_ms = h.gather_floats(ms_mine / args.steps)
     ms_nocomm = None
     if world > 1:
@@ -719,6 +732,9 @@ def run_k3(args, rank, world, local_rank):
     if rank != 0:
         h.finish()
         return
+    if args.dump_outputs:
+        dump_outputs(torch, args.dump_outputs, timed_outputs)
+    del timed_outputs
 
     views = args.steps * world
     value = views / (ms_dev * 1e-3) * 1e-6
@@ -738,8 +754,7 @@ def run_k3(args, rank, world, local_rank):
         "views_per_s": value * 1e6, "hbm_gbs_effective": eff_gbs, "hbm_frac_effective": eff_gbs / peak,
         "stage_ms": per_stage, "kernel_ms_per_step": sum(per_stage.values()),
         "roofline": roofline_block(per_stage, ab, ("blend_fwd", "blend_bwd", "dfeature", "alpha_pass"),
-                                   binfo["source_sha256_16"],
-                                   "C=256 blend is fp32-FMA bound by design (no tensor cores, north_star); see fma_roofline and DESIGN.md"),
+                                   "C=256 blend is fp32-FMA bound by design (no tensor cores, north_star); see fma_roofline"),
         # the C = 256 blend is three fp32 contractions on the CUDA cores (north_star rules out tensor cores):
         # algorithmic flops = 2*C per blended (pixel, Gaussian) pair for each of forward, s-pass, dL/dfeature
         "fma_roofline": fma_roofline(C, stats["blended_pairs"], per_stage),
@@ -788,10 +803,10 @@ def run_k3(args, rank, world, local_rank):
 
 
 def reference_cuda_times(torch, dev, sc, cam, dL, C, W, H, ours=None, cam_dev=None):
-    """The reference's channel-rasterization CUDA path recompiled for sm_100a, timed on this GPU: forward by the
+    """The reference's channel-rasterization CUDA path recompiled for sm_90a, timed on this GPU: forward by the
     stock library, forward as render_chn() ships it (debug=True: a CPU deep copy of every argument before the
-    call, channel_rasterization/__init__.py:86-87, model/renderer.py:181), backward by the NUM_CHANNELS=C rebuild
-    (SURVEY.md 2d-1).  Also compares our image with the reference's on this exact view."""
+    call, channel_rasterization/__init__.py:86-87, model/renderer.py:181), backward by the NUM_CHANNELS=C rebuild.
+    Also compares our image with the reference's on this exact view."""
     out = {}
     try:
         from oracle import ref as refmod
@@ -838,7 +853,7 @@ def reference_cuda_times(torch, dev, sc, cam, dL, C, W, H, ours=None, cam_dev=No
             r2 = refmod.RefRasterizer(f"chn_c{C}")
             r2.forward(**kw)
             out["bwd_ms"] = ev_time(lambda: r2.backward(dL), 1)
-        out["kind"] = "unmodified reference cuda_rasterizer compiled for sm_100a (oracle/_ref), debug=False unless named"
+        out["kind"] = "unmodified reference cuda_rasterizer compiled for sm_90a (oracle/_ref), debug=False unless named"
     except Exception as ex:  # pragma: no cover
         out["error"] = repr(ex)
     return out
@@ -907,7 +922,7 @@ def run_k2(args, rank, world, local_rank):
                    "l2": "8 cycling views; 45 M-instance sort streams (0.5 GB) exceed L2", **stats},
         "views_per_s": value * 1e6, "hbm_gbs_effective": eff, "hbm_frac_effective": eff / peak,
         "stage_ms": per_stage, "kernel_ms_per_step": sum(per_stage.values()),
-        "roofline": roofline_block(per_stage, ab, ("blend_fwd", "tile_sort"), binfo["source_sha256_16"], config="K2"),
+        "roofline": roofline_block(per_stage, ab, ("blend_fwd", "tile_sort")),
         "e2e": {"value": views / (ms_e2e * 1e-3) * 1e-6, "unit": "Mviews/s", "ms_per_step": ms_e2e / args.steps,
                 "h2d_bytes_per_step": 35 * 4, "d2h_bytes_per_step": 16 * W * H,
                 "api": "render(): camera from pinned host memory, RGB image + median depth copied back to pinned memory"},
@@ -974,6 +989,7 @@ def run_k4(args, rank, world, local_rank):
             if batched:
                 outs = render_chn_batch([cams[k] for k in sub], pc, Pipe, bg, num_channels=C, override_color=feats)
                 torch.autograd.backward([o["render"] for o in outs], [dL_fixed] * len(outs))
+                del outs   # a sub-batch's images (2.6 GB per view) must be gone before the next one renders
             else:
                 for k in sub:
                     render_chn(cams[k], pc, Pipe, bg, num_channels=C, override_color=feats)["render"].backward(dL_fixed)
@@ -1013,6 +1029,7 @@ def run_k4(args, rank, world, local_rank):
                 total = total + loss
                 grads.append(dL)
             torch.autograd.backward([o["render"] for o in outs], grads)
+            del outs, grads   # images and loss gradients of this sub-batch: 5.1 GB per view
         exchange()
         zero_grads()
         loss_host.copy_(total.reshape(1), non_blocking=False)                  # D2H 8 B: the step's loss
@@ -1052,8 +1069,7 @@ def run_k4(args, rank, world, local_rank):
                   "hbm_gbs_effective": batch_bytes / (ms_nc / steps * 1e-3) * 1e-9,
                   "hbm_frac_effective": batch_bytes / (ms_nc / steps * 1e-3) * 1e-9 / peak},
         "roofline": roofline_block(per_stage, ab, ("blend_fwd", "blend_bwd", "dfeature", "alpha_pass"),
-                                   binfo["source_sha256_16"], "C=512 blend: fp32-FMA bound by design; see fma_roofline",
-                                   config="K4"),
+                                   "C=512 blend: fp32-FMA bound by design; see fma_roofline"),
         "fma_roofline": fma_roofline(C, stats["blended_pairs"], per_stage),
         "batched_vs_loop": {"batched_ms_per_step_no_exchange": ms_nc / steps,
                             "per_view_loop_ms_per_step_no_exchange": ms_loop / nloop,
@@ -1170,7 +1186,7 @@ def run_k5(args, rank, world, local_rank):
     peak, peak_src = measured_peaks()
     binfo = build_info()
     nv_mean = float(np.mean(nvis)) if nvis else 0.0
-    # SURVEY.md §8(d): xyz + depth in, one C-vector gathered per visible Gaussian, fp32 accumulator read-modify-write
+    # xyz + depth in, one C-vector gathered per visible Gaussian, fp32 accumulator read-modify-write
     per_view = 12 * P + 4 * w * hh + nv_mean * C * 2 + nv_mean * C * 8 + nv_mean * 8
     kernel_view_ms = sum(v for k, v in per_stage.items() if k.startswith("fusion"))
     achieved = per_view / (kernel_view_ms * 1e-3) * 1e-9 if kernel_view_ms else float("nan")
@@ -1187,9 +1203,6 @@ def run_k5(args, rank, world, local_rank):
         "bytes": {"per_view_algorithmic": per_view, "final_normalise": 8 * P * C},
         "roofline": {"bound": "hbm", "kernel": "fusion view (project + sort + gather/accumulate kernels)", "achieved": achieved,
                      "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic_for("K5.fusion_gather", binfo["source_sha256_16"])[0],
-                     "traffic_source": "gather/accumulate kernel alone (the dominant launch of the view), " +
-                                       str(traffic_for("K5.fusion_gather", binfo["source_sha256_16"])[1]),
                      "algorithmic_bytes": per_view, "kernel_ms": kernel_view_ms, "peak_source": peak_src},
         "exchange": {"bytes": 4 * P * C + 4 * P, "ms_per_step_without_exchange_and_normalise": ms_nc / steps,
                      "exposed_ms_per_step": (ms_dev - ms_nc) / steps},
@@ -1221,7 +1234,13 @@ def main():
     ap.add_argument("--config", default="K3", choices=sorted(CONFIGS))
     ap.add_argument("--no-baselines", action="store_true", help="skip the reference-CUDA and CPU legs")
     ap.add_argument("--quick", action="store_true", help="skip the per-view cost spread")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="K3: write the outputs of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != "K3" or args.impl != "ours"):
+        ap.error("--dump-outputs is implemented for --config K3 --impl ours")
+    if args.steps is not None and args.steps < 1:
+        ap.error("--steps must be at least 1")
     claim_stdout()
     if args.steps is None:
         args.steps = {"K2": 40, "K3": 20, "K4": 3, "K5": 3}[args.config] if args.impl == "ours" else 2

@@ -1,5 +1,5 @@
 /*
- * sgb200 — B200-native Gaussian-splatting rasterizer + 2D->3D fusion kernels: C ABI.
+ * sgb200 — H100 (sm_90a) Gaussian-splatting rasterizer + 2D->3D fusion kernels: C ABI.
  *
  * This is the drop-in boundary for the reference's native rasterizer library.  Each entry
  * point names the reference interface it replaces (paths relative to
@@ -84,7 +84,7 @@ typedef struct sgb_view_grads {
     float* dL_dmeans2D;   /* [P,3]   .xy in the reference's units (backward.cu:455-456,540-541) */
     float* dL_dconic;     /* [P,4]   (x, y, _, w) as backward.cu:544-546 */
     float* dL_dopacity;   /* [P] */
-    float* dL_dcolors;    /* [P,C]   any C (the reference ships C==3 only, SURVEY 2d-1) */
+    float* dL_dcolors;    /* [P,C]   any C (the reference ships C==3 only) */
     float* dL_dmeans3D;   /* [P,3] */
     float* dL_dcov3D;     /* [P,6] */
     float* dL_dsh;        /* [P,M,3] or NULL when shs is NULL */
@@ -151,7 +151,7 @@ int sgb_backward(sgb_ctx* ctx, const sgb_view_inputs* in, int64_t num_rendered,
                  const void* image_state, const float* dL_dpix /* [C,H,W] */,
                  const sgb_view_grads* grads, void* stream);
 
-/* ---- batched views (SURVEY.md §8 row n2 / BASELINE config K4): V views of the SAME Gaussians in one call.
+/* ---- batched views (BASELINE config K4): V views of the SAME Gaussians in one call.
  *
  * The reference renders one view per call in a Python loop (eval_segmentation.py:146-157, fusion.py:58-64,106-144);
  * a view-sharded training / evaluation step renders a batch of views per GPU (K4: 32 views over 8 GPUs = 4 each).
@@ -248,7 +248,7 @@ int sgb_fusion_accumulate(sgb_ctx* ctx, const sgb_fusion_view* v, const void* fe
 /* fusion.py:146-147: count[count==0] = 1e-5; feat_sum /= count (in place). */
 int sgb_fusion_normalize(int32_t P, int32_t C, float* feat_sum, float* count, void* stream);
 
-/* ---- semantic head (SURVEY.md §8 row n1): what every render_chn caller runs on the rendered feature image.
+/* ---- semantic head: what every render_chn caller runs on the rendered feature image.
  *
  * sgb_semantic_head: render (C, N) planar fp32 with N = H*W, text (K, C) row-major:
  *     sim[k][p]  = sum_c text[k][c] * render[c][p] / (||render[:, p]||_2 + 1e-8)   eval_segmentation.py:155-156
@@ -277,7 +277,7 @@ int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const floa
                        float* out, void* stream);
 int sgb_label_argmax(int32_t K, int32_t first_class, int64_t N, const float* planes, int64_t* label, void* stream);
 
-/* ---- 3-nearest-neighbour mean squared distance (SURVEY.md §8 row n4): `distCUDA2` of the reference's
+/* ---- 3-nearest-neighbour mean squared distance: `distCUDA2` of the reference's
  * simple-knn extension (submodules/simple-knn/simple_knn.cu:185-220, spatial.cu), used by
  * GaussianModel.create_from_pcd (model/gaussian_model.py:150-186).  points (P,3) fp32 device, mean_dist2 (P) fp32
  * device: (d1+d2+d3)/3 of the three smallest squared distances to OTHER points (exact, bit-identical to the

@@ -81,7 +81,7 @@ def load() -> C.CDLL:
             return _lib
         if not os.path.exists(LIB_PATH):
             raise ImportError(
-                f"{LIB_PATH} not found: the sm_100a CUDA library is the rasterizer; build it with "
+                f"{LIB_PATH} not found: the sm_90a CUDA library is the rasterizer; build it with "
                 "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)")
         lib = C.CDLL(LIB_PATH)
         vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64

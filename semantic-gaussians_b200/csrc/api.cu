@@ -72,7 +72,7 @@ using namespace sgb;
 extern "C" {
 
 const char* sgb_last_error(void) { return g_err; }
-const char* sgb_version(void) { return "sgb200 0.2.0 (sm_100a)"; }
+const char* sgb_version(void) { return "sgb200 0.2.0 (sm_90a)"; }
 #ifndef SGB_BUILD_ID
 #define SGB_BUILD_ID "unknown"
 #endif

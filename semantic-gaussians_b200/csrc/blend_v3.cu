@@ -14,7 +14,7 @@
 //                     pixel skips it) appended to a per-tile linked list of 16-entry chunks.
 //   blend_forward_v3  CTA = (tile, 64-channel chunk), barrier-free: each warp streams the tile's
 //                     weight rows and feature slices straight from L2 and accumulates an
-//                     8 px x 8 ch register micro-tile per lane (outer product, packed FMA).
+//                     8 px x 8 ch register micro-tile per lane (outer product, paired FMAs).
 //   chain_backward_v3 CTA = tile: s = <feature, dL/dout> per (pixel, Gaussian) for all channels
 //                     (register micro-tiles + transposed shuffle reduce), then the reference's
 //                     back-to-front chain (backward.cu:477-550) in dot-product form -> dL/dmean2D,
@@ -37,12 +37,12 @@ namespace {
 
 constexpr int kThreads = SGB_TILE_PIX;
 
-// Lane -> operand-group mapping of the register-tiled GEMM loops (round 2, measured with tools/lds_probe.cu under ncu
-// on B200): a warp-wide LDS.128 costs 2 shared-memory wavefronts when every aligned group of 4 lanes reads at most 2
-// distinct 16-byte chunks and each half-warp at most 8 (conflict-free) chunks, and 4 wavefronts otherwise.  With the
-// natural split (one operand indexed by lane & 7, the other by lane >> 3) the lane & 7 operand pays 4 per load and the
-// L1 data pipe — not the FMA pipe — bounded all three contraction kernels (ncu r02: 68 / 74 / 83 % of peak).  Giving
-// each operand exactly one of the two low lane bits makes every operand load a 2-wavefront load.
+// Lane -> operand-group mapping of the register-tiled GEMM loops: a warp-wide LDS.128 costs 2 shared-memory
+// wavefronts when every aligned group of 4 lanes reads at most 2 distinct 16-byte chunks and each half-warp at most 8
+// (conflict-free) chunks, and 4 wavefronts otherwise.  With the natural split (one operand indexed by lane & 7, the
+// other by lane >> 3) the lane & 7 operand pays 4 per load, and the shared-memory pipe rather than the FMA pipe limits
+// the contraction kernels.  Giving each operand exactly one of the two low lane bits makes every operand load a
+// 2-wavefront load.
 __device__ __forceinline__ int lane_group8(int lane) { return (lane & 1) | (((lane >> 2) & 3) << 1); }  // bits 0, 2, 3
 __device__ __forceinline__ int lane_group4(int lane) { return ((lane >> 1) & 1) | ((lane >> 4) << 1); } // bits 1, 4
 
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(kThreads) alpha_pass_kernel(
 // before the accumulation).  A pair is blended exactly when its weight alpha * T is non-zero (alpha >= 1/255 and
 // T >= 1e-4 on that path), so the exact semantics are "accumulate only where w != 0".  Guarding every FMA would
 // double the inner loop; instead the epilogue tests the accumulators (acc * 0 summed: NaN iff any accumulator is
-// non-finite, 32 packed FMAs per lane) and only a warp that sees a non-finite value recomputes its 32 px x CH
+// non-finite, 32 paired FMAs per lane) and only a warp that sees a non-finite value recomputes its 32 px x CH
 // slice with the guarded loop below, straight from the weight rows and feature rows in global memory.
 template <int MCH>
 __device__ __forceinline__ bool acc_nonfinite(const float2 (&acc)[8][MCH / 2]) {
@@ -419,17 +419,16 @@ constexpr int kSeg = 64;  // entries per backward segment (4 chunks); S[8 warps]
 //     s-pass    S[256 px][G]        = dL[256 px][C]   . F^T[C][G]        K = C      lane tile 8 px x 8 entries
 //     dfeature  dF[G][64 ch]        = W[G][256 px]    . dL[256 px][64]   K = 256 px lane tile 4 entries x 8 ch
 // Register tiles make every product 64-128 FMAs per 4-6 shared-memory loads and need no cross-lane
-// reductions (an earlier shuffle-reduce formulation spent ~40 % of its issue slots on SHFL/FSEL/FADD).
-// Forward GEMM with a TMA-fed ring.  With plain loads of the weight rows 67 % of the instructions were
-// packed FMAs but only 28 % of the issue slots were used — every warp waited an L2/DRAM round trip per
-// entry (ncu long_scoreboard 9.2 stalls per issue).  Here one ring stage = one 16-entry chunk: per staged
+// reductions (a shuffle-reduce formulation spends its issue slots on SHFL/FSEL/FADD instead).
+// Forward GEMM with a TMA-fed ring.  With plain loads of the weight rows every warp waits an L2/DRAM round
+// trip per entry.  Here one ring stage = one 16-entry chunk: per staged
 // Gaussian two 1-D bulk copies (cp.async.bulk: the 1 KB weight row and the 256 B feature slice), NS stages
 // guarded by full/empty mbarriers.  Warp 0 is producer AND consumer, so nothing it does for production may
 // block its math: the chunk indices come from the tile's directory (copied to shared memory up front, no
 // pointer chasing), the (id, mask) records of the NEXT batch are fetched into registers one whole batch of
 // math before they are needed, and the stage it refills is the one everybody left TWO batches ago, so the
-// empty-barrier wait is already satisfied (refilling the stage of the previous batch coupled warp 0 to
-// the slowest warp on every batch: ncu showed the FMA pipe 50 % idle with long-scoreboard stalls on top).
+// empty-barrier wait is already satisfied (refilling the stage of the previous batch would couple warp 0 to
+// the slowest warp on every batch).
 template <int CH, int NS>
 __global__ void __launch_bounds__(kThreads, 2) blend_forward_tma_kernel(
     int W, int H, int C, const float* __restrict__ features, const float* __restrict__ bg_color,
@@ -552,8 +551,8 @@ __global__ void __launch_bounds__(kThreads, 2) blend_forward_tma_kernel(
             meta_next = load_meta(pb);  // lands while this batch is being consumed
         }
         mbar_wait(&full_bar[st], (uint32_t)((b / NS) & 1));
-        // dense on purpose: skipping strips whose 32 weights are all zero (about 15 % of the entries)
-        // breaks the unrolled load/FMA software pipeline and measured 10 % slower on K3
+        // dense on purpose: skipping strips whose 32 weights are all zero breaks the unrolled load/FMA
+        // software pipeline
         if (cnt == ES) {
 #pragma unroll
             for (int e = 0; e < ES; e++) entry(stg[st], e);
@@ -602,10 +601,10 @@ __global__ void __launch_bounds__(kThreads, 2) blend_forward_tma_kernel(
 // [channel][pixel] order by cp.async row pieces (no transposing stores); warp w owns entries
 // 16w..16w+15 of each 128-entry pass and streams their weight rows through a private double-buffered
 // slab [16][32 px].  Lane = (eg, cg) accumulates entries {eg + 4j} x channels {4cg..4cg+3} U {32+4cg..32+4cg+3}; one K
-// step covers 4 pixels with LDS.128 of both operands, and the packed FMAs pair (even, odd) pixels — no register
+// step covers 4 pixels with LDS.128 of both operands, and the paired FMAs take (even, odd) pixels — no register
 // duplication, the two halves are added at the end.
-// Round 2 (ncu + tools/lds_probe.cu): the kernel was bound by the LSU, not the FMA pipe — 32 scalar red.global per
-// lane and pass (~30-40 LSU cycles each) on top of 4-wavefront operand loads.  Now
+// The load/store unit, not the FMA pipe, limits this kernel when every lane issues 32 scalar red.global per pass on
+// top of 4-wavefront operand loads.  Therefore
 //   * a lane owns two blocks of 4 CONSECUTIVE channels, so a Gaussian's sums leave as two red.global.add.v4.f32
 //     (8 reductions per lane and pass instead of 32);
 //   * the 16-byte pixel quads of channel row r sit at quad ^ ((r >> 2) & 7): the 8 channel groups of one load then hit 8
@@ -689,8 +688,8 @@ __global__ void __launch_bounds__(kThreads, 2) dfeature_gemm_kernel(int W, int H
                 else cp_async_wait<0>();
                 __syncwarp();
                 // Fully unrolled and software-pipelined by hand: ptxas otherwise issues every LDS right in
-                // front of its first consumer (ncu: half of all stall samples were short-scoreboard waits on
-                // those FFMA2s).  dL rows are fetched two K-steps ahead, the next pixel quad's weights while
+                // front of its first consumer, and the FMAs wait on short-scoreboard stalls.  dL rows are
+                // fetched two K-steps ahead, the next pixel quad's weights while
                 // the current quad is being consumed.
                 const float* drow = &dLs[4 * cg][0];
                 const float* wbase = &wsl[buf][eg][0];
@@ -794,8 +793,7 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_gemm_kernel(
     const int woff = warp * 32 + lane;
 
     // background term of the own pixel over all channels (backward.cu:527-529).  With an all-zero background
-    // (the usual case) the term vanishes; skipping it saves a second full read of dL/dout (ncu: 4.6 GB read
-    // by this kernel against 2.1 GB of dL/dout).
+    // (the usual case) the term vanishes; skipping it saves a second full read of dL/dout.
     int bg_nonzero = 0;
     for (int ch = tid; ch < C; ch += kThreads) bg_nonzero |= (bg_color[ch] != 0.f);
     bg_nonzero = __syncthreads_or(bg_nonzero);
@@ -987,22 +985,20 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_gemm_kernel(
 }
 
 // ------------------------------------------------------------------------------------ warp-autonomous chain backward
-// Second generation of the chain backward (round 2).  ncu on the CTA-synchronous kernel above (K3): FMA pipe 50 %,
-// issue 49 %, 16 warps/SM; executed FMAs = 2.0 x the algorithmic ones — every warp multiplied all 64 slots of every
-// segment of the TILE list although its 32-pixel strip is touched by ~85 % of the tile's entries, and segments of 64
-// padded the list by another ~22 %; one CTA-wide barrier per 16-channel slab.  Here every warp owns its strip end to
-// end and nothing is CTA-synchronous after the prologue:
+// Second generation of the chain backward.  In the CTA-synchronous kernel above every warp multiplies all 64 slots of
+// every segment of the TILE list although its 32-pixel strip is touched by only part of the tile's entries, segments
+// of 64 pad the list further, and there is one CTA-wide barrier per 16-channel slab.  Here every warp owns its strip
+// end to end and nothing is CTA-synchronous after the prologue:
 //   * the warp walks the tile list from the back and COMPACTS it on the fly to the entries whose strip-mask bit is
 //     set (ballot + popc ranks), 32 entries per segment: no zero-strip work, padding
 //     <= 31 slots per strip instead of <= 63 per tile;
-//   * s-pass per segment: S[32 px][32 entries] over all channels, lane tile 8 px x 4 entries (16 packed FMAs per 3
+//   * s-pass per segment: S[32 px][32 entries] over all channels, lane tile 8 px x 4 entries (16 paired FMAs per 3
 //     LDS.128); the warp stages its own operands — the dL/dout slab [16 ch][32 px] by cp.async, the feature slab by
 //     4 x LDG.128 per lane (lane = entry) one slab ahead in registers, stored transposed [ch][entry];
 //   * S is parked in the warp's dL slab region (XOR-swizzled 16-byte chunks: conflict-free both ways) and lane = pixel
 //     runs the reference's back-to-front chain (backward.cu:477-550, dot-product form) over the 32 entries.
-// Shared memory 9.3 KB per warp, 128 registers, 2 CTAs/SM (a 80-register / 3-CTA build measured 13 % SLOWER on K3:
-// 5.22 vs 4.62 ms — the extra warps thrash the 28 KB of L1 that three CTAs leave for the gathered rows); the warps of
-// a tile share their feature rows through L1/L2 only.
+// Shared memory 9.3 KB per warp, 128 registers, 2 CTAs/SM (a third CTA would leave less L1 for the gathered feature
+// rows); the warps of a tile share their feature rows through L1/L2 only.
 constexpr int kChainRG = 5;  // entries whose six gradient terms are summed over the strip per flush (30 of 32 lanes busy)
 struct __align__(16) ChainWarpSmem {
     float DS[2][16][32];   // dL/dout slabs [buf][ch][px of the strip]; S[32 entries][32 px] aliases it after the s-pass
@@ -1177,8 +1173,7 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
         for (int i = 0; i < 8; i++) acc[i][0] = acc[i][1] = make_float2(0.f, 0.f);
         // Feature slab [32 entries][16 ch] -> FT[ch][entry].  Fast path (16-byte aligned rows, full slab): lane
         // (r8 = lane >> 2, c4 = lane & 3) loads channels 4c4..4c4+3 of entries r8 + 8q, so one LDG.128 covers 8 rows x
-        // 64 contiguous bytes (8 L1 tag lookups; lane = entry touched ~27 lines per instruction and the feature gather
-        // alone was a third of the kernel's L1 wavefronts, ncu r02).  FT rows of channels 8..15 hold their 8-entry
+        // 64 contiguous bytes (8 L1 tag lookups, where lane = entry would touch a separate line per lane).  FT rows of channels 8..15 hold their 8-entry
         // blocks swapped pairwise (block b at b ^ 1) — with the 36-float pitch that makes the transposing stores of
         // this mapping conflict-free; the s-pass reads entry group eg of channel k at chunk eg ^ ((k >> 3) << 1).
         float4 fpre[CK / 4];
@@ -1285,8 +1280,8 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
 
         // ---- back-to-front chain over the segment (backward.cu:477-550 in dot-product form); slot 0 is the
         // furthest-back entry.  Entries go in groups of kChainRG, fully unrolled (every shared-memory address of the
-        // group is a constant plus a lane term — ncu r02: 40 of ~170 instructions per entry were address arithmetic
-        // of the runtime-indexed version); the own-pixel weights of the next group are in flight during the current
+        // group is a constant plus a lane term, where a runtime-indexed loop spends instructions on address
+        // arithmetic); the own-pixel weights of the next group are in flight during the current
         // one.  The six per-Gaussian sums over the strip's 32 pixels go through shared memory instead of a shuffle
         // butterfly: every lane parks its terms as rows of RB, then lane r adds up row r with 8 x LDS.128 and issues
         // that row's one red.global.  16-byte chunk c of row r sits at c ^ (r & 7): conflict-free both ways.
@@ -1365,12 +1360,11 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
 }
 
 // ------------------------------------------------------------------------------------ warp-autonomous forward
-// Forward counterpart of chain_backward_warp_kernel (round 2).  The TMA-ring kernel above multiplies every entry of the
-// TILE list into every strip (ncu r01: 57 % FMA pipe, 13 % of the stalls on the per-CTA prologue, 35 % of the FMAs on
-// zero weights).  Here a warp owns (strip, 32-channel slice): it compacts the tile list to the entries whose
+// Forward counterpart of chain_backward_warp_kernel.  The TMA-ring kernel above multiplies every entry of the TILE
+// list into every strip, including the zero weights of strips an entry does not touch.  Here a warp owns (strip, 32-channel slice): it compacts the tile list to the entries whose
 // strip-mask bit is set, streams for each of them 128 B of weights (its strip only — the ring staged the whole 1 KB
 // row for every 64-channel slice) and 128 B of features through a private cp.async double buffer (8 entries per
-// stage) and accumulates an 8 px x 4 ch register tile per lane (16 packed FMAs per 3 LDS.128).  No CTA barrier after
+// stage) and accumulates an 8 px x 4 ch register tile per lane (16 paired FMAs per 3 LDS.128).  No CTA barrier after
 // the prologue; 64 registers, 4.4 KB of shared memory per warp.  CTA = (tile, SL consecutive slices handled one after
 // the other by every warp).  Accumulation order = list order, like forward.cu:355-356.
 struct __align__(16) FwdWarpSmem {
@@ -1659,8 +1653,8 @@ static int launch_forward_gemm(sgb_ctx* ctx, const sgb_view_inputs& in, ImgView 
     const int chunks = (in.C + 63) / 64;
     const bool vec = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(colors) & 15) == 0);
     if (vec && blend_mma_enabled()) return launch_forward_mma(ctx, in, im, colors, out_color, pv, s);  // opt-in experiment
-    // SGB_FWD_WARP=1 selects the warp-autonomous kernel (per-strip compacted lists; measured SLOWER than the TMA ring on
-    // K3: 2.98 vs 2.56 ms — kept for A/B measurements and for scenes with sparser strips)
+    // SGB_FWD_WARP=1 selects the warp-autonomous kernel (per-strip compacted lists, for A/B comparison and for scenes
+    // with sparser strips)
     static const bool use_warp = [] { const char* e = getenv("SGB_FWD_WARP"); return e && e[0] == '1'; }();
     StageTimer t(ctx, ST_BLEND_FWD, s);
     ctx->launches += 1;

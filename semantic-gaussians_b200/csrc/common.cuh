@@ -120,6 +120,7 @@ struct Profiler {
 
 namespace sgb {
 constexpr int kMaxBatch = 8;  // views per batched call == weight-pool slots kept per ctx
+constexpr int kNumSMs = 132;  // H100 SXM: sizes the grids of the grid-stride kernels
 
 // One weight pool (blend_v3.cu) = the per-tile alpha*T rows of ONE view.  A ctx keeps up to kMaxBatch of them so
 // that the backward of each view of a batch (or of a forward-forward-...-backward-backward sequence) finds the
@@ -265,16 +266,9 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                  "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-// packed fp32 FMA (sm_100+): d.xy = a.xy * b.xy + c.xy, one issue slot for two FMAs.
+// d.xy = a.xy * b.xy + c.xy as two round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rd, ra, rb, rc;\n\t"
-        "mov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y)
-        : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 // auxiliary.h:46-56 (getRect).  max_radius is an int parameter: the float radius is converted at
 // the call.  Used by preprocess and re-derived by the instance emitter exactly like

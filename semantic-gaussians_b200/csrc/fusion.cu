@@ -148,7 +148,7 @@ __device__ __forceinline__ float to_f32(float f) { return f; }
 // feat_sum[g, :] += map[:, pix(g)] for the visible Gaussians, in pixel order.  Work item of a warp = (32 consecutive
 // entries of the pixel-sorted list, one pass of CHP channels); items are handed out grid-stride with the pass index
 // fastest, so a view with few visible Gaussians still spreads over many warps (a first version walked all passes of a
-// batch in one warp: ~0.3 ms of serial latency per view however few Gaussians were visible).  Per item: load phase
+// batch in one warp: serial latency per view however few Gaussians were visible).  Per item: load phase
 // (lane = Gaussian, one element per channel plane, 16 loads in flight) into a private shared-memory tile [32][CHP]
 // (odd word pitch: the per-lane row writes and the per-row reads are both conflict-free), then the accumulate phase
 // adds 16 rows at a time to the fp32 sums, lanes along the channels (128-byte pieces, 32 loads in flight).
@@ -320,9 +320,9 @@ extern "C" int sgb_fusion_accumulate(sgb_ctx* ctx, const sgb_fusion_view* v, con
     }
     {
         StageTimer t(ctx, ST_FUSION_GATHER, s);
-        const int gblocks = 148 * 3;  // 3 CTAs/SM by shared memory (66 KB each); items are handed out grid-stride
+        const int gblocks = kNumSMs * 3;  // 3 CTAs/SM by shared memory (66 KB each); items are handed out grid-stride
         if (feat_dtype == SGB_FEAT_F16) {
-            constexpr int CHP = 128;  // (64-channel passes with twice the resident warps measured slower: 0.98 vs 0.81 ms/view)
+            constexpr int CHP = 128;  // channels per pass
             const size_t smem = 8 * 32 * (CHP + 2) * sizeof(__half);
             static DeviceOnce once;
             if (once.first_use_on_device())
@@ -350,7 +350,7 @@ extern "C" int sgb_fusion_normalize(int32_t P, int32_t C, float* feat_sum, float
     cudaStream_t s = (cudaStream_t)stream;
     if (P < 0 || C <= 0 || !feat_sum || !count) { set_error("sgb_fusion_normalize: bad arguments"); return SGB_E_INVALID; }
     if (P == 0) return SGB_OK;
-    fusion_normalize_kernel<<<148 * 8, 256, 0, s>>>(P, C, feat_sum, count);
+    fusion_normalize_kernel<<<kNumSMs * 8, 256, 0, s>>>(P, C, feat_sum, count);
     fusion_fix_count_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, count);
     SGB_LAUNCH_CHECK("fusion_normalize_kernel", 0, s);
     return SGB_OK;

@@ -1,4 +1,4 @@
-// Mean squared distance to the 3 nearest neighbours of every point (SURVEY.md §8 row n4): the contract of
+// Mean squared distance to the 3 nearest neighbours of every point: the contract of
 // the reference's `distCUDA2` (submodules/simple-knn/simple_knn.cu:185-220, called from
 // model/gaussian_model.py:150-186 create_from_pcd to initialise the Gaussian scales).
 //
@@ -266,7 +266,7 @@ extern "C" int sgb_knn_mean_dist2(sgb_ctx* ctx, int32_t P, const float* points, 
     void* cub_tmp = (char*)boxes + align_up(sizeof(Aabb) * (size_t)nboxes);
 
     knn_bounds_init_kernel<<<1, 32, 0, s>>>(mm);
-    knn_bounds_kernel<<<min((P + 255) / 256, 148 * 8), 256, 0, s>>>(P, points, mm);
+    knn_bounds_kernel<<<min((P + 255) / 256, kNumSMs * 8), 256, 0, s>>>(P, points, mm);
     knn_morton_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, points, mm, codes, ids);
     SGB_LAUNCH_CHECK("knn_morton_kernel", 0, s);
     SGB_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp, codes, codes_s, ids, ids_s, P, 0, 30, s));

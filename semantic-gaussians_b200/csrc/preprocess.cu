@@ -24,9 +24,11 @@ __device__ void computeCov3D(const float3 scale, float mod, const float4 rot, fl
     S.m[1][1] = mod * scale.y;
     S.m[2][2] = mod * scale.z;
     float r = rot.x, x = rot.y, y = rot.z, z = rot.w;
-    M3 R = cols(1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y),
+    // r * y + x * z and r * x + y * z: the operand order the reference's GLM code reaches in PTX.  The sum is the
+    // same either way, but ptxas fuses one of the two products into an FFMA, and on sm_90 it picks by operand order.
+    M3 R = cols(1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (r * y + x * z),
                 2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x),
-                2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y));
+                2.f * (x * z - r * y), 2.f * (r * x + y * z), 1.f - 2.f * (x * x + y * y));
     M3 M = S * R;
     M3 Sigma = transpose(M) * M;
     cov3D[0] = Sigma.m[0][0];

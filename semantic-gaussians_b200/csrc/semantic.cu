@@ -1,5 +1,5 @@
 // Open-vocabulary semantic head that every render_chn caller of the reference runs right after the
-// rasterizer (SURVEY.md §8 row n1):
+// rasterizer:
 //
 //   rendering = rendering / (rendering.norm(dim=0, keepdim=True) + 1e-8)      eval_segmentation.py:155,255,396
 //   sim       = torch.einsum("cq,qhw->chw", text_features, rendering)         eval_segmentation.py:156,256,397
@@ -132,12 +132,12 @@ __global__ void __launch_bounds__(kHeadThreads) semantic_head_kernel(
 }
 
 // Same head, fed by TMA.  The register-file version above keeps only ~4 x 16 B of loads in flight per
-// thread at 8 warps/SM (146 registers) and measured 1.8 TB/s on the K3 image; here the channel planes of a
+// thread at 8 warps/SM (146 registers); here the channel planes of a
 // 1024-pixel block stream through a ring of kHNS stages x kHCS channels x 4 KB filled by 1-D bulk copies
 // (cp.async.bulk + mbarrier complete_tx), ~96 KB in flight per SM, and the math never waits on a global
 // load.  Full stages run a branch-free fully unrolled 8-channel body (the per-channel tail test and the
-// per-stage barrier bookkeeping were 35 % of the instructions with 4-channel stages).  512 threads x 2 pixels: half the accumulators per thread of the 4-pixel layout, so 16 warps per SM
-// fit the register file (the 8-warp variant ran the FMA pipe at ~45 %).
+// per-stage barrier bookkeeping cost a large share of the instructions with 4-channel stages).  512 threads x 2
+// pixels: half the accumulators per thread of the 4-pixel layout, so 16 warps per SM fit the register file.
 // Requires the VEC conditions (N % 4 == 0, 16-byte aligned planes) and the transposed class embeddings of
 // one pass to fit next to the ring.
 constexpr int kHCS = 8;   // channels per stage
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) semantic_head_tma_kernel(
 // 16-byte loads (a row's 128-byte lines stay in L1 between iterations, so DRAM sees every line once); the
 // class embeddings sit transposed [C][KC] in shared memory and are read as broadcast LDS.128, 2 x KC register
 // accumulators, no cross-lane reduction.  (The first version — warp per row, butterfly reduction of every
-// class — spent most of its issue slots on SHFL/FADD and ran at 0.85 TB/s.)
+// class — spends most of its issue slots on SHFL/FADD.)
 template <int NK4>
 __global__ void __launch_bounds__(256) feature_logits_kernel(int P, int C, int K, int Kpad, int k0,
                                                              const float* __restrict__ features,
@@ -497,7 +497,7 @@ static int launch_logits_t(int P, int C, int K, int Kpad, int k0, const float* f
     if (attr_set.first_use_on_device()) {
         SGB_CUDA(cudaFuncSetAttribute(feature_logits_kernel<NK4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
-    const int blocks = min((P + 511) / 512, 148 * 8);
+    const int blocks = min((P + 511) / 512, kNumSMs * 8);
     feature_logits_kernel<NK4><<<blocks, 256, smem, s>>>(P, C, K, Kpad, k0, features, text, out);
     SGB_LAUNCH_CHECK("feature_logits_kernel", 0, s);
     return SGB_OK;
@@ -540,9 +540,9 @@ int sgb_distill_loss(int32_t C, int32_t K, int64_t N, const float* render, const
     const size_t smem = sizeof(float) * (size_t)C * ((K + 1) | 1);
     if (smem > 200 * 1024) { set_error("sgb_distill_loss: C x K = %d x %d does not fit shared memory", C, K); return SGB_E_INVALID; }
     if (labels_are_int64)
-        count_valid_labels_kernel<long long><<<148 * 4, 256, 0, s>>>(K, (long long)N, (const long long*)labels, loss + 1);
+        count_valid_labels_kernel<long long><<<kNumSMs * 4, 256, 0, s>>>(K, (long long)N, (const long long*)labels, loss + 1);
     else
-        count_valid_labels_kernel<int><<<148 * 4, 256, 0, s>>>(K, (long long)N, (const int*)labels, loss + 1);
+        count_valid_labels_kernel<int><<<kNumSMs * 4, 256, 0, s>>>(K, (long long)N, (const int*)labels, loss + 1);
     const bool vec = (N % 4 == 0) && ((reinterpret_cast<uintptr_t>(render) & 15) == 0) &&
                      ((reinterpret_cast<uintptr_t>(dL_drender) & 15) == 0);
     const unsigned blocks = (unsigned)((N + 1023) / 1024);

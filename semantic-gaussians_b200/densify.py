@@ -1,4 +1,4 @@
-"""Adaptive density control and optimiser bookkeeping of the 3DGS training loop (SURVEY.md §8 row n4): what
+"""Adaptive density control and optimiser bookkeeping of the 3DGS training loop: what
 consumes ``viewspace_points.grad`` and ``radii`` produced by the rasterizer (train.py:158-175).
 
 Behavioural contract: model/gaussian_model.py:196-240 (training_setup), :242-248 (update_learning_rate),

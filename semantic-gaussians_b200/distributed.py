@@ -1,6 +1,6 @@
 """View-sharded multi-GPU execution (new in this framework; the reference is single-GPU).
 
-The path shards by view (SURVEY.md §8e): every rank holds a replica of the Gaussian tensors,
+The path shards by view: every rank holds a replica of the Gaussian tensors,
 renders / fuses its own views, accumulates per-Gaussian sums locally in fp32 and then takes part in
 ONE exchange step — a sum all-reduce of the (P, C) gradient or feature-sum tensor plus the small
 geometry gradients / the view counts.  One process per GPU, torch.distributed for the plumbing
@@ -66,10 +66,10 @@ def allreduce_sums(tensors: Sequence[torch.Tensor], group=None, bucket_bytes: in
 
 def nccl_overlap_options():
     """Process-group options for ``dist.init_process_group("nccl", pg_options=...)``: NCCL's stream gets high
-    priority.  The chain-backward kernel fills every SM for ~5 ms in 27 waves; at equal priority the block
+    priority.  The chain-backward kernel fills every SM for many waves; at equal priority the block
     scheduler keeps handing freed SM slots to ITS pending CTAs, so an all-reduce launched meanwhile only
-    starts in the last wave (measured: no overlap at all).  With a high-priority stream the NCCL CTAs are
-    placed as soon as the first chain CTAs retire (~0.2 ms)."""
+    starts in the last wave.  With a high-priority stream the NCCL CTAs are placed as soon as the first
+    chain CTAs retire."""
     opts = dist.ProcessGroupNCCL.Options()
     opts.is_high_priority_stream = True
     max_ctas = int(os.environ.get("SGB_NCCL_MAX_CTAS", "0"))

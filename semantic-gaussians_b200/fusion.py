@@ -166,7 +166,7 @@ def fuse_views(gaussians, views, feature_maps, mapper_kwargs: dict, depths=None,
 
 def fuse_scene(gaussians, views, feature_maps, pipe, background, img_dim, visibility_threshold=0.25,
                cut_boundary=0, depth="render", depth_maps=None, every: int = 5) -> dict:
-    """fuse_one_scene (fusion.py:57-148) with every step on the device (SURVEY.md §8 row n2).
+    """fuse_one_scene (fusion.py:57-148) with every step on the device.
 
     The reference renders the depth map on the GPU, copies it to the host, projects all Gaussians in numpy,
     gathers the (C,h,w) feature map on the CPU and copies a (P,C) tensor back — per view (fusion.py:106-144).

@@ -1,4 +1,4 @@
-"""On-disk formats either side of the render / fusion path (SURVEY.md §8 row n3), without ``plyfile``:
+"""On-disk formats either side of the render / fusion path, without ``plyfile``:
 
 * Gaussian PLY — the 3DGS vertex layout the reference writes and reads with plyfile
   (model/gaussian_model.py:250-281 save_ply, :288-344 load_ply): binary little-endian, one ``vertex`` element,

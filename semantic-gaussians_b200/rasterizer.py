@@ -444,7 +444,7 @@ def make_module(variant: str):
                                          cov3Ds_precomp, raster_settings)
 
     class _RasterizeGaussiansBatch(torch.autograd.Function):
-        """V views of the same Gaussians in one native call each way (SURVEY.md §8 n2; the reference loops over
+        """V views of the same Gaussians in one native call each way (the reference loops over
         single-view calls in Python, eval_segmentation.py:146-157).  Outputs per view are those of
         _RasterizeGaussians; the backward sums the per-Gaussian gradients over the views, the (P, C) feature
         gradient in place inside the kernels."""

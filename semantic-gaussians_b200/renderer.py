@@ -1,5 +1,5 @@
 """render() / render_chn(): the reference's Render API (model/renderer.py:20-130 and :134-246) over
-the B200 rasterizer.  Signatures, argument semantics and returned dict keys are the reference's;
+the H100 rasterizer.  Signatures, argument semantics and returned dict keys are the reference's;
 ``pc`` is any object with the GaussianModel getters the reference reads (get_xyz, get_opacity,
 get_scaling, get_rotation, get_features, get_covariance[_rotation], active_sh_degree,
 max_sh_degree) and ``pipe`` any object with convert_shs_python / compute_cov3d_python / debug.

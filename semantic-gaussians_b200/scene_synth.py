@@ -1,6 +1,6 @@
 """Synthetic scenes and cameras for tests, golden fixtures and bench (numpy only).
 
-The reference ships no generator; distributions follow SURVEY.md §8(d).  Camera matrices
+The reference ships no generator; its distributions are the blob and room scenes below.  Camera matrices
 follow the reference's conventions exactly:
 
 * ``world_view_transform`` = W2C transposed            (scene/camera.py:87)
@@ -147,7 +147,7 @@ class SynthScene:
 
 def make_scene(P: int, seed: int = 0, kind: str = "blob", sh: bool = False, channels: int = 0,
                scale_mean: float = 0.02) -> SynthScene:
-    """SURVEY.md §8(d): blob U([-1.3,1.3]^3) (model/gaussian_model.py:158) or room
+    """blob U([-1.3,1.3]^3) (model/gaussian_model.py:158) or room
     U([-4,4]x[-4,4]x[-1.5,1.5]); log-normal scales; random unit quaternions; sigmoid(N(0,2^2))
     opacity; SH dc U(-1.5,1.5) rest N(0,0.1^2); L2-normalised N(0,1) feature rows."""
     rng = np.random.default_rng(seed)

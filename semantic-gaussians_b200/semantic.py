@@ -1,4 +1,4 @@
-"""Open-vocabulary semantic head on the GPU (SURVEY.md §8 row n1): what every ``render_chn`` caller of
+"""Open-vocabulary semantic head on the GPU: what every ``render_chn`` caller of
 the reference does with the rendered feature image (eval_segmentation.py:153-157, 253-257, 394-398;
 view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:132, view_viser.py:185).
 

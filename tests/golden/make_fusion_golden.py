@@ -5,7 +5,9 @@ statements of fusion.py:136-147 on seeded synthetic inputs.  Run in the build co
 
     python tests/golden/make_fusion_golden.py
 
-Inputs are regenerated from the seed by the tests; only outputs are stored."""
+Inputs are regenerated from the seed by the tests; only outputs are stored: the mappings as int16, the fused fp32
+features as the SHA-256 of their bytes (the tests compare them bit for bit).  A second, smaller case (seed 7, two
+views, three depth modes) pins the numpy oracle at other parameters ("other_*" keys)."""
 import collections
 import collections.abc
 import os
@@ -13,6 +15,9 @@ import sys
 import types
 
 import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from make_raster_golden import digest  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
@@ -49,6 +54,10 @@ def fusion_inputs(seed=0, P=20000, w=160, h=120, C=16, nviews=3):
     return scene, cams, feats, depths
 
 
+def other_seed_inputs():
+    return fusion_inputs(seed=7, P=5000, w=96, h=64, C=4, nviews=2)
+
+
 def main():
     import torch
     Mapper = import_reference_mapper()
@@ -65,7 +74,7 @@ def main():
             depth = depths[i] if dsel == "per-view" else dsel
             mapping = np.ones([P, 4], dtype=int)
             mapping[:, 1:4], weight = mapper.compute_mapping(cam.world_view_transform, scene.xyz, depth)
-            out[f"{mode}_mapping_{i}"] = mapping[:, 1:4].astype(np.int64)
+            out[f"{mode}_mapping_{i}"] = mapping[:, 1:4].astype(np.int16)
             if mapping[:, 3].sum() == 0:
                 continue
             mp = torch.from_numpy(mapping)
@@ -77,8 +86,13 @@ def main():
             feat_sum[mask_k] += fm[mask_k]                            # fusion.py:144
         times[times == 0] = 1e-5                                      # fusion.py:146
         feat_sum /= times                                             # fusion.py:147
-        out[f"{mode}_fused"] = feat_sum.numpy()
+        out[f"{mode}_fused.sha256"] = digest(feat_sum.numpy())
         out[f"{mode}_times"] = times.numpy()
+    scene, cams, feats, depths = other_seed_inputs()
+    for i, cam in enumerate(cams):
+        for j, depth in enumerate((None, "surface", depths[i])):
+            want, _ = Mapper([96, 64], 0.1, 2, cam.intrinsics()).compute_mapping(cam.world_view_transform, scene.xyz, depth)
+            out[f"other_mapping_{i}_{j}"] = np.asarray(want).astype(np.int16)
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "fusion_golden.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, {k: v.shape for k, v in out.items()})

@@ -24,18 +24,18 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/sgb200.h but not exported"
     assert set(_lib.EXPORTS) <= set(names)
-    assert b"sm_100a" in lib.sgb_version()
+    assert b"sm_90a" in lib.sgb_version()
 
 
-def test_library_contains_sm100a_code_with_tma_and_packed_fma():
+def test_library_contains_sm90a_code_with_tma_and_wgmma():
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass
     assert "UBLKCP" in sass          # cp.async.bulk (TMA engine) staging of the per-tile Gaussian blocks
-    assert "FFMA2" in sass           # packed fp32 FMA in the C-channel blend
+    assert "HGMMA" in sass           # wgmma of the opt-in tensor-core contractions (blend_mma.cu)
 
 
 def test_state_sizes_are_sane():

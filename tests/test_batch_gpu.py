@@ -1,4 +1,4 @@
-"""Batched multi-view path (SURVEY.md §8 n2 / BASELINE config K4): render_chn_batch / render_batch over
+"""Batched multi-view path (BASELINE config K4): render_chn_batch / render_batch over
 sgb_forward_geometry_batch / sgb_forward_render_batch / sgb_backward_batch must give, per view, exactly what the
 single-view calls give, and gradients equal to the sum over the views (fp32 re-association only: the (P, C)
 feature gradient is accumulated in place across the views by red.add)."""

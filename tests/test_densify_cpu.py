@@ -1,4 +1,4 @@
-"""CPU: adaptive density control + optimiser bookkeeping (SURVEY §8 n4; model/gaussian_model.py:196-248, 420-612)."""
+"""CPU: adaptive density control + optimiser bookkeeping (model/gaussian_model.py:196-248, 420-612)."""
 import math
 import os
 import sys

@@ -1,4 +1,4 @@
-"""CPU: on-disk formats (SURVEY.md §8 n3) — Gaussian PLY in the reference's vertex layout, fused-feature .pt."""
+"""CPU: on-disk formats — Gaussian PLY in the reference's vertex layout, fused-feature .pt."""
 import os
 import sys
 

@@ -1,5 +1,6 @@
-"""distCUDA2 (SURVEY §8 n4): csrc/knn.cu against the compiled unmodified reference simple-knn (bit-exact) and
-against the numpy brute-force oracle."""
+"""distCUDA2: csrc/knn.cu against the compiled unmodified reference simple-knn (bit-exact, through
+the results it computed for these inputs: tests/golden/ref, util.RefRecord) and against the numpy brute-force
+oracle."""
 import ctypes as C
 import os
 import sys
@@ -10,6 +11,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from util import RefRecord  # noqa: E402
+
 pytestmark = pytest.mark.gpu
 REF = os.path.join(ROOT, "oracle", "_ref", "libref_knn.so")
 
@@ -34,15 +38,16 @@ def _ref(points_dev):
     return out
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="oracle/_ref/libref_knn.so not built")
 @pytest.mark.parametrize("n", [5, 300, 20000, 200001])
 def test_bit_exact_vs_compiled_reference(n):
     from semantic_gaussians_b200.simple_knn._C import distCUDA2
     dev = torch.device("cuda:0")
+    rec = RefRecord(f"knn_{n}")
     for name, pts in _clouds(n, n).items():
         p = torch.from_numpy(pts).to(dev)
-        ours, ref = distCUDA2(p), _ref(p)
-        assert torch.equal(ours, ref), (name, n, float((ours - ref).abs().max()))
+        ours = distCUDA2(p)
+        assert rec.equal(name, ours.view(torch.int32), lambda: _ref(p).view(torch.int32)), (name, n)
+    rec.save()
 
 
 @pytest.mark.parametrize("n", [4, 7, 257, 1500])

@@ -1,4 +1,4 @@
-"""GPU parity of the semantic head (SURVEY.md §8 n1) against the numpy oracle and against the reference's
+"""GPU parity of the semantic head against the numpy oracle and against the reference's
 torch expressions, plus the logit-space label renderer against render_chn + head."""
 import os
 import sys

@@ -2,7 +2,10 @@
 the compiled reference (oracle/_ref) and the CPU oracle on the same seeded scene."""
 from __future__ import annotations
 
+import hashlib
 import math
+import os
+import zlib
 
 import numpy as np
 import torch
@@ -92,6 +95,79 @@ def ours_state(sc, cm, C, *, use_features, want_depth=False, sh_degree=3):
     torch.cuda.synchronize(dev)
     st.update(R=R, color=color, radii=radii, depth=depth)
     return st
+
+
+GOLDEN_REF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref")
+
+
+def _np(t):
+    return t.detach().contiguous().cpu().numpy() if isinstance(t, torch.Tensor) else np.ascontiguousarray(t)
+
+
+class RefRecord:
+    """What one test compares against the compiled reference rasterizer (oracle/_ref), stored in
+    tests/golden/ref/<case>.npz so that the comparison runs where the reference is not built: arrays compared bit
+    for bit as the SHA-256 of their bytes, arrays compared to a tolerance as a fixed seeded sample of their entries
+    plus the whole array's max |x|.  With SGB_RECORD_REF=1 the test runs the reference live, checks against the full
+    arrays and rewrites the record (`SGB_RECORD_REF=1 python -m pytest tests -m gpu` with oracle/_ref built).  `ref`
+    arguments are callables that produce the live reference array; they are only called when recording."""
+    SAMPLE = 16384   # 64 KB per array: a record of seven sampled arrays stays well under 1 MB
+
+    def __init__(self, case):
+        self.path = os.path.join(GOLDEN_REF, case + ".npz")
+        self.live = os.environ.get("SGB_RECORD_REF") == "1"
+        self.data = {} if self.live else dict(np.load(self.path))
+
+    def save(self):
+        if self.live:
+            os.makedirs(GOLDEN_REF, exist_ok=True)
+            np.savez_compressed(self.path, **self.data)
+
+    @staticmethod
+    def _digest(a):
+        a = _np(a)
+        h = hashlib.sha256(str((a.dtype.str, a.shape)).encode())
+        h.update(a.tobytes())
+        return np.frombuffer(h.digest(), np.uint8)
+
+    def equal(self, key, ours, ref=None):
+        """Same dtype, shape and bytes as the reference array."""
+        if self.live:
+            self.data[key + ".sha256"] = self._digest(ref())
+        return bool(np.array_equal(self._digest(ours), self.data[key + ".sha256"]))
+
+    def _pair(self, key, ours, ref):
+        a = _np(ours).astype(np.float64).reshape(-1)
+        if self.live:
+            b = _np(ref()).astype(np.float64).reshape(-1)
+            assert a.size == b.size, key
+            idx = self._index(key, b.size)
+            self.data[key + ".sample"] = b[idx].astype(np.float32)   # the reference computes in fp32
+            self.data[key + ".maxabs"] = np.float64(np.abs(b).max() if b.size else 0.0)
+            self.data[key + ".size"] = np.int64(b.size)
+            return a, b, float(self.data[key + ".maxabs"])
+        assert a.size == int(self.data[key + ".size"]), key
+        return a[self._index(key, a.size)], self.data[key + ".sample"].astype(np.float64), float(self.data[key + ".maxabs"])
+
+    def _index(self, key, n):
+        if n <= self.SAMPLE:
+            return np.arange(n)
+        rng = np.random.default_rng(zlib.crc32(key.encode()))
+        return np.unique(rng.integers(0, n, self.SAMPLE))
+
+    def frac_bad(self, key, ours, ref=None, rtol=1e-4, atol_scale=1e-4):
+        """frac_bad() against the reference: over the whole array when recording, over the sample otherwise."""
+        a, b, m = self._pair(key, ours, ref)
+        return float((np.abs(a - b) > rtol * np.abs(b) + atol_scale * m).mean()) if b.size else 0.0
+
+    def max_abs_diff(self, key, ours, ref=None):
+        """(max |ours - ref|, max |ref|), the first over the whole array when recording, over the sample otherwise."""
+        a, b, m = self._pair(key, ours, ref)
+        return (float(np.abs(a - b).max()) if b.size else 0.0), m
+
+    def rel_err(self, key, ours, ref=None):
+        d, m = self.max_abs_diff(key, ours, ref)
+        return d / (m + 1e-30)
 
 
 def rel_err(a, b):

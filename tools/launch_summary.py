@@ -1,5 +1,5 @@
 """Summarises an `ncu --metrics gpu__time_duration.sum --csv` launch list: share of each kernel.
-usage: python tools/launch_summary.py profiles/r01_launches_k3.csv "<header line>" """
+usage: python tools/launch_summary.py launches.csv "<header line>" """
 import collections
 import csv
 import sys

@@ -1,8 +1,8 @@
 // Shared-memory wavefront probe: warp-wide LDS.32 / LDS.64 / LDS.128 with the address of lane l given by a pattern of
 // its lane bits (the patterns the blend kernels use or could use).
-//   nvcc -arch=sm_100a -O3 -o /tmp/lds_probe tools/lds_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lds_probe tools/lds_probe.cu
 //   ncu --metrics l1tex__data_pipe_lsu_wavefronts_mem_shared_op_ld.sum,smsp__inst_executed_op_shared_ld.sum \
-//       --csv --log-file out.csv /tmp/lds_probe 16 quick          (tools/run_probe.sh; table: profiles/r02_lds_probe_wavefronts.txt)
+//       --csv --log-file out.csv ./lds_probe 16 quick
 // The wavefront counters of ncu are the measurement; the cycles the program prints itself are issue-bound (3 instructions
 // per load) and only rank the patterns.  One CTA of NW warps per SM; every warp issues 8 independent loads per iteration.
 #include <cstdio>

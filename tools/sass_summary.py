@@ -1,6 +1,6 @@
 """Opcode histogram per kernel of libsgb200.so from `cuobjdump -sass` (no GPU needed): which hardware paths each
-kernel uses — packed FMA (FFMA2), bulk / tensor copies (UBLKCP, UTMALDG), cp.async (LDGSTS), mbarriers (SYNCS),
-tensor cores (UTC*MMA, LDTM), legacy tensor path (HMMA).   usage: python tools/sass_summary.py > profiles/r02_sass_summary.txt"""
+kernel uses — bulk / tensor copies (UBLKCP, UTMALDG), cp.async (LDGSTS), mbarriers (SYNCS), warpgroup tensor-core
+MMAs (HGMMA, the opt-in path of blend_mma.cu), legacy tensor path (HMMA).   usage: python tools/sass_summary.py [lib]"""
 import collections
 import os
 import re
@@ -10,8 +10,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "semantic-gaussians_b200", "libsgb200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-KEY = ("FFMA2", "FFMA", "FMUL", "FADD", "MUFU", "LDS", "STS", "LDG", "STG", "RED", "ATOM", "LDGSTS", "UBLKCP", "UTMALDG", "UTMASTG",
-       "SYNCS", "BAR", "SHFL", "VOTE", "UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "HMMA", "IMAD", "BRA")
+KEY = ("FFMA", "FMUL", "FADD", "MUFU", "LDS", "STS", "LDG", "STG", "RED", "ATOM", "LDGSTS", "UBLKCP", "UTMALDG", "UTMASTG",
+       "SYNCS", "BAR", "SHFL", "VOTE", "HGMMA", "WARPGROUP", "HMMA", "IMAD", "BRA")
 kern, hist = None, {}
 arch = None
 for line in out.splitlines():
