@@ -105,6 +105,7 @@ void sgb_ctx_destroy(sgb_ctx* c) {
     if (c->geom.p) cudaFree(c->geom.p);
     if (c->bin.p) cudaFree(c->bin.p);
     if (c->misc.p) cudaFree(c->misc.p);
+    if (c->work.p) cudaFree(c->work.p);
     for (PoolSlot& sl : c->pools)
         if (sl.mem.p) cudaFree(sl.mem.p);
     if (c->pinned) cudaFreeHost(c->pinned);
@@ -156,7 +157,7 @@ uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
 
 size_t sgb_ctx_scratch_bytes(const sgb_ctx* c) {
     if (!c) return 0;
-    size_t n = c->geom.cap + c->bin.cap + c->misc.cap;
+    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap;
     for (const PoolSlot& sl : c->pools) n += sl.mem.cap;
     return n;
 }

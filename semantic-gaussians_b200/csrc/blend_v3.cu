@@ -19,12 +19,14 @@
 //                     (register micro-tiles + transposed shuffle reduce), then the reference's
 //                     back-to-front chain (backward.cu:477-550) in dot-product form -> dL/dmean2D,
 //                     dL/dconic, dL/dopacity.
-//   dfeature_v3       CTA = (tile, 64-channel chunk): dL/dfeature[g][ch] = sum_px w * dL/dout, one
-//                     warp per 8-channel slice over all 256 pixels, one 32-byte reduction per
-//                     (Gaussian, tile, slice).
+//   dfeature          persistent CTAs claim (tile, 64-channel chunk) items: dL/dfeature[g][ch] = sum_px
+//                     w * dL/dout, a producer warp streams dL tiles and weight slabs by TMA, every
+//                     compute warp owns 8 channels of all the tile's entries, one 16-byte reduction
+//                     per (Gaussian, tile, 4 channels).
 //
 // Results are unchanged: the integer outputs come from the verbatim chain; every accumulator still
 // adds its Gaussians in depth order.
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
@@ -597,160 +599,274 @@ __global__ void __launch_bounds__(kThreads, 2) blend_forward_tma_kernel(
 }
 
 // dF[entry][ch] = sum over the tile's 256 pixels of w[entry][px] * dL/dout[px][ch]   (K = pixels).
-// CTA = (tile, 64-channel chunk).  The dL tile is copied once into shared memory in its native
-// [channel][pixel] order by cp.async row pieces (no transposing stores); warp w owns entries
-// 16w..16w+15 of each 128-entry pass and streams their weight rows through a private double-buffered
-// slab [16][32 px].  Lane = (eg, cg) accumulates entries {eg + 4j} x channels {4cg..4cg+3} U {32+4cg..32+4cg+3}; one K
-// step covers 4 pixels with LDS.128 of both operands, and the paired FMAs take (even, odd) pixels — no register
-// duplication, the two halves are added at the end.
-// The load/store unit, not the FMA pipe, limits this kernel when every lane issues 32 scalar red.global per pass on
-// top of 4-wavefront operand loads.  Therefore
-//   * a lane owns two blocks of 4 CONSECUTIVE channels, so a Gaussian's sums leave as two red.global.add.v4.f32
-//     (8 reductions per lane and pass instead of 32);
-//   * the 16-byte pixel quads of channel row r sit at quad ^ ((r >> 2) & 7): the 8 channel groups of one load then hit 8
-//     different bank groups although their rows are 4 apart (pitch 256 floats, no padding);
-//   * eg / cg come from lane_group4 / lane_group8: every operand load is a 2-wavefront LDS.128.
-template <int CH>
-__global__ void __launch_bounds__(kThreads, 2) dfeature_gemm_kernel(int W, int H, int C,
-                                                                   const float* __restrict__ dL_dpixels,
-                                                                   PoolView pool, float* __restrict__ dL_dcolors) {
-    static_assert(CH == 64, "64-channel chunks");
-    constexpr int DP = SGB_TILE_PIX;  // pitch of a channel row of the dL tile (quads XOR-swizzled, see above)
-    constexpr int WP = 36;            // pitch of the per-warp weight slab rows (32 px + pad)
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    float(*dLs)[DP] = reinterpret_cast<float(*)[DP]>(smem_raw);
-    float* wslab = reinterpret_cast<float*>(smem_raw + sizeof(float) * CH * DP);
-    __shared__ const float* Wrow[128];
-    __shared__ uint32_t Gid[128];
+// Persistent: the grid fills the GPU once and every CTA claims work items (tile, 64-channel chunk; the chunk varies
+// fastest, so the CTAs of one tile meet its weight rows in L2) from a counter until none are left; an empty tile
+// costs one claim.  Warp 8 is the producer and warps 0-7 only compute:
+//   * the dL tile of an item, [16 rows][64 ch][16 px] = 64 KB, is ONE 3-D TMA box into one of two buffers.  The
+//     producer issues the next item's box while the current item is being contracted (at its 5th weight slab, when
+//     every warp has provably released the buffer).  Layouts TMA cannot take (W % 4 != 0 or a misaligned base) are
+//     staged by the producer warp with 4-byte cp.async into the same (swizzled) layout, on the same mbarrier;
+//   * the weight rows of a pass (up to 128 entries) stream as 32-pixel slabs, one 3-D TMA box [16 rows][32 px] per
+//     16-entry pool chunk, through a ring of kDfStages stages.
+// Every hand-off is a full/empty mbarrier pair; there is no CTA-wide barrier after the set-up.  Warp w owns channels
+// 8w..8w+7 of the chunk and ALL entries of the pass, so every warp computes on every item however few entries the
+// tile has.  Lane (eg = lane >> 1, cgp = lane & 1) accumulates entries {eg + 16j, j < R} x channels 8w + 4cgp + {0..3}
+// in scalar registers, R = ceil(entries / 16) <= 8: per 4-pixel K step 16R FMAs for R + 4 LDS.128.  The TMA swizzles
+// keep every operand load at 2 shared-memory wavefronts or less (see lane_group8):
+//   * weights, SWIZZLE_128B: quad q of the 128-byte row e sits at q ^ (e & 7); each 4-lane group reads 2 rows and each
+//     half-warp 8 consecutive rows -> 8 distinct bank groups;
+//   * dL, SWIZZLE_64B over a [row][ch][16 px] box: quad p of channel c sits at p ^ ((c >> 1) & 3), so channels c and
+//     c + 4 (the two cgp halves of a load) land in different banks.
+constexpr int kDfCH = 64;                   // channels per work item
+constexpr int kDfStages = 4;                // weight-slab ring depth
+constexpr int kDfThreads = kThreads + 32;   // 8 compute warps + 1 producer warp
+constexpr int kDfPass = 128;                // entries per pass (8 pool chunks)
+constexpr int kDfSlabs = SGB_TILE_PIX / 32;  // 32-pixel K slabs per pass
+constexpr uint32_t kDfTileBytes = SGB_TILE_PIX * kDfCH * 4;
 
-    const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
-    const int nchunksC = (C + CH - 1) / CH;
-    const int tile = blockIdx.x / nchunksC;
-    const int ch0 = (blockIdx.x % nchunksC) * CH;
-    const int nch = min(CH, C - ch0);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t n = pool.count[tile];
-    if (n == 0) return;  // (empty tiles are common: returning before the 64 KB dL copy matters)
-    const uint32_t dbase = __ldg(pool.dirbase + tile);
-    const uint2 pix_min = {(uint32_t)(tile % tiles_x) * SGB_TILE, (uint32_t)(tile / tiles_x) * SGB_TILE};
-    const size_t plane = (size_t)H * W;
-    const bool rows16 = (W & 3) == 0 && (reinterpret_cast<uintptr_t>(dL_dpixels) & 15) == 0;
-    // dL tile -> smem [ch][quad ^ swizzle][4 px]: 16-byte pieces (4 pixels of one tile row of one channel)
-    for (int idx = tid; idx < CH * SGB_TILE * 4; idx += kThreads) {
-        const int pc = idx & 3, r = (idx >> 2) & (SGB_TILE - 1), c = idx >> 6;
-        const uint32_t y = pix_min.y + r, x = pix_min.x + pc * 4;
-        float* dst = &dLs[c][((r * 4 + pc) ^ ((c >> 2) & 7)) * 4];
-        const float* src = dL_dpixels + (size_t)(ch0 + c) * plane + (size_t)W * y + x;
-        const bool rowok = c < nch && y < (uint32_t)H;
-        if (rows16) {
-            const bool ok = rowok && x + 4 <= (uint32_t)W;
-            cp_async16(dst, ok ? src : dL_dpixels, ok ? 16 : 0);
-        } else {
+struct DfHdr {  // one weight-ring stage's description, written by the producer before the stage is armed
+    int end;            // no more work
+    int cnt;            // entries of the pass
+    int slab;           // pixels 32 slab .. 32 slab + 31
+    int first, last;    // first slab of the item (wait for its dL tile) / last slab of the item (release the tile)
+    int dbuf;           // dL buffer of the item and the parity of its fill
+    uint32_t dpar;
+    int ch0, nch;
+    uint32_t gid[kDfPass];  // Gaussian ids of the pass (written for the last slab of a pass)
+};
+struct DfSmem {  // at a 1024-byte aligned offset of the dynamic shared memory (TMA swizzle atoms)
+    float dl[2][SGB_TILE_PIX * kDfCH];
+    float w[kDfStages][kDfPass * 32];
+    DfHdr hdr[kDfStages];
+    uint64_t wfull[kDfStages], wempty[kDfStages], dfull[2], dempty[2];
+};
+constexpr size_t kDfSmemBytes = sizeof(DfSmem) + 1024;
+static_assert(kDfSmemBytes <= 227 * 1024, "dL/dfeature shared memory exceeds the sm_90 opt-in limit");
+
+__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src, int src_bytes) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes)
+                 : "memory");
+}
+// Arrives on `bar` once every cp.async this thread issued so far has landed (the arrival is part of the init count).
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+// One 32-pixel slab of a pass: acc[j][k] += sum over the slab of w[eg + 16j][px] * dL[px][cl + k].
+// dl points at channel cl of the item's dL buffer, ws at the stage's weight rows; swz = (cl >> 1) & 3.
+template <int R>
+__device__ __forceinline__ void df_slab(float (&acc)[8][4], const float* __restrict__ ws, const float* __restrict__ dl,
+                                        int slab, int eg, int swz) {
 #pragma unroll
-            for (int i = 0; i < 4; i++) dst[i] = (rowok && x + i < (uint32_t)W) ? __ldg(src + i) : 0.f;
+    for (int q = 0; q < 8; q++) {
+        const int Q = slab * 8 + q;  // pixel quad of the tile: row Q >> 2, quad Q & 3 of the row
+        float4 d[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+            d[k] = *reinterpret_cast<const float4*>(dl + (Q >> 2) * (kDfCH * 16) + k * 16 +
+                                                    (((Q & 3) ^ swz ^ (k >> 1)) << 2));
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            const float4 wv = *reinterpret_cast<const float4*>(ws + (eg + 16 * j) * 32 + ((q ^ (eg & 7)) << 2));
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                acc[j][k] = fmaf(wv.x, d[k].x, acc[j][k]);
+                acc[j][k] = fmaf(wv.y, d[k].y, acc[j][k]);
+                acc[j][k] = fmaf(wv.z, d[k].z, acc[j][k]);
+                acc[j][k] = fmaf(wv.w, d[k].w, acc[j][k]);
+            }
         }
     }
-    cp_async_commit();
+}
 
-    const int eg = lane_group4(lane), cg = lane_group8(lane);
-    const bool red16 = ((C & 3) == 0) && ((reinterpret_cast<uintptr_t>(dL_dcolors) & 15) == 0);
-    for (uint32_t base = 0; base < n; base += 128) {
-        const int cnt = (int)min(128u, n - base);
-        __syncthreads();  // previous pass done with Wrow / Gid
-        if (tid < cnt) {
-            const WChunk* ck = pool.chunks + chunk_of(pool, dbase, (int)((base + tid) / kChunkEntries));
-            const int s = (base + tid) & (kChunkEntries - 1);
-            Wrow[tid] = &ck->w[s][0];
-            Gid[tid] = ck->meta[s].x;
+__global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
+    int W, int H, int C, const float* __restrict__ dL_dpixels, PoolView pool, float* __restrict__ dL_dcolors,
+    int* __restrict__ work_counter, const __grid_constant__ CUtensorMap dl_map,
+    const __grid_constant__ CUtensorMap w_map, const int use_tma) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    DfSmem& sm = *reinterpret_cast<DfSmem*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int kComputeWarps = kThreads / 32;
+    if (tid == 0) {
+        for (int i = 0; i < kDfStages; i++) {
+            mbar_init(&sm.wfull[i], 1);
+            mbar_init(&sm.wempty[i], kComputeWarps);
         }
-        cp_async_wait<0>();
-        __syncthreads();  // Wrow / Gid visible; dL tile landed (first pass)
-        if (warp * 16 < cnt) {
-            float(*wsl)[16][WP] = reinterpret_cast<float(*)[16][WP]>(wslab + (size_t)warp * 2 * 16 * WP);
-            const float* lrow[4];
+        for (int i = 0; i < 2; i++) {
+            mbar_init(&sm.dfull[i], use_tma ? 1 : 32);
+            mbar_init(&sm.dempty[i], kComputeWarps);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (warp < kComputeWarps) {
+        const int eg = lane >> 1, cgp = lane & 1;
+        const int cl = warp * 8 + cgp * 4;  // channel (within the chunk) of k = 0
+        const bool red16 = ((C & 3) == 0) && ((reinterpret_cast<uintptr_t>(dL_dcolors) & 15) == 0);
+        float acc[8][4];
+        for (uint32_t step = 0;; step++) {
+            const int st = (int)(step % kDfStages);
+            mbar_wait(&sm.wfull[st], (step / kDfStages) & 1u);
+            const DfHdr& h = sm.hdr[st];
+            if (h.end) break;
+            const int slab = h.slab, cnt = h.cnt, dbuf = h.dbuf, nch = h.nch, last = h.last;
+            const int R = (cnt + 15) >> 4;
+            if (h.first) mbar_wait(&sm.dfull[dbuf], h.dpar);
+            if (slab == 0) {
 #pragma unroll
-            for (int i = 0; i < 4; i++) lrow[i] = Wrow[min(warp * 16 + (lane >> 3) + 4 * i, cnt - 1)] + (lane & 7) * 4;
-            auto issue = [&](int sl, int buf) {
+                for (int j = 0; j < 8; j++)
 #pragma unroll
-                for (int i = 0; i < 4; i++)
-                    cp_async16(&wsl[buf][(lane >> 3) + 4 * i][(lane & 7) * 4], lrow[i] + sl * 32, 16);
-                cp_async_commit();
-            };
-            float2 acc[4][8];  // [entry eg+4j][channel (k >> 2) * 32 + 4 cg + (k & 3)], .x even pixels, .y odd pixels
-#pragma unroll
-            for (int j = 0; j < 4; j++)
-#pragma unroll
-                for (int k = 0; k < 8; k++) acc[j][k] = make_float2(0.f, 0.f);
-            issue(0, 0);
-            for (int sl = 0; sl < SGB_TILE_PIX / 32; sl++) {
-                const int buf = sl & 1;
-                if (sl + 1 < SGB_TILE_PIX / 32) { issue(sl + 1, buf ^ 1); cp_async_wait<1>(); }
-                else cp_async_wait<0>();
-                __syncwarp();
-                // Fully unrolled and software-pipelined by hand: ptxas otherwise issues every LDS right in
-                // front of its first consumer, and the FMAs wait on short-scoreboard stalls.  dL rows are
-                // fetched two K-steps ahead, the next pixel quad's weights while
-                // the current quad is being consumed.
-                const float* drow = &dLs[4 * cg][0];
-                const float* wbase = &wsl[buf][eg][0];
-                auto ld_d = [&](int step) {  // step = p4 * 8 + k; row (k >> 2) * 32 + 4 cg + (k & 3), quad sl * 8 + p4
-                    const int k = step & 7, p4 = step >> 3;
-                    return *reinterpret_cast<const float4*>(drow + ((k >> 2) * 32 + (k & 3)) * DP +
-                                                            (((sl * 8 + p4) ^ cg) << 2));
-                };
-                float4 wq[4], wn[4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) wq[j] = *reinterpret_cast<const float4*>(wbase + 4 * j * WP);
-                float4 d0 = ld_d(0), d1 = ld_d(1);
-#pragma unroll
-                for (int p4 = 0; p4 < 8; p4++) {
-#pragma unroll
-                    for (int k = 0; k < 8; k++) {
-                        const int step = p4 * 8 + k;
-                        float4 d2 = d1;
-                        if (step + 2 < 64) d2 = ld_d(step + 2);
-                        if (k == 2 && p4 + 1 < 8) {
-#pragma unroll
-                            for (int j = 0; j < 4; j++)
-                                wn[j] = *reinterpret_cast<const float4*>(wbase + 4 * j * WP + (p4 + 1) * 4);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 4; j++) {
-                            acc[j][k] = ffma2(make_float2(wq[j].x, wq[j].y), make_float2(d0.x, d0.y), acc[j][k]);
-                            acc[j][k] = ffma2(make_float2(wq[j].z, wq[j].w), make_float2(d0.z, d0.w), acc[j][k]);
-                        }
-                        d0 = d1;
-                        d1 = d2;
-                    }
-                    if (p4 + 1 < 8) {
-#pragma unroll
-                        for (int j = 0; j < 4; j++) wq[j] = wn[j];
-                    }
-                }
-                __syncwarp();  // slab `buf` may be refilled by the next issue
+                    for (int k = 0; k < 4; k++) acc[j][k] = 0.f;
             }
+            if (warp * 8 < nch) {
+                const float* ws = sm.w[st];
+                const float* dl = sm.dl[dbuf] + cl * 16;
+                const int swz = (cl >> 1) & 3;
+                switch (R) {
+                    case 1: df_slab<1>(acc, ws, dl, slab, eg, swz); break;
+                    case 2: df_slab<2>(acc, ws, dl, slab, eg, swz); break;
+                    case 3: df_slab<3>(acc, ws, dl, slab, eg, swz); break;
+                    case 4: df_slab<4>(acc, ws, dl, slab, eg, swz); break;
+                    case 5: df_slab<5>(acc, ws, dl, slab, eg, swz); break;
+                    case 6: df_slab<6>(acc, ws, dl, slab, eg, swz); break;
+                    case 7: df_slab<7>(acc, ws, dl, slab, eg, swz); break;
+                    default: df_slab<8>(acc, ws, dl, slab, eg, swz); break;
+                }
+                if (slab == kDfSlabs - 1 && cl < nch) {
+                    const int ch0 = h.ch0;
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const int e = warp * 16 + eg + 4 * j;
-                if (e < cnt) {
-                    float* dst = dL_dcolors + (size_t)Gid[e] * C + ch0 + 4 * cg;
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        const int chl = h * 32 + 4 * cg;
-                        const float4 v = make_float4(acc[j][4 * h + 0].x + acc[j][4 * h + 0].y, acc[j][4 * h + 1].x + acc[j][4 * h + 1].y,
-                                                     acc[j][4 * h + 2].x + acc[j][4 * h + 2].y, acc[j][4 * h + 3].x + acc[j][4 * h + 3].y);
-                        if (red16 && chl + 4 <= nch) {
-                            red_add_v4_f32(dst + h * 32, v);
+                    for (int j = 0; j < 8; j++) {
+                        const int e = eg + 16 * j;
+                        if (j >= R || e >= cnt) continue;
+                        float* dst = dL_dcolors + (size_t)h.gid[e] * C + ch0 + cl;
+                        if (red16 && cl + 4 <= nch) {
+                            red_add_v4_f32(dst, make_float4(acc[j][0], acc[j][1], acc[j][2], acc[j][3]));
                         } else {
-                            if (chl + 0 < nch) red_add_f32(dst + h * 32 + 0, v.x);
-                            if (chl + 1 < nch) red_add_f32(dst + h * 32 + 1, v.y);
-                            if (chl + 2 < nch) red_add_f32(dst + h * 32 + 2, v.z);
-                            if (chl + 3 < nch) red_add_f32(dst + h * 32 + 3, v.w);
+#pragma unroll
+                            for (int k = 0; k < 4; k++)
+                                if (cl + k < nch) red_add_f32(dst + k, acc[j][k]);
                         }
                     }
                 }
             }
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&sm.wempty[st]);
+                if (last) mbar_arrive(&sm.dempty[dbuf]);
+            }
         }
+        return;
+    }
+
+    // ---- producer warp
+    const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
+    const int tiles = tiles_x * ((H + SGB_TILE - 1) / SGB_TILE);
+    const int nchunksC = (C + kDfCH - 1) / kDfCH;
+    const int total = tiles * nchunksC;
+    const size_t plane = (size_t)H * W;
+    uint32_t step = 0;   // ring stages armed so far
+    uint32_t items = 0;  // non-empty items whose dL tile was issued
+    struct Item { int tile, ch0; uint32_t n; int dbuf; uint32_t dpar; };
+    auto acquire = [&]() -> int {  // next ring stage, once the compute warps released its previous use
+        const int st = (int)(step % kDfStages);
+        if (step >= kDfStages) mbar_wait(&sm.wempty[st], ((step / kDfStages) - 1) & 1u);
+        return st;
+    };
+    // Claims items until a non-empty one and issues its dL tile; tile < 0 when the work is exhausted.
+    auto claim = [&]() -> Item {
+        Item it{-1, 0, 0u, 0, 0u};
+        for (;;) {
+            int k = 0;
+            if (lane == 0) k = atomicAdd(work_counter, 1);
+            k = __shfl_sync(0xffffffffu, k, 0);
+            if (k >= total) return it;
+            it.tile = k / nchunksC;
+            it.ch0 = (k % nchunksC) * kDfCH;
+            it.n = pool.count[it.tile];
+            if (it.n != 0) break;
+        }
+        it.dbuf = (int)(items & 1);
+        it.dpar = (items >> 1) & 1u;
+        if (items >= 2) mbar_wait(&sm.dempty[it.dbuf], ((items >> 1) - 1) & 1u);  // item `items - 2` released it
+        items++;
+        const int x0 = (it.tile % tiles_x) * SGB_TILE, y0 = (it.tile / tiles_x) * SGB_TILE;
+        float* dst = sm.dl[it.dbuf];
+        if (use_tma) {
+            if (lane == 0) {
+                mbar_arrive_expect_tx(&sm.dfull[it.dbuf], kDfTileBytes);
+                tma_tile3d_g2s(dst, &dl_map, x0, it.ch0, y0, &sm.dfull[it.dbuf]);
+            }
+        } else {
+            for (int idx = lane; idx < SGB_TILE_PIX * kDfCH; idx += 32) {
+                const int x = idx & (SGB_TILE - 1), r = (idx >> 4) & (SGB_TILE - 1), c = idx >> 8;
+                const int gx = x0 + x, gy = y0 + r;
+                const bool ok = it.ch0 + c < C && gx < W && gy < H;
+                const float* src = ok ? dL_dpixels + (size_t)(it.ch0 + c) * plane + (size_t)W * gy + gx : dL_dpixels;
+                cp_async4(dst + r * (kDfCH * 16) + c * 16 + ((((x >> 2) ^ ((c >> 1) & 3)) << 2) | (x & 3)), src,
+                          ok ? 4 : 0);
+            }
+            cp_async_mbar_arrive_noinc(&sm.dfull[it.dbuf]);
+        }
+        return it;
+    };
+
+    Item cur = claim();
+    while (cur.tile >= 0) {
+        Item nxt{-1, 0, 0u, 0, 0u};
+        bool claimed = false;
+        const uint32_t dbase = pool.dirbase[cur.tile];
+        const int nch = min(kDfCH, C - cur.ch0);
+        int slab_of_item = 0;
+        for (uint32_t base = 0; base < cur.n; base += kDfPass) {
+            const int cnt = (int)min((uint32_t)kDfPass, cur.n - base);
+            const int nck = (cnt + kChunkEntries - 1) / kChunkEntries;
+            const uint32_t cid = lane < nck ? chunk_of(pool, dbase, (int)(base / kChunkEntries) + lane) : 0u;
+            uint32_t gid[kDfPass / 32];
+#pragma unroll
+            for (int i = 0; i < kDfPass / 32; i++) {
+                const int e = lane + 32 * i;
+                const uint32_t c = __shfl_sync(0xffffffffu, cid, e / kChunkEntries);
+                gid[i] = e < cnt ? pool.chunks[c].meta[e & (kChunkEntries - 1)].x : 0u;
+            }
+            for (int s = 0; s < kDfSlabs; s++, slab_of_item++) {
+                if (!claimed && slab_of_item == kDfStages) {
+                    // the stage acquired below was released by every warp after the item's first slab, so every
+                    // warp is past the previous item and its dL buffer is free: prefetch the next item's tile now
+                    nxt = claim();
+                    claimed = true;
+                }
+                const int st = acquire();
+                DfHdr& h = sm.hdr[st];
+                if (lane == 0) {
+                    h.end = 0;
+                    h.cnt = cnt;
+                    h.slab = s;
+                    h.first = base == 0 && s == 0;
+                    h.last = base + kDfPass >= cur.n && s == kDfSlabs - 1;
+                    h.dbuf = cur.dbuf;
+                    h.dpar = cur.dpar;
+                    h.ch0 = cur.ch0;
+                    h.nch = nch;
+                }
+                if (s == kDfSlabs - 1) {
+#pragma unroll
+                    for (int i = 0; i < kDfPass / 32; i++) h.gid[lane + 32 * i] = gid[i];
+                }
+                if (lane < nck)
+                    tma_tile3d_g2s(&sm.w[st][lane * kChunkEntries * 32], &w_map, 32 * s, 0, (int)cid, &sm.wfull[st]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive_expect_tx(&sm.wfull[st], (uint32_t)nck * (kChunkEntries * 32 * 4));
+                step++;
+            }
+        }
+        if (!claimed) nxt = claim();
+        cur = nxt;
+    }
+    const int st = acquire();
+    if (lane == 0) {
+        sm.hdr[st].end = 1;
+        mbar_arrive(&sm.wfull[st]);
     }
 }
 
@@ -1779,6 +1895,54 @@ static int pool_for_backward(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R,
     return SGB_E_NOMEM;
 }
 
+using TensorMapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link); nullptr when unavailable.
+static TensorMapEncodeFn tensor_map_encoder() {
+    static const TensorMapEncodeFn encode = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return (TensorMapEncodeFn)fn;
+    }();
+    return encode;
+}
+
+// dL/dout (C, H, W) fp32 for dfeature_persistent_kernel, described with its dimensions in the order (x, channel, y) so
+// that one [16 px][64 ch][16 rows] box lands as [row][ch][16 px] under the 64-byte swizzle.  Returns false (the kernel
+// then stages the tile with cp.async) when the layout does not meet the TMA rules (base and row pitch multiples of 16
+// bytes) or the driver entry point is not available.
+static bool encode_dfeature_dl_map(CUtensorMap* map, const float* dL_dpix, int W, int H, int C) {
+    const TensorMapEncodeFn encode = tensor_map_encoder();
+    memset(map, 0, sizeof(*map));
+    if (!encode || (W & 3) != 0 || (reinterpret_cast<uintptr_t>(dL_dpix) & 15) != 0) return false;
+    const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)C, (cuuint64_t)H};
+    const cuuint64_t strides[2] = {(cuuint64_t)W * H * sizeof(float), (cuuint64_t)W * sizeof(float)};
+    const cuuint32_t box[3] = {SGB_TILE, kDfCH, SGB_TILE};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(dL_dpix), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// The weight rows of a pool as (pixel, row of the chunk, chunk): a [32 px][16 rows] box is one 32-pixel slab of a
+// 16-entry chunk, stored under the 128-byte swizzle.
+static bool encode_dfeature_w_map(CUtensorMap* map, const PoolView& pv) {
+    const TensorMapEncodeFn encode = tensor_map_encoder();
+    memset(map, 0, sizeof(*map));
+    if (!encode) return false;
+    const cuuint64_t dims[3] = {(cuuint64_t)SGB_TILE_PIX, (cuuint64_t)kChunkEntries, (cuuint64_t)pv.capacity};
+    const cuuint64_t strides[2] = {(cuuint64_t)SGB_TILE_PIX * sizeof(float), (cuuint64_t)sizeof(WChunk)};
+    const cuuint32_t box[3] = {32, kChunkEntries, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, reinterpret_cast<char*>(pv.chunks) + offsetof(WChunk, w),
+                  dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
                                const float* dL_dpix, float* dL_dcolors, cudaStream_t s) {
     PoolView pv;
@@ -1786,16 +1950,38 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t 
     if (rc) return rc;
     if (blend_mma_enabled() && in.C % 4 == 0 && (reinterpret_cast<uintptr_t>(dL_dcolors) & 15) == 0)
         return launch_dfeature_mma(ctx, in, dL_dpix, dL_dcolors, pv, s);  // opt-in experiment
-    const int tiles = num_tiles(in);
-    const int chunks = (in.C + 63) / 64;
-    const size_t smem_d = sizeof(float) * (64 * SGB_TILE_PIX + 8 * 2 * 16 * 36);
+    const int items = num_tiles(in) * ((in.C + kDfCH - 1) / kDfCH);
+    if (items == 0) return SGB_OK;
+    CUtensorMap dl_map, w_map;
+    const int use_tma = encode_dfeature_dl_map(&dl_map, dL_dpix, in.W, in.H, in.C) ? 1 : 0;
+    if (!encode_dfeature_w_map(&w_map, pv)) {
+        set_error("dL/dfeature: cuTensorMapEncodeTiled is unavailable or rejected the weight pool");
+        return SGB_E_CUDA;
+    }
+    rc = ctx->work.ensure(sizeof(int));
+    if (rc) return rc;
+    // persistent grid: as many CTAs as are co-resident on the device
     static DeviceOnce attr_set;
-    if (attr_set.first_use_on_device())
-        SGB_CUDA(cudaFuncSetAttribute(dfeature_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_d));
+    static int grid_of_device[64];
+    int dev = 0;
+    SGB_CUDA(cudaGetDevice(&dev));
+    int& grid = grid_of_device[dev < 64 ? dev : 63];
+    if (attr_set.first_use_on_device()) {
+        SGB_CUDA(cudaFuncSetAttribute(dfeature_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)kDfSmemBytes));
+        int per_sm = 0, sms = 0;
+        SGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dfeature_persistent_kernel, kDfThreads,
+                                                               kDfSmemBytes));
+        SGB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        grid = per_sm * sms > 0 ? per_sm * sms : 1;
+    }
+    int* counter = static_cast<int*>(ctx->work.p);
     StageTimer t(ctx, ST_DFEATURE, s);
+    SGB_CUDA(cudaMemsetAsync(counter, 0, sizeof(int), s));
     ctx->launches += 1;
-    dfeature_gemm_kernel<64><<<tiles * chunks, kThreads, smem_d, s>>>(in.W, in.H, in.C, dL_dpix, pv, dL_dcolors);
-    SGB_LAUNCH_CHECK("dfeature_gemm_kernel", in.debug, s);
+    dfeature_persistent_kernel<<<grid < items ? grid : items, kDfThreads, kDfSmemBytes, s>>>(
+        in.W, in.H, in.C, dL_dpix, pv, dL_dcolors, counter, dl_map, w_map, use_tma);
+    SGB_LAUNCH_CHECK("dfeature_persistent_kernel", in.debug, s);
     return SGB_OK;
 }
 
@@ -1803,17 +1989,7 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t 
 // false (the kernel then stages the slabs with cp.async) when the layout does not meet the TMA rules (base and row
 // pitch multiples of 16 bytes) or the driver entry point is not available.  SGB_CHAIN_TMA=0 forces the cp.async path.
 static bool encode_dl_map(CUtensorMap* map, const float* dL_dpix, int W, int H, int C) {
-    using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static const EncodeFn encode = [] {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            fn = nullptr;
-        return (EncodeFn)fn;
-    }();
+    const TensorMapEncodeFn encode = tensor_map_encoder();
     memset(map, 0, sizeof(*map));
     const char* off = getenv("SGB_CHAIN_TMA");
     if (off && off[0] == '0') return false;

@@ -145,6 +145,7 @@ struct sgb_ctx {
     sgb::Scratch geom;     // depth-sort keys/values, offsets, CUB temp (one slice per view of a batch)
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
+    sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
     sgb::PoolSlot pools[sgb::kMaxBatch];  // per-tile weight rows of the C-channel blend (blend_v3.cu)
     uint64_t pool_clock = 0;
     uint64_t pool_chunks_hint = 0;  // high-water mark of the pool demand (chunks)
