@@ -284,6 +284,34 @@ int sgb_label_argmax(int32_t K, int32_t first_class, int64_t N, const float* pla
  * reference).  Fewer than 4 points leave FLT_MAX terms, as in the reference. */
 int sgb_knn_mean_dist2(sgb_ctx* ctx, int32_t P, const float* points, float* mean_dist2, void* stream);
 
+/* ---- photometric training loss: the RGB loss of the reference's training step (train.py:141-149)
+ *     loss = (1 - lambda) * L1(x, y) + lambda * (1 - SSIM(x, y))
+ * with SSIM as utils/loss_utils.py:38-72 computes it: an 11x11 Gaussian window (sigma 1.5, fp32 taps divided by
+ * their fp32 sum) over zero padding, C1 = 0.01^2, C2 = 0.03^2, averaged over every pixel.
+ *
+ * x (the rendered image) and y (the target) are `planes` fp32 planes of h x w (one plane = one channel of one
+ * image: C planes for (C,H,W), N*C for (N,C,H,W)), each given as a base pointer plus a plane stride and a row
+ * stride in elements; the pixel stride is 1.  A border crop (train.py's cut_edge) is thus a pointer offset with
+ * the full image's strides.  The plane stride is ignored when planes == 1.
+ *
+ * sgb_photometric_forward: sums (2 doubles, device, zeroed by the call) receive [0] sum |x - y| and [1] sum of
+ * the per-pixel SSIM map over all planes.  partials (device, (3, planes, h, w) fp32, contiguous) receives the
+ * three per-pixel maps backward needs; NULL when no gradient is wanted.
+ *
+ * sgb_photometric_backward: dL_dx[p][r][c] (written through its own strides, only inside the h x w planes) =
+ *     coef[0] * sign(x - y) + coef[1] * d(sum SSIM map)/dx
+ * with coef (2 floats, DEVICE) = {g (1 - lambda) / n, -g lambda / n} for the loss above (n = planes * h * w,
+ * g = the upstream gradient), or {0, g / n} for mean SSIM alone.  sign(0) = 0.
+ *
+ * Both calls are asynchronous on `stream` and never copy to the host. */
+int sgb_photometric_forward(int32_t planes, int32_t h, int32_t w, const float* x, int64_t x_plane_stride,
+                            int64_t x_row_stride, const float* y, int64_t y_plane_stride, int64_t y_row_stride,
+                            double* sums, float* partials, void* stream);
+int sgb_photometric_backward(int32_t planes, int32_t h, int32_t w, const float* x, int64_t x_plane_stride,
+                             int64_t x_row_stride, const float* y, int64_t y_plane_stride, int64_t y_row_stride,
+                             const float* partials, const float* coef, float* dL_dx, int64_t dx_plane_stride,
+                             int64_t dx_row_stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
