@@ -22,8 +22,8 @@ namespace {
 constexpr int kThreads = SGB_TILE_PIX;
 constexpr int kWarps = kThreads / 32;
 constexpr int kBatchB = 32;  // Gaussians per stage (one bit each in the per-warp activity mask)
+constexpr int CH = 4;        // channels per CTA: all of them (C <= 4)
 
-template <int CH>
 struct __align__(16) BwdSmem {
     float4 recA[2][kBatchB];
     float4 recB[2][kBatchB];
@@ -40,28 +40,6 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// Sum v[k] over the 32 lanes for every k with log-step exchange: after the call lane l holds the
-// totals of channels l*(CH/32) + i in v[i], i < CH/32 (CH >= 32).  CH - 1 shuffles instead of 5*CH.
-template <int CH>
-__device__ __forceinline__ void warp_transpose_reduce(float (&v)[CH], int lane) {
-    static_assert(CH >= 32 && (CH & (CH - 1)) == 0, "CH must be a power of two >= 32");
-    int n = CH;
-#pragma unroll
-    for (int step = 16; step >= 1; step >>= 1) {
-        n >>= 1;
-        const bool upper = (lane & step) != 0;
-#pragma unroll
-        for (int i = 0; i < CH / 2; i++) {
-            if (i < n) {
-                const float send = upper ? v[i] : v[i + n];
-                const float keep = upper ? v[i + n] : v[i];
-                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, step);
-            }
-        }
-    }
-}
-
-template <int CH, bool BULK>
 __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int C,
     const float* __restrict__ bg_color, const SplatRec* __restrict__ rec, const float* __restrict__ colors,
@@ -69,8 +47,7 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
     const uint32_t* __restrict__ tile_last, const float* __restrict__ dL_dpixels, float* __restrict__ dL_dmean2D,
     float* __restrict__ dL_dconic2D, float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    BwdSmem<CH>& sm = *reinterpret_cast<BwdSmem<CH>*>(smem_raw);
-    __shared__ uint64_t bar[2];
+    BwdSmem& sm = *reinterpret_cast<BwdSmem*>(smem_raw);
 
     const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
     const int tile = blockIdx.x;
@@ -89,11 +66,6 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
     const int nbatches = (total + kBatchB - 1) / kBatchB;
     if (nbatches == 0) return;
 
-    if (tid == 0 && BULK) {
-        mbar_init(&bar[0], 1);
-        mbar_init(&bar[1], 1);
-        mbar_fence_init();
-    }
     // Unused tail of the last (partial) chunk must read as zero: it is multiplied into sums.
     if (nch < CH)
         for (int e = tid; e < 2 * kBatchB * CH; e += kThreads) {
@@ -107,28 +79,17 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
         const int st = b & 1;
         const int hi = total - b * kBatchB;
         const int cnt = min(kBatchB, hi);
-        if (BULK) {
-            if (tid == 0) mbar_arrive_expect_tx(&bar[st], (uint32_t)cnt * (32u + (uint32_t)nch * 4u));
-            if (tid < cnt) {
-                const uint32_t id = point_list[range.x + hi - 1 - tid];
-                sm.ids[st][tid] = id;
-                bulk_g2s(&sm.recA[st][tid], reinterpret_cast<const float4*>(rec + id), 16, &bar[st]);
-                bulk_g2s(&sm.recB[st][tid], reinterpret_cast<const float4*>(rec + id) + 1, 16, &bar[st]);
-                bulk_g2s(&sm.feat[st][tid][0], colors + (size_t)id * C + ch0, (uint32_t)nch * 4u, &bar[st]);
-            }
-        } else {
-            if (tid < cnt) {
-                const uint32_t id = point_list[range.x + hi - 1 - tid];
-                sm.ids[st][tid] = id;
-                const float4* rp = reinterpret_cast<const float4*>(rec + id);
-                sm.recA[st][tid] = __ldg(rp);
-                sm.recB[st][tid] = __ldg(rp + 1);
-            }
-            for (int e = tid; e < cnt * nch; e += kThreads) {
-                const int j = e / nch, k = e - j * nch;
-                const uint32_t id = point_list[range.x + hi - 1 - j];
-                sm.feat[st][j][k] = __ldg(colors + (size_t)id * C + ch0 + k);
-            }
+        if (tid < cnt) {
+            const uint32_t id = point_list[range.x + hi - 1 - tid];
+            sm.ids[st][tid] = id;
+            const float4* rp = reinterpret_cast<const float4*>(rec + id);
+            sm.recA[st][tid] = __ldg(rp);
+            sm.recB[st][tid] = __ldg(rp + 1);
+        }
+        for (int e = tid; e < cnt * nch; e += kThreads) {
+            const int j = e / nch, k = e - j * nch;
+            const uint32_t id = point_list[range.x + hi - 1 - j];
+            sm.feat[st][j][k] = __ldg(colors + (size_t)id * C + ch0 + k);
         }
     };
 
@@ -154,8 +115,7 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
         const int cnt = min(kBatchB, hi);
         __syncthreads();  // batch b-1 fully consumed and flushed: stage (b+1)&1 and dF/geo are free
         if (b + 1 < nbatches) issue(b + 1);
-        if (BULK) mbar_wait(&bar[st], (uint32_t)((b >> 1) & 1));
-        __syncthreads();  // ids[] (generic-proxy stores) visible; also orders the non-BULK loads
+        __syncthreads();  // batch b staged by every thread
         uint32_t my_active = 0;
 
         for (int j = 0; j < cnt; j++) {
@@ -199,20 +159,10 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
                 *reinterpret_cast<float4*>(gp) = make_float4(g0, g1, g2, g3);
                 *reinterpret_cast<float2*>(gp + 4) = make_float2(g4, g5);
             }
-            if (CH >= 32) {
-                float v[CH >= 32 ? CH : 32];
 #pragma unroll
-                for (int k = 0; k < CH; k++) v[k] = w * dL[k];  // :519
-                warp_transpose_reduce<(CH >= 32 ? CH : 32)>(v, lane);
-                constexpr int per = CH / 32 > 0 ? CH / 32 : 1;
-#pragma unroll
-                for (int i = 0; i < per; i++) sm.dF[warp][j][lane * per + i] = v[i];
-            } else {
-#pragma unroll
-                for (int k = 0; k < CH; k++) {
-                    const float t = warp_sum(w * dL[k]);
-                    if (lane == 0) sm.dF[warp][j][k] = t;
-                }
+            for (int k = 0; k < CH; k++) {
+                const float t = warp_sum(w * dL[k]);  // :519
+                if (lane == 0) sm.dF[warp][j][k] = t;
             }
             my_active |= 1u << j;
         }
@@ -248,25 +198,6 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
     }
 }
 
-template <int CH, bool BULK>
-int launch_one(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
-               const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolors,
-               cudaStream_t s) {
-    const int tiles = ((in.W + SGB_TILE - 1) / SGB_TILE) * ((in.H + SGB_TILE - 1) / SGB_TILE);
-    const int chunks = (in.C + CH - 1) / CH;
-    const size_t smem = sizeof(BwdSmem<CH>);
-    auto kern = blend_backward_kernel<CH, BULK>;
-    static DeviceOnce attr_set;
-    if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    kern<<<dim3(tiles, chunks), kThreads, smem, s>>>(im.ranges, b.point_list, in.W, in.H, in.C, in.background, g.rec,
-                                                    colors, im.final_T, im.n_contrib, im.tile_last, dL_dpix,
-                                                    dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
-    SGB_LAUNCH_CHECK("blend_backward_kernel", in.debug, s);
-    return SGB_OK;
-}
-
 }  // namespace
 
 int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
@@ -276,7 +207,18 @@ int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgV
         set_error("launch_blend_backward handles C <= 4 only");
         return SGB_E_INVALID;
     }
-    return launch_one<4, false>(in, g, b, im, colors, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, s);
+    const int tiles = ((in.W + SGB_TILE - 1) / SGB_TILE) * ((in.H + SGB_TILE - 1) / SGB_TILE);
+    const int chunks = (in.C + CH - 1) / CH;
+    const size_t smem = sizeof(BwdSmem);
+    static DeviceOnce attr_set;
+    if (attr_set.first_use_on_device()) {
+        SGB_CUDA(cudaFuncSetAttribute(blend_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    blend_backward_kernel<<<dim3(tiles, chunks), kThreads, smem, s>>>(
+        im.ranges, b.point_list, in.W, in.H, in.C, in.background, g.rec, colors, im.final_T, im.n_contrib,
+        im.tile_last, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
+    SGB_LAUNCH_CHECK("blend_backward_kernel", in.debug, s);
+    return SGB_OK;
 }
 
 }  // namespace sgb

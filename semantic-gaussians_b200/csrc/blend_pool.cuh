@@ -1,5 +1,5 @@
 // Weight pool of the C-channel blend (blend_v3.cu): per tile the alpha * T rows of every Gaussian that touches it,
-// in 16-entry chunks found through a per-tile directory.  Shared by blend_v3.cu and the opt-in blend_mma.cu.
+// in 16-entry chunks found through a per-tile directory.
 #pragma once
 #include "common.cuh"
 
@@ -38,15 +38,5 @@ struct PoolView {
 __device__ __forceinline__ uint32_t chunk_of(const PoolView& pool, uint32_t dbase, int k) {
     return min(__ldg(pool.dir + dbase + k), pool.capacity - 1);
 }
-
-// opt-in tensor-core forward (blend_mma.cu)
-bool blend_mma_enabled();
-int launch_forward_mma(sgb_ctx* ctx, const sgb_view_inputs& in, ImgView im, const float* colors, float* out_color,
-                       const PoolView& pv, cudaStream_t s);
-int launch_chain_mma(sgb_ctx* ctx, const sgb_view_inputs& in, GeomView g, ImgView im, const float* colors,
-                     const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, const PoolView& pv,
-                     cudaStream_t s);
-int launch_dfeature_mma(sgb_ctx* ctx, const sgb_view_inputs& in, const float* dL_dpix, float* dL_dcolors,
-                        const PoolView& pv, cudaStream_t s);
 
 }  // namespace sgb

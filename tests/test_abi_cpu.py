@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     assert b"sm_90a" in lib.sgb_version()
 
 
-def test_library_contains_sm90a_code_with_tma_and_wgmma():
+def test_library_contains_sm90a_code_with_bulk_and_tensor_copies():
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
@@ -35,7 +35,7 @@ def test_library_contains_sm90a_code_with_tma_and_wgmma():
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert "sm_90a" in sass
     assert "UBLKCP" in sass          # cp.async.bulk (TMA engine) staging of the per-tile Gaussian blocks
-    assert "HGMMA" in sass           # wgmma of the opt-in tensor-core contractions (blend_mma.cu)
+    assert "UTMALDG" in sass         # tensor-map tile copies of dfeature_persistent_kernel and chain_backward_warp_kernel
 
 
 def test_state_sizes_are_sane():

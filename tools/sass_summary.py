@@ -1,6 +1,6 @@
 """Opcode histogram per kernel of libsgb200.so from `cuobjdump -sass` (no GPU needed): which hardware paths each
 kernel uses — bulk / tensor copies (UBLKCP, UTMALDG), cp.async (LDGSTS), mbarriers (SYNCS), warpgroup tensor-core
-MMAs (HGMMA, the opt-in path of blend_mma.cu), legacy tensor path (HMMA).   usage: python tools/sass_summary.py [lib]"""
+MMAs (HGMMA), legacy tensor path (HMMA).   usage: python tools/sass_summary.py [lib]"""
 import collections
 import os
 import re

@@ -1,6 +1,5 @@
-"""Stage timings (library tracing) of one workload under the env knobs SGB_FWD_IMPL / SGB_BWD_IMPL.
+"""Stage timings (library tracing) of one C-channel forward + backward workload.
 usage: python tools/time_stages.py [P W H C reps]"""
-import math
 import os
 import sys
 
@@ -31,25 +30,17 @@ def step(i):
             v.grad = None
 
 
-for cfg in sys.stdin.read().split() if not sys.stdin.isatty() else ["default"]:
-    for kv in cfg.split(","):
-        if "=" in kv:
-            k, v = kv.split("=")
-            os.environ[k] = v
-    for i in range(2):
-        step(i)
-    torch.cuda.synchronize()
-    _lib.profile_enable(ctx, True)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(reps):
-        step(i)
-    e1.record()
-    torch.cuda.synchronize()
-    st = _lib.profile_read(ctx)
-    _lib.profile_enable(ctx, False)
-    print(cfg, f"total {e0.elapsed_time(e1) / reps:.3f} ms/step |",
-          " ".join(f"{k}={v[0] / max(v[1], 1):.3f}" for k, v in st.items() if v[1]), flush=True)
-    for kv in cfg.split(","):
-        if "=" in kv:
-            os.environ.pop(kv.split("=")[0], None)
+for i in range(2):
+    step(i)
+torch.cuda.synchronize()
+_lib.profile_enable(ctx, True)
+e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+e0.record()
+for i in range(reps):
+    step(i)
+e1.record()
+torch.cuda.synchronize()
+st = _lib.profile_read(ctx)
+_lib.profile_enable(ctx, False)
+print(f"total {e0.elapsed_time(e1) / reps:.3f} ms/step |",
+      " ".join(f"{k}={v[0] / max(v[1], 1):.3f}" for k, v in st.items() if v[1]), flush=True)
