@@ -106,7 +106,7 @@ def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_ch
     single = render if variant == "rgbd" else (
         lambda cam, *a, **k: render_chn(cam, *a, num_channels=num_channels, **k))
     per_view_colors = override_color is None and pipe.convert_shs_python   # python SH -> colours depend on the camera
-    if per_view_colors or pc.get_xyz.shape[0] == 0:
+    if per_view_colors:
         return [single(cam, pc, pipe, bg_color, scaling_modifier=scaling_modifier, override_color=override_color,
                        override_shape=override_shape, foreground=foreground, world_rotate=world_rotate)
                 for cam in cameras]

@@ -256,6 +256,12 @@ def test_empty_and_degenerate_inputs():
     color, radii = chn.GaussianRasterizer(rs(8))(means3D=z(0, 3), means2D=z(0, 3), opacities=z(0, 1),
                                                  colors_precomp=z(0, 8), scales=z(0, 3), rotations=z(0, 4))
     assert color.shape == (8, 48, 64) and radii.numel() == 0 and torch.all(color == 0.0)
+    s = rs(8)
+    outs = chn.GaussianRasterizer.rasterize_batch(z(0, 3), [z(0, 3), z(0, 3)], z(0, 1), [s, s], colors_precomp=z(0, 8),
+                                                  scales=z(0, 3), rotations=z(0, 4))
+    assert len(outs) == 2
+    for color, radii in outs:
+        assert color.shape == (8, 48, 64) and radii.numel() == 0 and torch.all(color == 0.0)
     # everything behind the camera: nothing rendered, R = 0
     xyz = torch.tensor([[0.0, 0.0, 0.0]], device=dev) + torch.as_tensor(cam.camera_center, device=dev) * 2
     color, radii = chn.GaussianRasterizer(rs(4))(means3D=xyz, means2D=z(1, 3), opacities=torch.ones(1, 1, device=dev),
