@@ -158,14 +158,7 @@ int run_depth_order_and_scan(sgb_ctx* ctx, const sgb_view_inputs& in_common, int
     if (rc) return rc;
     unsigned long long* h = (unsigned long long*)ctx->pinned;
     for (int v = 0; v < V; v++) {
-        sgb_view_inputs in = in_common;
-        if (cams) {
-            in.viewmatrix = cams[v].viewmatrix;
-            in.projmatrix = cams[v].projmatrix;
-            in.campos = cams[v].campos;
-            in.tan_fovx = cams[v].tan_fovx;
-            in.tan_fovy = cams[v].tan_fovy;
-        }
+        const sgb_view_inputs in = with_camera(in_common, cams[v]);
         GeomView g = GeomView::carve(geometry_states[v], P);
         char* base = (char*)ctx->geom.p + (size_t)v * per_view;
         uint32_t* keys_in = (uint32_t*)(base);

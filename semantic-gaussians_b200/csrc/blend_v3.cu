@@ -62,11 +62,10 @@ struct __align__(16) AlphaSmem {
     uint32_t s_last;
 };
 
-template <bool DEPTH>
 __global__ void __launch_bounds__(kThreads) alpha_pass_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
     const SplatRec* __restrict__ rec, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
-    uint32_t* __restrict__ tile_last, float* __restrict__ out_depth, PoolView pool) {
+    uint32_t* __restrict__ tile_last, PoolView pool) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     AlphaSmem& sm = *reinterpret_cast<AlphaSmem*>(smem_raw);
 
@@ -88,7 +87,6 @@ __global__ void __launch_bounds__(kThreads) alpha_pass_kernel(
 
     float T = 1.0f;
     uint32_t last_contributor = 0;
-    float D = 15.0f;
     uint32_t n_tile = 0;  // entries appended so far (uniform)
     uint32_t n_blend = 0; // Gaussians blended into this pixel
 
@@ -144,9 +142,6 @@ __global__ void __launch_bounds__(kThreads) alpha_pass_kernel(
                             done = true;
                         } else {
                             w = alpha * T;
-                            if (DEPTH) {
-                                if (T > 0.5f && test_T < 0.5) D = a.z;
-                            }
                             T = test_T;
                             last_contributor = (uint32_t)(base + j + 1);
                         }
@@ -201,7 +196,6 @@ __global__ void __launch_bounds__(kThreads) alpha_pass_kernel(
     if (inside) {
         final_T[pix_id] = T;
         n_contrib[pix_id] = last_contributor;
-        if (DEPTH) out_depth[pix_id] = D;
         atomicMax(&sm.s_last, last_contributor);
     }
     n_blend = __reduce_add_sync(0xffffffffu, n_blend);
@@ -368,11 +362,6 @@ __global__ void __launch_bounds__(kThreads, 2) blend_forward_v3_kernel(
 }
 
 // ------------------------------------------------------------------------------------ async-copy helpers
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src, int src_bytes) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 // 3-D tensor tile global -> shared through the TMA engine (SASS: UTMALDG): box corner (x, y, z) in elements, out-of-range
 // elements arrive as zeros; completion is signalled on `bar` as the box's bytes.  dst 128-byte aligned.
 __device__ __forceinline__ void tma_tile3d_g2s(void* dst_smem, const CUtensorMap* map, int x, int y, int z, uint64_t* bar) {
@@ -384,10 +373,6 @@ __device__ __forceinline__ void tma_tile3d_g2s(void* dst_smem, const CUtensorMap
 }
 // Orders this thread's earlier generic-proxy shared-memory accesses before later async-proxy (TMA) writes.
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
 
 // ------------------------------------------------------------------------------------ GEMM-shaped kernels
 // With the weights materialised per tile, the three C-wide contractions are small dense GEMMs over the
@@ -853,8 +838,9 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
 //   * the warp walks the tile list from the back and COMPACTS it on the fly to the entries whose strip-mask bit is
 //     set (ballot + popc ranks), 32 entries per segment: no zero-strip work, padding <= 31 slots per strip;
 //   * s-pass per segment: S[32 px][32 entries] over all channels, lane tile 8 px x 4 entries (16 paired FMAs per 3
-//     LDS.128); the warp stages its own operands — the dL/dout slab [16 ch][32 px] by cp.async, the feature slab by
-//     4 x LDG.128 per lane (lane = entry) one slab ahead in registers, stored transposed [ch][entry];
+//     LDS.128); the warp stages its own operands — the dL/dout slab [16 ch][32 px] by TMA (plain loads for rows that
+//     are not 16-byte aligned), the feature slab by 4 x LDG.128 per lane (lane = entry) one slab ahead in registers,
+//     stored transposed [ch][entry];
 //   * S is parked in the warp's dL slab region (XOR-swizzled 16-byte chunks: conflict-free both ways) and lane = pixel
 //     runs the reference's back-to-front chain (backward.cu:477-550, dot-product form) over the 32 entries.
 // Shared memory 9.3 KB per warp, 128 registers, 2 CTAs/SM (a third CTA would leave less L1 for the gathered feature
@@ -871,6 +857,28 @@ struct __align__(16) ChainWarpSmem {
     uint32_t Gid[32];
 };
 constexpr int kMetaCap = 512;  // tile-list entries whose (id, mask) records are cached in shared memory
+
+// dL slab sl [16 ch][32 px of strip `warp`] by plain loads, for image rows that are not 16-byte aligned (no tensor
+// map): lane -> (channel row (lane >> 3) + 4 i of the slab, 4-pixel piece pc = lane & 7: tile row pc >> 2 of the strip,
+// columns (pc & 3) * 4 ..).  Out of line so that its addressing holds no registers in the kernel, which runs at its
+// 128-register limit.
+__device__ __noinline__ void dl_slab_plain(float (*DS)[32], const float* __restrict__ dL_dpixels, int W, int H, int C,
+                                           uint2 pix_min, int warp, int lane, int sl) {
+    constexpr int CK = 16;
+    const size_t plane = (size_t)H * W;
+    const int pc = lane & 7;
+    const uint32_t y = pix_min.y + 2 * warp + (pc >> 2), x = pix_min.x + (pc & 3) * 4;
+    const float* srcs = dL_dpixels + (size_t)(sl * CK + (lane >> 3)) * plane + (size_t)W * y + x;
+#pragma unroll
+    for (int i = 0; i < CK / 4; i++) {
+        const int chl = (lane >> 3) + 4 * i;
+        const bool chin = sl * CK + chl < C;
+        const float* src = srcs + (size_t)(4 * i) * plane;
+#pragma unroll
+        for (int u = 0; u < 4; u++)
+            DS[chl][pc * 4 + u] = (chin && y < (uint32_t)H && x + u < (uint32_t)W) ? __ldg(src + u) : 0.f;
+    }
+}
 
 template <bool VEC>
 __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
@@ -899,7 +907,6 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
     if (n == 0) return;
     const uint32_t dbase = pool.dirbase[tile];
     const size_t plane = (size_t)H * W;
-    const bool rows16 = ((W & 3) == 0) && ((reinterpret_cast<uintptr_t>(dL_dpixels) & 15) == 0);
     const int woff = warp * 32 + lane;
 
     // ---- CTA prologue: directory + (id, mask) records of the tile list -> shared memory; background flag
@@ -935,22 +942,8 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
     const int nslab = (C + CK - 1) / CK;
     float (*S)[32] = reinterpret_cast<float (*)[32]>(&ws.DS[0][0][0]);
 
-    // dL slab [CK ch][32 px of this strip]: 4 x cp.async(16 B) per lane; lane -> (channel row (lane >> 3) + 4 i of the
-    // slab, 16-byte piece lane & 7: tile row pc >> 2 of the strip, columns (pc & 3) * 4 ..)
-    const int d_pc = lane & 7;
-    const uint32_t d_y = pix_min.y + 2 * warp + (d_pc >> 2), d_x = pix_min.x + (d_pc & 3) * 4;
-    const bool d_rowin = d_y < (uint32_t)H;
-    const bool d_vec_ok = d_rowin && d_x + 4 <= (uint32_t)W;
-    const float* d_src0 = dL_dpixels + (size_t)(lane >> 3) * plane + (size_t)W * d_y + d_x;
-    // Fast path (16-byte aligned image rows, full slab): the lane keeps a running source pointer; a lane whose piece is
-    // outside the image points at the image base with zero strides and copies 0 bytes (cp.async zero-fills).
-    const char* const d_base = reinterpret_cast<const char*>(d_vec_ok ? d_src0 : dL_dpixels);
-    const size_t d_step4 = d_vec_ok ? 4 * plane * sizeof(float) : 0;       // 4 channel rows further
-    const size_t d_stepslab = d_vec_ok ? CK * plane * sizeof(float) : 0;   // next slab
-    const int d_bytes = d_vec_ok ? 16 : 0;
-    const char* d_run = d_base;
-    // TMA path (image rows 16-byte aligned; the map is encoded per launch by the host): ONE instruction of one lane
-    // fetches the whole [16 ch][2 rows][16 px] box — rows below the image, columns right of it and channels >= C arrive
+    // dL slab [CK ch][32 px of this strip].  TMA path (image rows 16-byte aligned; the map is encoded per launch by
+    // the host): ONE instruction of one lane fetches the whole [16 ch][2 rows][16 px] box — rows below the image, columns right of it and channels >= C arrive
     // as zeros — and none of it passes through the LSU data pipe (the four LDGSTS per lane it replaces were 64 of the
     // ~210 L1 wavefronts per slab, and the L1 data pipe bounds this kernel).
     uint32_t dphase = 0;  // bit b: parity the next wait on buffer b expects
@@ -964,33 +957,7 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
             }
             return;
         }
-        if (rows16 && (sl + 1) * CK <= C) {
-            float* dst = &ws.DS[buf][lane >> 3][d_pc * 4];
-            const char* src = d_run;
-#pragma unroll
-            for (int i = 0; i < CK / 4; i++) {
-                cp_async16(dst + i * 4 * 32, src, d_bytes);
-                src += d_step4;
-            }
-        } else {
-            const float* srcs = d_src0 + (size_t)sl * CK * plane;
-#pragma unroll
-            for (int i = 0; i < CK / 4; i++) {
-                const int chl = (lane >> 3) + 4 * i;
-                const bool chin = sl * CK + chl < C;
-                const float* src = srcs + (size_t)(4 * i) * plane;
-                if (rows16) {
-                    const bool ok = chin && d_vec_ok;
-                    cp_async16(&ws.DS[buf][chl][d_pc * 4], ok ? src : dL_dpixels, ok ? 16 : 0);
-                } else {  // image rows not 16-byte aligned: plain loads, ordered by the warp barrier of the slab loop
-#pragma unroll
-                    for (int u = 0; u < 4; u++)
-                        ws.DS[buf][chl][d_pc * 4 + u] = (chin && d_rowin && d_x + u < (uint32_t)W) ? __ldg(src + u) : 0.f;
-                }
-            }
-        }
-        d_run += d_stepslab;
-        cp_async_commit();
+        dl_slab_plain(ws.DS[buf], dL_dpixels, W, H, C, pix_min, warp, lane, sl);  // ordered by the slab loop's barrier
     };
 
     uint32_t cursor = n;  // tile-list entries [0, cursor) are still to be visited (back to front)
@@ -1089,10 +1056,9 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
             }
         };
         // One warp barrier per slab: at the top of iteration sl every lane has finished the math of slab sl-1, so the
-        // other buffers (dL by cp.async, features from the registers loaded one slab earlier) can be refilled BEFORE
+        // other buffers (dL by TMA or plain loads, features from the registers loaded one slab earlier) can be refilled BEFORE
         // the math of slab sl and their latency hides behind it.
         fload(0);
-        d_run = d_base;
         dissue(0, 0);
         fstore(0, 0);
         if (nslab > 1) fload(1);
@@ -1101,8 +1067,6 @@ __global__ void __launch_bounds__(kThreads, 2) chain_backward_warp_kernel(
             if (use_tma) {
                 mbar_wait(&dbar[warp][buf], (dphase >> buf) & 1u);
                 dphase ^= 1u << buf;
-            } else {
-                cp_async_wait<0>();
             }
             __syncwarp();  // DS[buf] landed, FT[buf] stored by every lane; DS/FT[buf ^ 1] are free
             if (sl + 1 < nslab) {
@@ -1239,38 +1203,29 @@ size_t pool_bytes(int tiles, uint32_t chunks, int64_t R, PoolView* v, void* base
 }  // namespace
 
 // ---- weight-pool slots ---------------------------------------------------------------------------------------
+// A view's slot is the one keyed by its binning-state pointer.  The pool header of slot i is read back through
+// pinned header i: the views of one batch have distinct slots, so one sync reads all their headers.
+constexpr int kMaxAlphaPasses = 4;  // per view and call: the first guess and up to three grown pools
+
 static inline int num_tiles(const sgb_view_inputs& in) {
     return ((in.W + SGB_TILE - 1) / SGB_TILE) * ((in.H + SGB_TILE - 1) / SGB_TILE);
 }
 
-static PoolSlot* pool_find(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, BinView b) {
+static PoolSlot* slot_of(sgb_ctx* ctx, const ViewState& w) {
     for (PoolSlot& sl : ctx->pools)
-        if (sl.valid && sl.key_bin == (const void*)b.point_list && sl.key_R == R && sl.key_W == in.W && sl.key_H == in.H &&
-            sl.key_P == in.P) {
-            sl.stamp = ++ctx->pool_clock;
-            return &sl;
-        }
+        if (sl.key_bin == (const void*)w.b.point_list) return &sl;
     return nullptr;
 }
 
-// Slot for a view that is about to be (re)built: the one already keyed by this binning state (a new forward
-// through the same pointer replaces it), else an empty one, else the least recently used.
-static PoolSlot* pool_acquire(sgb_ctx* ctx, BinView b) {
-    PoolSlot* pick = nullptr;
-    for (PoolSlot& sl : ctx->pools)
-        if (sl.key_bin == (const void*)b.point_list) { pick = &sl; break; }
-    if (!pick)
-        for (PoolSlot& sl : ctx->pools)
-            if (!sl.valid && !sl.key_bin) { pick = &sl; break; }
-    if (!pick) {
-        pick = &ctx->pools[0];
-        for (PoolSlot& sl : ctx->pools)
-            if (sl.stamp < pick->stamp) pick = &sl;
-    }
-    pick->valid = false;
-    pick->key_bin = (const void*)b.point_list;
-    pick->stamp = ++ctx->pool_clock;
-    return pick;
+// pinned readback layout: [0, 8 * SGB_MAX_BATCH) the R values of a geometry batch; then one PoolHdr (16 B) per slot
+static inline PoolHdr* pinned_hdr(sgb_ctx* ctx, const PoolSlot* sl) {
+    return reinterpret_cast<PoolHdr*>(reinterpret_cast<char*>(ctx->pinned) + 8 * SGB_MAX_BATCH) + (sl - ctx->pools);
+}
+
+static PoolView slot_view(const ViewState& w, const PoolSlot& sl) {
+    PoolView pv;
+    pool_bytes(num_tiles(w.in), sl.chunks, w.R, &pv, sl.mem.p);
+    return pv;
 }
 
 static uint64_t pool_first_guess(sgb_ctx* ctx, int tiles, int64_t R) {
@@ -1283,33 +1238,117 @@ static uint64_t pool_first_guess(sgb_ctx* ctx, int tiles, int64_t R) {
     return guess;
 }
 
-static int launch_alpha_pass(sgb_ctx* ctx, const sgb_view_inputs& in, GeomView g, BinView b, ImgView im,
-                             float* out_depth, const PoolView& pv, cudaStream_t s) {
-    const int tiles = num_tiles(in);
+// Slot of a view that is about to be (re)built: the one already keyed by its binning state (a new forward through
+// the same pointer replaces it), else an empty one, else the least recently used.  It is carved for the first guess,
+// or keeps a larger existing carve that its memory still holds.
+int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s) {
+    PoolSlot* sl = slot_of(ctx, w);
+    if (!sl)
+        for (PoolSlot& c : ctx->pools)
+            if (!c.valid && !c.key_bin) { sl = &c; break; }
+    if (!sl) {
+        sl = &ctx->pools[0];
+        for (PoolSlot& c : ctx->pools)
+            if (c.stamp < sl->stamp) sl = &c;
+    }
+    sl->valid = false;
+    sl->key_bin = (const void*)w.b.point_list;
+    sl->stamp = ++ctx->pool_clock;
+    const int tiles = num_tiles(w.in);
+    uint64_t want = pool_first_guess(ctx, tiles, w.R);
+    if (sl->chunks > want && sl->mem.cap >= pool_bytes(tiles, sl->chunks, w.R, nullptr, nullptr)) want = sl->chunks;
+    const uint32_t chunks = (uint32_t)want;
+    int rc = sl->mem.ensure(pool_bytes(tiles, chunks, w.R, nullptr, nullptr));
+    if (rc) return rc;
+    sl->chunks = chunks;
+    const PoolView pv = slot_view(w, *sl);
     const size_t smem = sizeof(AlphaSmem);
     static DeviceOnce attr_set;
-    if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
+    if (attr_set.first_use_on_device())
+        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     SGB_CUDA(cudaMemsetAsync(pv.hdr, 0, sizeof(PoolHdr), s));
-    StageTimer t(ctx, ST_ALPHA, s);
-    if (out_depth)
-        alpha_pass_kernel<true><<<tiles, kThreads, smem, s>>>(im.ranges, b.point_list, in.W, in.H, g.rec, im.final_T,
-                                                            im.n_contrib, im.tile_last, out_depth, pv);
-    else
-        alpha_pass_kernel<false><<<tiles, kThreads, smem, s>>>(im.ranges, b.point_list, in.W, in.H, g.rec, im.final_T,
-                                                             im.n_contrib, im.tile_last, nullptr, pv);
-    SGB_LAUNCH_CHECK("alpha_pass_kernel", in.debug, s);
-    ctx->launches += 1;
+    {
+        StageTimer t(ctx, ST_ALPHA, s);
+        alpha_pass_kernel<<<tiles, kThreads, smem, s>>>(w.im.ranges, w.b.point_list, w.in.W, w.in.H, w.g.rec,
+                                                        w.im.final_T, w.im.n_contrib, w.im.tile_last, pv);
+        SGB_LAUNCH_CHECK("alpha_pass_kernel", w.in.debug, s);
+        ctx->launches += 1;
+    }
+    SGB_CUDA(cudaMemcpyAsync(pinned_hdr(ctx, sl), pv.hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, s));
     return SGB_OK;
 }
 
-static int launch_forward_gemm(sgb_ctx* ctx, const sgb_view_inputs& in, ImgView im, const float* colors,
-                               float* out_color, const PoolView& pv, cudaStream_t s) {
+// A pool that overflowed is re-carved for the demand its header reports (the counter keeps counting past capacity)
+// and built again; the rebuilt views are checked after one more sync.
+int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s, const bool* only) {
+    bool pending[SGB_MAX_BATCH];
+    for (int v = 0; v < V; v++) pending[v] = !only || only[v];
+    for (int pass = 1;; pass++) {
+        SGB_CUDA(cudaStreamSynchronize(s));
+        bool again = false;
+        for (int v = 0; v < V; v++) {
+            if (!pending[v]) continue;
+            const ViewState& w = vw[v];
+            PoolSlot* sl = slot_of(ctx, w);
+            if (!sl) { set_error("weight-pool slot of the view vanished"); return SGB_E_INVALID; }
+            const PoolHdr h = *pinned_hdr(ctx, sl);
+            if (h.overflow) {
+                const uint64_t need = (uint64_t)h.counter + h.counter / 8 + 64;
+                if (need > ctx->pool_chunks_hint) ctx->pool_chunks_hint = need;
+                sl->chunks = 0;  // re-carve with the new hint
+                if (pass == kMaxAlphaPasses) { set_error("weight pool kept overflowing"); return SGB_E_NOMEM; }
+                int rc = weight_pool_build(ctx, w, s);
+                if (rc) return rc;
+                again = true;
+                continue;
+            }
+            ctx->stat_blended_pairs = (int64_t)h.blended;
+            ctx->stat_pool_chunks = h.counter;
+            if (h.counter > ctx->pool_chunks_hint) ctx->pool_chunks_hint = (uint64_t)h.counter + h.counter / 16 + 16;
+            sl->valid = true;
+            sl->key_R = w.R;
+            sl->key_W = w.in.W;
+            sl->key_H = w.in.H;
+            sl->key_P = w.in.P;
+            pv[v] = slot_view(w, *sl);
+            pending[v] = false;
+        }
+        if (!again) return SGB_OK;
+    }
+}
+
+// A rebuild is needed only when the forward ran through another ctx or its slot was recycled.  Every hit is stamped
+// before the first miss takes a slot, so the least recently used slot a miss may evict is never one of this batch.
+int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s) {
+    bool miss[SGB_MAX_BATCH] = {};
+    bool any = false;
+    for (int v = 0; v < V; v++) {
+        const ViewState& w = vw[v];
+        if (w.R <= 0) continue;
+        PoolSlot* sl = slot_of(ctx, w);
+        if (sl && sl->valid && sl->key_R == w.R && sl->key_W == w.in.W && sl->key_H == w.in.H && sl->key_P == w.in.P) {
+            sl->stamp = ++ctx->pool_clock;
+            pv[v] = slot_view(w, *sl);
+        } else {
+            miss[v] = any = true;
+        }
+    }
+    if (!any) return SGB_OK;
+    for (int v = 0; v < V; v++) {
+        if (!miss[v]) continue;
+        int rc = weight_pool_build(ctx, vw[v], s);
+        if (rc) return rc;
+    }
+    return weight_pool_settle(ctx, V, vw, pv, s, miss);
+}
+
+// Forward GEMM of one view.  The host waited for the alpha passes only, so the caller keeps enqueueing the rest of
+// its step while the GEMM runs.
+int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s) {
+    const sgb_view_inputs& in = w.in;
     const int tiles = num_tiles(in);
     const int chunks = (in.C + 63) / 64;
-    const bool vec = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(colors) & 15) == 0);
+    const bool vec = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(w.colors) & 15) == 0);
     StageTimer t(ctx, ST_BLEND_FWD, s);
     ctx->launches += 1;
     if (vec) {
@@ -1320,103 +1359,16 @@ static int launch_forward_gemm(sgb_ctx* ctx, const sgb_view_inputs& in, ImgView 
             SGB_CUDA(cudaFuncSetAttribute(blend_forward_tma_kernel<64, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)smem_f));
         }
-        blend_forward_tma_kernel<64, NS><<<tiles * chunks, kThreads, smem_f, s>>>(in.W, in.H, in.C, colors, in.background,
-                                                                                  im.final_T, pv, out_color);
+        blend_forward_tma_kernel<64, NS><<<tiles * chunks, kThreads, smem_f, s>>>(in.W, in.H, in.C, w.colors,
+                                                                                  in.background, w.im.final_T, pv,
+                                                                                  out_color);
     } else {
         // feature rows that are not 16-byte aligned slices (C % 4 != 0) cannot be bulk-copied: plain loads
-        blend_forward_v3_kernel<64><<<tiles * chunks, kThreads, 0, s>>>(in.W, in.H, in.C, colors, in.background,
-                                                                         im.final_T, pv, out_color);
+        blend_forward_v3_kernel<64><<<tiles * chunks, kThreads, 0, s>>>(in.W, in.H, in.C, w.colors, in.background,
+                                                                         w.im.final_T, pv, out_color);
     }
     SGB_LAUNCH_CHECK("blend_forward kernel", in.debug, s);
     return SGB_OK;
-}
-
-// pinned readback layout: [0, 8 * kMaxBatch) the R values of a geometry batch; then one PoolHdr (16 B) per view slot
-static inline PoolHdr* pinned_hdr(sgb_ctx* ctx, int view_slot) {
-    return reinterpret_cast<PoolHdr*>(reinterpret_cast<char*>(ctx->pinned) + 8 * kMaxBatch) + view_slot;
-}
-
-// Alpha pass of one view into a pool slot; no stream sync (the pool header is copied to pinned slot `view_slot`).
-// The forward GEMM is launched by blend_forward_v3_gemm once blend_forward_v3_finish has validated the slot: the
-// host blocks only for the alpha pass (not for the GEMM), so the caller keeps enqueueing the rest of its step
-// while the GEMM runs.
-int blend_forward_v3_alpha(sgb_ctx* ctx, int view_slot, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b,
-                           ImgView im, cudaStream_t s) {
-    const int tiles = num_tiles(in);
-    PoolSlot* sl = pool_acquire(ctx, b);
-    uint64_t want = pool_first_guess(ctx, tiles, R);
-    if (sl->chunks > want && sl->mem.cap >= pool_bytes(tiles, sl->chunks, R, nullptr, nullptr)) want = sl->chunks;
-    const uint32_t chunks = (uint32_t)want;
-    int rc = sl->mem.ensure(pool_bytes(tiles, chunks, R, nullptr, nullptr));
-    if (rc) return rc;
-    sl->chunks = chunks;
-    PoolView pv;
-    pool_bytes(tiles, chunks, R, &pv, sl->mem.p);
-    rc = launch_alpha_pass(ctx, in, g, b, im, nullptr, pv, s);
-    if (rc) return rc;
-    SGB_CUDA(cudaMemcpyAsync(pinned_hdr(ctx, view_slot), pv.hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, s));
-    return SGB_OK;
-}
-
-int blend_forward_v3_gemm(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, BinView b, ImgView im,
-                          const float* colors, float* out_color, cudaStream_t s) {
-    PoolSlot* sl = pool_find(ctx, in, R, b);
-    if (!sl) { set_error("forward GEMM without validated weight rows"); return SGB_E_INVALID; }
-    PoolView pv;
-    pool_bytes(num_tiles(in), sl->chunks, R, &pv, sl->mem.p);
-    return launch_forward_gemm(ctx, in, im, colors, out_color, pv, s);
-}
-
-// After the stream sync: 0 = the view is done (slot validated), 1 = the pool overflowed — the slot was grown to the
-// real demand (the counter keeps counting past capacity) and the caller runs the alpha pass again; < 0 error.
-int blend_forward_v3_finish(sgb_ctx* ctx, int view_slot, const sgb_view_inputs& in, int64_t R, BinView b) {
-    PoolSlot* sl = nullptr;
-    for (PoolSlot& c : ctx->pools)
-        if (c.key_bin == (const void*)b.point_list) { sl = &c; break; }
-    if (!sl) { set_error("weight-pool slot of the view vanished"); return SGB_E_INVALID; }
-    const PoolHdr h = *pinned_hdr(ctx, view_slot);
-    if (h.overflow) {
-        const uint64_t need = (uint64_t)h.counter + h.counter / 8 + 64;
-        if (need > ctx->pool_chunks_hint) ctx->pool_chunks_hint = need;
-        sl->chunks = 0;  // re-carve with the new hint
-        return 1;
-    }
-    ctx->stat_blended_pairs = (int64_t)h.blended;
-    ctx->stat_pool_chunks = h.counter;
-    if (h.counter > ctx->pool_chunks_hint) ctx->pool_chunks_hint = (uint64_t)h.counter + h.counter / 16 + 16;
-    sl->valid = true;
-    sl->key_R = R;
-    sl->key_W = in.W;
-    sl->key_H = in.H;
-    sl->key_P = in.P;
-    return 0;
-}
-
-// Weight rows of a view for its backward: the slot its forward filled, else rebuilt here (one more alpha pass and a
-// stream sync for the pool check — only when the forward ran through another ctx or the slot was recycled).
-static int pool_for_backward(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
-                             PoolView* pv, cudaStream_t s) {
-    const int tiles = num_tiles(in);
-    if (PoolSlot* hit = pool_find(ctx, in, R, b)) {
-        pool_bytes(tiles, hit->chunks, R, pv, hit->mem.p);
-        return SGB_OK;
-    }
-    for (int attempt = 0; attempt < 4; attempt++) {
-        PoolSlot* sl = pool_acquire(ctx, b);
-        const uint32_t chunks = (uint32_t)pool_first_guess(ctx, tiles, R);
-        int rc = sl->mem.ensure(pool_bytes(tiles, chunks, R, nullptr, nullptr));
-        if (rc) return rc;
-        sl->chunks = chunks;
-        pool_bytes(tiles, chunks, R, pv, sl->mem.p);
-        rc = launch_alpha_pass(ctx, in, g, b, im, nullptr, *pv, s);
-        if (rc) return rc;
-        SGB_CUDA(cudaMemcpyAsync(pinned_hdr(ctx, 0), pv->hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, s));
-        SGB_CUDA(cudaStreamSynchronize(s));
-        rc = blend_forward_v3_finish(ctx, 0, in, R, b);
-        if (rc <= 0) return rc;
-    }
-    set_error("weight pool kept overflowing");
-    return SGB_E_NOMEM;
 }
 
 using TensorMapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1467,11 +1419,9 @@ static bool encode_dfeature_w_map(CUtensorMap* map, const PoolView& pv) {
                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
-                               const float* dL_dpix, float* dL_dcolors, cudaStream_t s) {
-    PoolView pv;
-    int rc = pool_for_backward(ctx, in, R, g, b, im, &pv, s);
-    if (rc) return rc;
+int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+                               float* dL_dcolors, cudaStream_t s) {
+    const sgb_view_inputs& in = w.in;
     const int items = num_tiles(in) * ((in.C + kDfCH - 1) / kDfCH);
     if (items == 0) return SGB_OK;
     CUtensorMap dl_map, w_map;
@@ -1480,7 +1430,7 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t 
         set_error("dL/dfeature: cuTensorMapEncodeTiled is unavailable or rejected the weight pool");
         return SGB_E_CUDA;
     }
-    rc = ctx->work.ensure(sizeof(int));
+    int rc = ctx->work.ensure(sizeof(int));
     if (rc) return rc;
     // persistent grid: as many CTAs as are co-resident on the device
     static DeviceOnce attr_set;
@@ -1508,7 +1458,7 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t 
 }
 
 // Tensor map of dL/dout (C, H, W) fp32 with a [16 ch][2 rows][16 px] box for the chain kernel's slab loads.  Returns
-// false (the kernel then stages the slabs with cp.async) when the layout does not meet the TMA rules (base and row
+// false (the kernel then loads the slabs with plain loads) when the layout does not meet the TMA rules (base and row
 // pitch multiples of 16 bytes) or the driver entry point is not available.
 static bool encode_dl_map(CUtensorMap* map, const float* dL_dpix, int W, int H, int C) {
     const TensorMapEncodeFn encode = tensor_map_encoder();
@@ -1523,14 +1473,11 @@ static bool encode_dl_map(CUtensorMap* map, const float* dL_dpix, int W, int H, 
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int blend_backward_v3_chain(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
-                            const float* colors, const float* dL_dpix, float* dL_dmean2D, float* dL_dconic,
-                            float* dL_dopacity, cudaStream_t s) {
-    PoolView pv;
-    int rc = pool_for_backward(ctx, in, R, g, b, im, &pv, s);
-    if (rc) return rc;
+int blend_backward_v3_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+                            float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, cudaStream_t s) {
+    const sgb_view_inputs& in = w.in;
     const int tiles = num_tiles(in);
-    const bool vec = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(colors) & 15) == 0);
+    const bool vec = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(w.colors) & 15) == 0);
     const size_t smem = sizeof(ChainWarpSmem) * (kThreads / 32);
     static DeviceOnce attr_set;
     if (attr_set.first_use_on_device()) {
@@ -1542,7 +1489,7 @@ int blend_backward_v3_chain(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, 
     CUtensorMap dl_map;
     const int use_tma = encode_dl_map(&dl_map, dL_dpix, in.W, in.H, in.C) ? 1 : 0;
     auto kern = vec ? chain_backward_warp_kernel<true> : chain_backward_warp_kernel<false>;
-    kern<<<tiles, kThreads, smem, s>>>(in.W, in.H, in.C, in.background, g.rec, colors, im.final_T, dL_dpix, pv,
+    kern<<<tiles, kThreads, smem, s>>>(in.W, in.H, in.C, in.background, w.g.rec, w.colors, w.im.final_T, dL_dpix, pv,
                                        dL_dmean2D, dL_dconic, dL_dopacity, dl_map, use_tma);
     SGB_LAUNCH_CHECK("chain backward kernel", in.debug, s);
     return SGB_OK;

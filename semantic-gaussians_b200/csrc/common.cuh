@@ -91,6 +91,37 @@ struct ImgView {  // carved out of image_state
     }
 };
 
+// `in` with the camera of `cam`: the views of a batched call share every other input.
+static inline sgb_view_inputs with_camera(const sgb_view_inputs& in, const sgb_camera& cam) {
+    sgb_view_inputs o = in;
+    o.viewmatrix = cam.viewmatrix;
+    o.projmatrix = cam.projmatrix;
+    o.campos = cam.campos;
+    o.tan_fovx = cam.tan_fovx;
+    o.tan_fovy = cam.tan_fovy;
+    return o;
+}
+
+struct ViewState {  // one view of a render or backward call: its inputs, instance count and carved states
+    sgb_view_inputs in;
+    int64_t R;
+    GeomView g;
+    BinView b;
+    ImgView im;
+    const float* colors;
+    static ViewState carve(const sgb_view_inputs& shared, const sgb_camera& cam, int64_t num_rendered,
+                           const void* geometry_state, const void* binning_state, const void* image_state) {
+        ViewState w;
+        w.in = with_camera(shared, cam);
+        w.R = w.in.P > 0 ? num_rendered : 0;
+        w.g = GeomView::carve(const_cast<void*>(geometry_state), w.in.P > 0 ? w.in.P : 1);
+        w.b = BinView::carve(const_cast<void*>(binning_state), w.R);
+        w.im = ImgView::carve(const_cast<void*>(image_state), w.in.W, w.in.H);
+        w.colors = w.in.colors_precomp ? w.in.colors_precomp : w.g.rgb;  // rasterizer_impl.cu:324
+        return w;
+    }
+};
+
 // ------------------------------------------------------------------ scratch context
 struct Scratch {
     void* p = nullptr;
@@ -119,10 +150,9 @@ struct Profiler {
 }  // namespace sgb
 
 namespace sgb {
-constexpr int kMaxBatch = 8;  // views per batched call == weight-pool slots kept per ctx
 constexpr int kNumSMs = 132;  // H100 SXM: sizes the grids of the grid-stride kernels
 
-// One weight pool (blend_v3.cu) = the per-tile alpha*T rows of ONE view.  A ctx keeps up to kMaxBatch of them so
+// One weight pool (blend_v3.cu) = the per-tile alpha*T rows of ONE view.  A ctx keeps SGB_MAX_BATCH of them so
 // that the backward of each view of a batch (or of a forward-forward-...-backward-backward sequence) finds the
 // rows its forward built.  A slot is identified by the view's binning-state pointer: a new forward through the
 // same pointer necessarily overwrites that slot, so a slot can never describe a different view's instance list.
@@ -146,7 +176,10 @@ struct sgb_ctx {
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
     sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
-    sgb::PoolSlot pools[sgb::kMaxBatch];  // per-tile weight rows of the C-channel blend (blend_v3.cu)
+    // Per-tile weight rows of the C-channel blend (blend_v3.cu).  As many slots as views per batch: the backward
+    // resolves the rows of all V views before its first kernel, and V <= slots guarantees that rebuilding one view
+    // cannot evict another view of the same batch.
+    sgb::PoolSlot pools[SGB_MAX_BATCH];
     uint64_t pool_clock = 0;
     uint64_t pool_chunks_hint = 0;  // high-water mark of the pool demand (chunks)
     int64_t* pinned = nullptr;  // host-pinned readback slots (1 KB)
@@ -156,8 +189,8 @@ struct sgb_ctx {
     // cached layout of the last sgb_forward_geometry[_batch] call (consumed by sgb_forward_render[_batch])
     int64_t last_P = 0;
     int last_V = 0;
-    uint32_t* d_perm[sgb::kMaxBatch] = {};     // [P] Gaussian ids in (depth bits, id) order, per view of the batch
-    uint32_t* d_offsets[sgb::kMaxBatch] = {};  // [P] inclusive scan of tiles_touched in that order
+    uint32_t* d_perm[SGB_MAX_BATCH] = {};     // [P] Gaussian ids in (depth bits, id) order, per view of the batch
+    uint32_t* d_offsets[SGB_MAX_BATCH] = {};  // [P] inclusive scan of tiles_touched in that order
 };
 
 namespace sgb {
@@ -194,8 +227,8 @@ struct DeviceOnce {
 int launch_preprocess(const sgb_view_inputs& in, GeomView g, int32_t* radii, uint32_t* depth_keys,
                       cudaStream_t s);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t s);
-// Depth order + scan of V views of the same Gaussians (cams[v] replaces the camera fields of `in`; V = 1 with
-// cams = nullptr is the single-view call): everything is enqueued back to back, ONE stream sync reads all R.
+// Depth order + scan of V views of the same Gaussians (cams[v] replaces the camera fields of `in`): everything is
+// enqueued back to back, ONE stream sync reads all R.
 int run_depth_order_and_scan(sgb_ctx* ctx, const sgb_view_inputs& in, int V, const sgb_camera* cams,
                              void* const* geometry_states, int32_t* const* radii, int64_t* R_host, cudaStream_t s);
 int reserve_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, cudaStream_t s);
@@ -206,23 +239,25 @@ int launch_blend_forward(const sgb_view_inputs& in, GeomView g, BinView b, ImgVi
 int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
                           const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
                           float* dL_dcolors, cudaStream_t s);
-// C > 4 forward blend of one view, split so that a batch can enqueue the alpha passes of all its views before the
-// one stream sync that validates their weight pools:
-//   alpha    alpha pass into a weight-pool slot (no sync; pool header -> pinned slot `view_slot`)
-//   finish   after the stream was synchronised: 0 = slot valid, 1 = the pool overflowed (slot grown: alpha again)
-//   gemm     forward GEMM from the validated slot
-int blend_forward_v3_alpha(sgb_ctx* ctx, int view_slot, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b,
-                           ImgView im, cudaStream_t s);
-int blend_forward_v3_finish(sgb_ctx* ctx, int view_slot, const sgb_view_inputs& in, int64_t R, BinView b);
-int blend_forward_v3_gemm(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, BinView b, ImgView im,
-                          const float* colors, float* out_color, cudaStream_t s);
-// backward of one view in two halves (a batch runs all dL/dfeature kernels first, records the feature-gradient
-// event, then the chain kernels): `prepare` finds or rebuilds the view's weight rows.
-int blend_backward_v3_dfeature(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
-                               const float* dL_dpix, float* dL_dcolors, cudaStream_t s);
-int blend_backward_v3_chain(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
-                            const float* colors, const float* dL_dpix, float* dL_dmean2D, float* dL_dconic,
-                            float* dL_dopacity, cudaStream_t s);
+struct PoolView;
+// C > 4 blend.  The weight pool of a view (blend_pool.cuh) is built by its alpha pass; blend_v3.cu owns the slots:
+//   weight_pool_build         enqueue the alpha pass of one view into its slot (no sync), so that a batch enqueues
+//                             the alpha passes of all its views before the one sync that checks their pools
+//   weight_pool_settle        one stream sync, then the pool check of views [0, V) (of those with only[v], when
+//                             given); a view whose pool overflowed is grown and built again; fills pv[v]
+//   weight_rows_for_backward  pv[v] of every view with R > 0: the slot its forward filled, else rebuilt (all misses
+//                             under one sync)
+// The blend kernels take the PoolView and look up nothing.  A batched backward runs all dL/dfeature kernels first,
+// records the feature-gradient event, then the chain kernels.
+int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s);
+int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s,
+                       const bool* only = nullptr);
+int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s);
+int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s);
+int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+                               float* dL_dcolors, cudaStream_t s);
+int blend_backward_v3_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+                            float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, cudaStream_t s);
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,
                          const float* dL_dcolor_rgb, const sgb_view_grads& gr, cudaStream_t s);
 
