@@ -277,6 +277,31 @@ int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const floa
                        float* out, void* stream);
 int sgb_label_argmax(int32_t K, int32_t first_class, int64_t N, const float* planes, int64_t* label, void* stream);
 
+/* ---- segmentation confusion matrix: the counting of utils/metric.py::confusion_matrix, on the device.
+ *
+ * sgb_confusion_accumulate adds N (prediction, ground truth) pairs into counts, a full (nb, nb) row-major uint64
+ * histogram with nb = num_classes + 1 (rows: prediction, columns: ground truth; the caller drops column 0 as the
+ * reference does).  For every p:
+ *     pr  = pred[p] + pred_offset                 (the reference's `label += 1` is pred_offset = 1)
+ *     g   = gt[p]
+ *     bin = pr * nb + g                           (exact, 64-bit)
+ *     pr < 0 or g < 0 or bin >= nb * nb  ->  *invalid += 1
+ *     otherwise                          ->  counts[bin] += 1
+ * The reference raises on a view with such a pair (negative bincount input, failed reshape).  The exceptions are a
+ * negative g whose flat bin stays >= 0 and labels near 2^63 whose int64 sum wraps into range: numpy silently counts
+ * those in the wrong cell, and they are invalid here (pr and bin are exact).
+ * The upper test is on the flat index, as np.bincount + reshape do: a g > num_classes whose bin still fits counts
+ * in the next row.  counts and invalid accumulate across calls; the call never zeroes them.
+ * pred: SGB_LABEL_I32 or SGB_LABEL_I64; gt: SGB_LABEL_U8, SGB_LABEL_I32 or SGB_LABEL_I64.  pred / gt may have any
+ * alignment (views into larger tensors).  1 <= num_classes <= 225: (num_classes + 1)^2 uint32 bins must fit one
+ * CTA's shared memory.  Enqueued on `stream`, no host synchronisation, no ctx.  N == 0 launches nothing. */
+#define SGB_LABEL_U8 0
+#define SGB_LABEL_I32 1
+#define SGB_LABEL_I64 2
+int sgb_confusion_accumulate(int64_t N, const void* pred, int32_t pred_dtype, const void* gt, int32_t gt_dtype,
+                             int32_t pred_offset, int32_t num_classes, uint64_t* counts, uint32_t* invalid,
+                             void* stream);
+
 /* ---- 3-nearest-neighbour mean squared distance: `distCUDA2` of the reference's
  * simple-knn extension (submodules/simple-knn/simple_knn.cu:185-220, spatial.cu), used by
  * GaussianModel.create_from_pcd (model/gaussian_model.py:150-186).  points (P,3) fp32 device, mean_dist2 (P) fp32

@@ -65,7 +65,7 @@ EXPORTS = (
     "sgb_profile_num_stages", "sgb_profile_stage_name", "sgb_ctx_launch_count",
     "sgb_ctx_set_feature_grad_event", "sgb_semantic_head", "sgb_feature_logits", "sgb_label_argmax", "sgb_ctx_view_stat", "sgb_knn_mean_dist2", "sgb_distill_loss",
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
-    "sgb_photometric_forward", "sgb_photometric_backward",
+    "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate",
 )
 
 _lib = None
@@ -133,6 +133,7 @@ def load() -> C.CDLL:
         lib.sgb_label_argmax.argtypes = [i32, i32, i64, vp, vp, vp]
         lib.sgb_photometric_forward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp]
         lib.sgb_photometric_backward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp, i64, i64, vp]
+        lib.sgb_confusion_accumulate.argtypes = [i64, vp, i32, vp, i32, i32, i32, vp, vp, vp]
         _lib = lib
         return lib
 
