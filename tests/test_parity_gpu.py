@@ -12,6 +12,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+from test_blend_fp64_gpu import FRAGILE_MAX as FP64_FRAGILE_MAX, check_views  # noqa: E402
 from util import RefRecord, dev_cam, dev_scene, frac_bad, ours_state, run_ours  # noqa: E402
 
 from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras  # noqa: E402
@@ -326,6 +327,11 @@ def test_channel_forward_and_backward_above_65535_tiles():
         lhs = float((g.double() * sd["features"].double()).sum())
         rhs = float(((o["color"].detach() - o0).double() * dL.double()).sum())
     assert abs(lhs - rhs) <= 1e-4 * abs(rhs) + 1e-6
+    # every blend gradient against the float64 restatement, with dL/dout in tile rows 254-256 only: tile row 255
+    # starts at tile id 255 * 257 = 65535, so those ~770 tiles straddle the 16-bit boundary
+    res = check_views(scene, [cam], bg.cpu().numpy(), tile_rows=(254, 257))
+    assert res["fragile"] <= FP64_FRAGILE_MAX, res["fragile"]
+    assert all(e <= 1.0 for e in res["errs"].values()), res["errs"]
 
 
 @pytest.mark.parametrize("C,W,H", [(6, 250, 100), (5, 333, 211), (36, 641, 479)])
