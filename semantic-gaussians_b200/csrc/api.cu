@@ -371,6 +371,16 @@ int sgb_backward_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const
         set_error("sgb_backward_batch: null argument");
         return SGB_E_INVALID;
     }
+    // with SH colours the geometry kernel of view v reads dL_dcolors as view v's RGB gradient, after view v's blend
+    // has added into it: a buffer shared with an earlier view would carry that view's gradient too
+    if (in->shs)
+        for (int v = 1; v < V; v++)
+            for (int u = 0; u < v; u++)
+                if (grads[v].dL_dcolors == grads[u].dL_dcolors) {
+                    set_error("sgb_backward_batch: views %d and %d share one dL_dcolors buffer; with shs every view "
+                              "needs its own dL_dcolors", u, v);
+                    return SGB_E_INVALID;
+                }
     return backward_impl(ctx, *in, V, cams, num_rendered, radii, geometry_states, binning_states, image_states, dL_dpix,
                          grads, (cudaStream_t)stream);
 }

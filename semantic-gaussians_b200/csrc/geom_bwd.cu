@@ -60,7 +60,9 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
         geomgrad::factor_grad(g_cov, q, s, g_s, g_q);
 #pragma unroll
         for (int i = 0; i < 3; i++) dL_dscale[3 * g + i] = g_s[i];
-        *reinterpret_cast<float4*>(dL_drot + 4 * g) = make_float4(g_q[0], g_q[1], g_q[2], g_q[3]);
+        // scalar stores: dL_drot may be any 4-byte-aligned view, as the other per-Gaussian buffers
+#pragma unroll
+        for (int i = 0; i < 4; i++) dL_drot[4 * g + i] = g_q[i];
     }
 }
 

@@ -97,7 +97,7 @@ __device__ V3 computeColorFromSH(int idx, int deg, int max_coeffs, const float* 
 
 __global__ void __launch_bounds__(256) preprocess_kernel(
     int P, int D, int M, const float* __restrict__ orig_points, const float3* __restrict__ scales,
-    const float scale_modifier, const float4* __restrict__ rotations, const float* __restrict__ opacities,
+    const float scale_modifier, const float* __restrict__ rotations, const float* __restrict__ opacities,
     const float* __restrict__ shs, uint8_t* __restrict__ clamped, const float* __restrict__ cov3D_precomp,
     const float* __restrict__ colors_precomp, const float* __restrict__ viewmatrix,
     const float* __restrict__ projmatrix, const float* __restrict__ cam_pos, const int W, int H,
@@ -130,7 +130,9 @@ __global__ void __launch_bounds__(256) preprocess_kernel(
     if (cov3D_precomp != nullptr) {
         cov3D = cov3D_precomp + (size_t)idx * 6;
     } else {
-        computeCov3D(scales[idx], scale_modifier, rotations[idx], cov3Ds + (size_t)idx * 6);
+        // scalar loads: the caller's rotations may be any 4-byte-aligned view (e.g. into a flat parameter buffer)
+        const float* q = rotations + (size_t)idx * 4;
+        computeCov3D(scales[idx], scale_modifier, make_float4(q[0], q[1], q[2], q[3]), cov3Ds + (size_t)idx * 6);
         cov3D = cov3Ds + (size_t)idx * 6;
     }
 
@@ -192,7 +194,7 @@ int launch_preprocess(const sgb_view_inputs& in, GeomView g, int32_t* radii, uin
     const float focal_x = in.W / (2.0f * in.tan_fovx);
     dim3 tile_grid((in.W + SGB_TILE - 1) / SGB_TILE, (in.H + SGB_TILE - 1) / SGB_TILE, 1);
     preprocess_kernel<<<(in.P + 255) / 256, 256, 0, s>>>(
-        in.P, in.D, in.M, in.means3D, (const float3*)in.scales, in.scale_modifier, (const float4*)in.rotations,
+        in.P, in.D, in.M, in.means3D, (const float3*)in.scales, in.scale_modifier, in.rotations,
         in.opacities, in.shs, g.clamped, in.cov3D_precomp, in.colors_precomp, in.viewmatrix, in.projmatrix,
         in.campos, in.W, in.H, in.tan_fovx, in.tan_fovy, focal_x, focal_y, radii, g.rec, g.cov3D, g.rgb, tile_grid,
         g.tiles_touched, depth_keys, in.prefiltered != 0);

@@ -91,3 +91,19 @@ def test_missing_library_is_an_import_error(monkeypatch, tmp_path):
     monkeypatch.setattr(_lib, "LIB_PATH", str(tmp_path / "libsgb200.so"))
     with pytest.raises(ImportError, match="no CPU fallback"):
         _lib.load()
+
+
+def test_shared_dcolors_with_sh_is_rejected_before_cuda():
+    """With shs, every view of sgb_backward_batch needs its own dL_dcolors: the geometry kernel of view v reads it as
+    view v's RGB gradient after view v's blend added into it.  A shared buffer is refused during argument checking
+    (no ctx is dereferenced and no CUDA call is made, so this runs without a GPU)."""
+    lib = _lib.load()
+    V = 3
+    inp = _inputs(colors_precomp=None, shs=1, M=16, D=3)
+    cams = (_lib.Camera * V)(*[_lib.Camera(1, 1, 1, 0.5, 0.5) for _ in range(V)])
+    arr = (C.c_void_p * V)(*[1] * V)
+    R = (C.c_int64 * V)(*[1] * V)
+    grads = (_lib.ViewGrads * V)(*[_lib.ViewGrads(*[1, 1, 1, 42, 1, 1, 1, 1, 1]) for _ in range(V)])
+    rc = lib.sgb_backward_batch(1, C.byref(inp), V, cams, R, arr, arr, arr, arr, arr, grads, None)
+    assert rc == -1
+    assert b"dL_dcolors" in lib.sgb_last_error()

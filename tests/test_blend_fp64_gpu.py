@@ -22,8 +22,8 @@ Which case reaches which branch (C <= 4: blend_fwd.cu / blend_bwd.cu; C > 4: ble
   calibration ................ the configurations test_parity_gpu.py::test_backward_vs_reference pins to the
                                compiled reference
 test_parity_gpu.py::test_channel_forward_and_backward_above_65535_tiles checks tile rows 254-256 of a 257 x 257
-tile image (tile ids across 65535) with check_views() below."""
-import ctypes as Ct
+tile image (tile ids across 65535) with check_views() (tests/raster_check.py), which
+also checks every view's geometry stage against tests/geom_ref.py."""
 import os
 import sys
 import time
@@ -33,159 +33,15 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import blend_ref as br  # noqa: E402
-from util import dev_cam, dev_scene  # noqa: E402
+from raster_check import assert_ok as _assert_ok, check_views, report  # noqa: E402
 
-from semantic_gaussians_b200 import _lib  # noqa: E402
 from semantic_gaussians_b200.scene_synth import look_at_camera, make_scene, orbit_cameras  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-FRAGILE_MAX = 0.02   # at most this fraction of pixels may be left out of the comparison
-DEV = torch.device("cuda:0")
-
-
-def read_state(lib, P, R, W, H, geom, binning, img):
-    """The blend's inputs and forward state of one view, as the kernels left them."""
-    tiles = ((W + 15) // 16) * ((H + 15) // 16)
-    spec = dict(means2D=(torch.float32, (P, 2)), conic_opacity=(torch.float32, (P, 4)),
-                point_list=(torch.int32, (max(R, 1),)), ranges=(torch.int32, (tiles, 2)),
-                n_contrib=(torch.int32, (H * W,)), final_T=(torch.float32, (H * W,)))
-    st = {}
-    for name, (dt, shape) in spec.items():
-        t = torch.zeros(shape, dtype=dt, device=DEV)
-        n = lib.sgb_state_field(name.encode(), P, R, W, H, geom.data_ptr(), binning.data_ptr(), img.data_ptr(),
-                                t.data_ptr(), torch.cuda.current_stream(DEV).cuda_stream)
-        assert n >= 0, lib.sgb_last_error()
-        st[name] = t[:R] if name == "point_list" else t
-    return st
-
-
-def _placed(t, offset):
-    """A copy of t whose data pointer is `offset` bytes past a 16-byte boundary (the C ABI takes any pointer)."""
-    buf = torch.zeros(t.numel() + 4, dtype=t.dtype, device=t.device)
-    v = buf[offset // 4: offset // 4 + t.numel()].view(t.shape)
-    v.copy_(t)
-    assert v.data_ptr() % 16 == offset
-    return v
-
-
-def check_views(scene, cams, bg, *, dl_offset=0, feat_offset=0, dcolors_offset=0, tile_rows=None, seed=0):
-    """Forward and backward of len(cams) views of `scene` (features as colors_precomp) in one sgb_*_batch call
-    sequence on a fresh ctx, each view checked against the float64 restatement on its own state; dL/dout is
-    random, zero at fragile pixels and, with tile_rows, outside those tile rows.  Returns per-case statistics:
-    compare() of every output (<= 1 passes), fragile fraction, list lengths and the weight-pool chunks."""
-    lib = _lib.load()
-    W, H = cams[0].image_width, cams[0].image_height
-    P, Cn = scene.features.shape
-    V = len(cams)
-    sc = dev_scene(scene, DEV)
-    feats = _placed(sc["features"], feat_offset)
-    bg = torch.as_tensor(bg, dtype=torch.float32, device=DEV)
-    cms = [dev_cam(c, DEV) for c in cams]
-    inp = _lib.ViewInputs(
-        P=P, D=0, M=0, W=W, H=H, C=Cn, background=bg.data_ptr(), means3D=sc["means3D"].data_ptr(), shs=None,
-        colors_precomp=feats.data_ptr(), opacities=sc["opacities"].data_ptr(), scales=sc["scales"].data_ptr(),
-        scale_modifier=1.0, rotations=sc["rotations"].data_ptr(), cov3D_precomp=None, viewmatrix=None,
-        projmatrix=None, campos=None, tan_fovx=0.0, tan_fovy=0.0, prefiltered=0, debug=0)
-    cam_arr = (_lib.Camera * V)(*[_lib.Camera(c["viewmatrix"].data_ptr(), c["projmatrix"].data_ptr(),
-                                              c["campos"].data_ptr(), c["tanfovx"], c["tanfovy"]) for c in cms])
-    ptrs = lambda ts: (Ct.c_void_p * V)(*[t.data_ptr() for t in ts])
-    u8 = dict(dtype=torch.uint8, device=DEV)
-    stream = torch.cuda.current_stream(DEV).cuda_stream
-    ctx = Ct.c_void_p()
-    _lib.check(lib.sgb_ctx_create(Ct.byref(ctx), DEV.index), "sgb_ctx_create")
-    try:
-        radii = [torch.empty((P,), dtype=torch.int32, device=DEV) for _ in cams]
-        geom = [torch.empty((lib.sgb_geometry_bytes(P),), **u8) for _ in cams]
-        img = [torch.empty((lib.sgb_image_bytes(W, H),), **u8) for _ in cams]
-        Rs = (Ct.c_int64 * V)()
-        _lib.check(lib.sgb_forward_geometry_batch(ctx, Ct.byref(inp), V, cam_arr, ptrs(geom), ptrs(radii), Rs, stream),
-                   "sgb_forward_geometry_batch")
-        binning = [torch.empty((lib.sgb_binning_bytes(R),), **u8) for R in Rs]
-        color = [torch.empty((Cn, H, W), device=DEV) for _ in cams]
-        _lib.check(lib.sgb_forward_render_batch(ctx, Ct.byref(inp), V, cam_arr, Rs, ptrs(geom), ptrs(binning),
-                                                ptrs(img), ptrs(radii), ptrs(color), None, stream),
-                   "sgb_forward_render_batch")
-        chunks = lib.sgb_ctx_view_stat(ctx, 1)
-
-        # the float64 forward of every view on the kernel's own state; dL/dout from it
-        g = torch.Generator(device=DEV).manual_seed(seed)
-        views, dLs = [], []
-        for v in range(V):
-            R = Rs[v]
-            if R == 0:
-                views.append(None)
-                dLs.append(torch.randn((Cn, H, W), device=DEV, generator=g))
-                continue
-            st = read_state(lib, P, R, W, H, geom[v], binning[v], img[v])
-            args = (st["means2D"], st["conic_opacity"], st["point_list"], st["ranges"], sc["features"], bg, W, H)
-            want = br.blend_forward(*args, tile_rows=tile_rows)
-            dL = torch.randn((Cn, H * W), device=DEV, generator=g)
-            dL[:, want["fragile"]] = 0.0
-            if tile_rows is not None:
-                dL[:, :tile_rows[0] * 16 * W] = 0.0
-                dL[:, tile_rows[1] * 16 * W:] = 0.0
-            views.append((st, args, want))
-            dLs.append(dL.reshape(Cn, H, W))
-        dL_in = [_placed(d, dl_offset) for d in dLs]
-        z = lambda *s: torch.zeros(s, device=DEV)
-        dcolors = _placed(z(P, Cn), dcolors_offset)
-        grads = [dict(dL_dmeans2D=z(P, 3), dL_dconic=z(P, 4), dL_dopacity=z(P), dL_dcolors=dcolors,
-                      dL_dmeans3D=z(P, 3), dL_dcov3D=z(P, 6), dL_dscales=z(P, 3), dL_drotations=z(P, 4))
-                 for _ in cams]
-        gr = (_lib.ViewGrads * V)(*[_lib.ViewGrads(dL_dsh=None, **{k: t.data_ptr() for k, t in gv.items()})
-                                    for gv in grads])
-        _lib.check(lib.sgb_backward_batch(ctx, Ct.byref(inp), V, cam_arr, Rs, ptrs(radii), ptrs(geom), ptrs(binning),
-                                          ptrs(img), ptrs(dL_in), gr, stream), "sgb_backward_batch")
-    finally:
-        torch.cuda.synchronize(DEV)
-        lib.sgb_ctx_destroy(ctx)
-
-    errs = {}
-    frag, lens = [], []
-    want_colors = torch.zeros((P, Cn), dtype=torch.float64, device=DEV)
-    for v in range(V):
-        if views[v] is None:   # nothing in view: the image is the background, no gradient
-            assert torch.equal(color[v], bg[:, None, None].expand(Cn, H, W))
-            for name in ("dL_dmeans2D", "dL_dconic", "dL_dopacity"):
-                assert float(grads[v][name].abs().max()) == 0.0, name
-            continue
-        st, args, want = views[v]
-        wb = br.blend_backward(*args, dLs[v], tile_rows=tile_rows)
-        want_colors += wb["dL_dcolors"]
-        fragile = want["fragile"]
-        ok = ~fragile
-        if tile_rows is not None:
-            ok[:tile_rows[0] * 16 * W] = False
-            ok[tile_rows[1] * 16 * W:] = False
-        frag.append(float(fragile[ok | fragile].double().mean()))
-        assert torch.equal(st["n_contrib"][ok].long(), want["n_contrib"][ok]), v
-        got_grads = {k: grads[v][k] for k in ("dL_dmeans2D", "dL_dconic", "dL_dopacity")}
-        got_grads["dL_dcolors"] = wb["dL_dcolors"]   # the shared buffer is checked against the sum below
-        e = dict(final_T=br.compare(st["final_T"][ok], want["final_T"][ok]),
-                 color=br.compare(color[v].reshape(Cn, -1)[:, ok], want["color"].reshape(Cn, -1)[:, ok]))
-        e.update({k: x for k, x in br.grad_errors(got_grads, wb).items() if k != "dL_dcolors"})
-        for k, x in e.items():
-            errs[k] = max(errs.get(k, 0.0), x)
-        for name in ("dL_dmeans2D", "dL_dconic", "dL_dopacity"):
-            assert float(wb[name].abs().max()) > 0, name
-        rg = st["ranges"].long()
-        lens.append(rg[:, 1] - rg[:, 0])
-    errs["dL_dcolors"] = br.compare(dcolors, want_colors)
-    assert float(want_colors.abs().max()) > 0
-    return dict(errs=errs, fragile=max(frag), lens=torch.cat(lens).cpu(), chunks=chunks,
-                n_contrib=views[0][0]["n_contrib"].cpu() if views[0] else None, W=W, H=H)
-
 
 def _report(name, res, t0):
-    e = " ".join(f"{k}={v:.3g}" for k, v in res["errs"].items())
-    print(f"\n[fp64 blend] {name}: fragile={res['fragile']:.4%} {e} ({time.time() - t0:.1f} s)")
-
-
-def _assert_ok(res):
-    assert res["fragile"] <= FRAGILE_MAX, res["fragile"]
-    assert all(v <= 1.0 for v in res["errs"].values()), res["errs"]
+    report("blend", name, res, t0)
 
 
 BG_RAMP = "ramp"

@@ -12,7 +12,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from test_blend_fp64_gpu import FRAGILE_MAX as FP64_FRAGILE_MAX, check_views  # noqa: E402
+from raster_check import FRAGILE_MAX as FP64_FRAGILE_MAX, check_views  # noqa: E402
 from util import RefRecord, dev_cam, dev_scene, frac_bad, ours_state, run_ours  # noqa: E402
 
 from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras  # noqa: E402

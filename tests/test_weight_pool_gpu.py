@@ -12,7 +12,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import blend_ref as br  # noqa: E402
 from test_batch_gpu import Pipe, _cams, _grads, _model  # noqa: E402
-from test_blend_fp64_gpu import FRAGILE_MAX, read_state  # noqa: E402
+from raster_check import FRAGILE_MAX, read_state  # noqa: E402
 from util import dev_cam, dev_scene, frac_bad  # noqa: E402
 
 from semantic_gaussians_b200 import _lib  # noqa: E402
