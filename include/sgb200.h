@@ -275,6 +275,25 @@ int sgb_fusion_normalize(int32_t P, int32_t C, float* feat_sum, float* count, vo
  * loss: TWO doubles on the device (zeroed by the call): [0] the loss, [1] Nv. */
 int sgb_distill_loss(int32_t C, int32_t K, int64_t N, const float* render, const float* class_emb, const void* labels,
                      int32_t labels_are_int64, float* dL_drender, double* loss, void* stream);
+/* Distillation loss of a rendered feature image against a 2D model's feature map (distill.py:111-124) and its
+ * gradient.  render / dL_drender (C, N) planar fp32, target (C, N) planar, SGB_FEAT_F16 or SGB_FEAT_F32; pixel p is
+ * the row x_p = render[:, p], y_p = target[:, p] (converted to fp32):
+ *     SGB_FEATLOSS_COSINE  loss = (1 / Nv) sum_{p valid} (1 - cos_p),  cos_p = x_p.y_p / (max(|x_p|, 1e-8) max(|y_p|, 1e-8))
+ *                          (torch.nn.CosineSimilarity), dL_drender its torch autograd gradient on valid pixels and
+ *                          0 elsewhere.  Valid: y_p has a non-zero element; Nv = the number of valid pixels.
+ *                          Nv = 0 gives loss 0 and an all-zero gradient.
+ *     SGB_FEATLOSS_L1      loss = (1 / (N C)) sum |x - y|,     dL_drender = sign(x - y) / (N C), sign(0) = 0
+ *     SGB_FEATLOSS_L2      loss = (1 / (N C)) sum (x - y)^2,   dL_drender = 2 (x - y) / (N C)
+ * loss: TWO doubles on the device (zeroed by the call): [0] the loss, [1] the pixels the mean runs over (Nv for
+ * cosine, N for l1 / l2), so a caller can skip an empty step without a host sync.  1 <= C <= 1024.  Each input is
+ * read once and dL_drender written once.  Asynchronous on `stream`, no host copy, no ctx; N == 0 only zeroes loss. */
+#define SGB_FEATLOSS_COSINE 0
+#define SGB_FEATLOSS_L1 1
+#define SGB_FEATLOSS_L2 2
+int sgb_feature_map_loss(int32_t C, int64_t N, const float* render, const void* target,
+                         int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type,
+                         float* dL_drender, double* loss /* [2] device: loss, Nv; zeroed by the call */,
+                         void* stream);
 int sgb_semantic_head(sgb_ctx* ctx, int32_t C, int32_t K, int64_t N, const float* render, const float* text,
                       int32_t first_class, float* sim, int64_t* label, void* stream);
 int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const float* features, const float* text,

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libsgb200.so")
 SGB_OK = 0
 DEPTH_NONE, DEPTH_F32, DEPTH_F64, DEPTH_SURFACE = 0, 1, 2, 3
 FEAT_F16, FEAT_F32 = 0, 1
+FEATLOSS_COSINE, FEATLOSS_L1, FEATLOSS_L2 = 0, 1, 2
 
 
 class SgbError(RuntimeError):
@@ -65,7 +66,7 @@ EXPORTS = (
     "sgb_profile_num_stages", "sgb_profile_stage_name", "sgb_ctx_launch_count",
     "sgb_ctx_set_feature_grad_event", "sgb_semantic_head", "sgb_feature_logits", "sgb_label_argmax", "sgb_ctx_view_stat", "sgb_knn_mean_dist2", "sgb_distill_loss",
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
-    "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate",
+    "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
 )
 
 _lib = None
@@ -134,6 +135,7 @@ def load() -> C.CDLL:
         lib.sgb_photometric_forward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp]
         lib.sgb_photometric_backward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp, i64, i64, vp]
         lib.sgb_confusion_accumulate.argtypes = [i64, vp, i32, vp, i32, i32, i32, vp, vp, vp]
+        lib.sgb_feature_map_loss.argtypes = [i32, i64, vp, vp, i32, i32, vp, vp, vp]
         _lib = lib
         return lib
 

@@ -29,7 +29,6 @@
 // adds its Gaussians in depth order.
 #include <cstddef>
 #include <cstring>
-#include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include "common.cuh"
 #include "blend_pool.cuh"
 
@@ -1369,22 +1368,6 @@ int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float
     }
     SGB_LAUNCH_CHECK("blend_forward kernel", in.debug, s);
     return SGB_OK;
-}
-
-using TensorMapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link); nullptr when unavailable.
-static TensorMapEncodeFn tensor_map_encoder() {
-    static const TensorMapEncodeFn encode = [] {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            fn = nullptr;
-        return (TensorMapEncodeFn)fn;
-    }();
-    return encode;
 }
 
 // dL/dout (C, H, W) fp32 for dfeature_persistent_kernel, described with its dimensions in the order (x, channel, y) so

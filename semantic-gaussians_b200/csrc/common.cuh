@@ -2,6 +2,7 @@
 #pragma once
 #include <cstdint>
 #include <cstdio>
+#include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
 #include "../../include/sgb200.h"
 
@@ -222,6 +223,22 @@ struct DeviceOnce {
         return true;
     }
 };
+
+using TensorMapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link); nullptr when unavailable.
+inline TensorMapEncodeFn tensor_map_encoder() {
+    static const TensorMapEncodeFn encode = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return (TensorMapEncodeFn)fn;
+    }();
+    return encode;
+}
 
 // ------------------------------------------------------------------ stage launchers
 int launch_preprocess(const sgb_view_inputs& in, GeomView g, int32_t* radii, uint32_t* depth_keys,

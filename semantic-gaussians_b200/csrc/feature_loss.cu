@@ -1,0 +1,342 @@
+// Feature-map distillation loss of a rendered (C, H, W) feature image against a 2D model's feature map of the same
+// shape (fp16 or fp32), and its gradient, in the three forms of the reference's distill.py:111-124:
+//
+//   cosine   (1 / Nv) sum_{p valid} (1 - cos_p),  cos_p = x_p.y_p / (max(|x_p|, 1e-8) max(|y_p|, 1e-8))
+//            (torch.nn.CosineSimilarity(eps=1e-8): each norm clamped separately; valid = y_p has a non-zero element)
+//   l1       (1 / (N C)) sum |x - y|          (torch.nn.L1Loss)
+//   l2       (1 / (N C)) sum (x - y)^2        (torch.nn.MSELoss)
+//
+// Each input is read once and the gradient written once.  l1 / l2 are elementwise over the N*C values (16-byte
+// loads where the layout allows).  cosine needs three reductions over C per pixel (x.y, |x|^2, |y|^2) before any
+// gradient element of that pixel can be written, and both images are planar with plane stride N: a CTA owns a
+// block of PB pixels and stages their full C-long columns of render and target in shared memory (a TMA tensor copy
+// of a (channels x PB) box, or plain loads when the layout does not meet the TMA rules), reduces per pixel and
+// writes the gradient from the staged copy.  The normaliser 1/Nv is global, so a small pre-pass counts the valid
+// pixels into loss[1] (a pixel's column is read only up to its first non-zero channel: about one plane on real
+// feature maps) and the main kernel reads it from device memory in stream order.
+//
+// H100 80GB HBM3 at 700 W, 256 x 1080 x 1920, fp16 target (tools/time_feature_loss.py): count 0.08 ms + cosine
+// kernel 1.94 ms; l1 / l2 kernel 1.85 ms (2.9 TB/s over the 5.3 GB that must move).
+#include <algorithm>
+#include <cstring>
+#include <cuda_fp16.h>
+
+#include "common.cuh"
+
+namespace sgb {
+namespace {
+
+constexpr int kFlThreads = 256;
+constexpr int kFlMaxC = 1024;              // widest feature map accepted (OpenSeg 768, LSeg 512)
+constexpr int kFlMaxBox = 256;             // TMA box limit per dimension
+constexpr size_t kFlStageTarget = 48 * 1024;  // staged bytes per CTA aimed at: four CTAs per SM
+
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+
+// 2-D tensor tile global -> shared (SASS: UTMALDG): box corner (x, y) in elements, out-of-range elements arrive as
+// zeros; completion is signalled on `bar` as the box's bytes.
+__device__ __forceinline__ void tma_tile2d_g2s(void* dst_smem, const CUtensorMap* map, int x, int y, uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+            smem_u32(dst_smem)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
+        : "memory");
+}
+
+// loss[1] = number of pixels whose target column has a non-zero element (features_gt.norm(dim=-1) > 0).  Thread =
+// one pixel.  Channel 0 decides almost every pixel of a real feature map; the rest of a column is read in groups of
+// kCountGroup independent loads, so an all-zero column costs C / kCountGroup dependent memory round trips, not C.
+constexpr int kCountGroup = 16;
+template <typename T>
+__global__ void __launch_bounds__(256) count_valid_pixels_kernel(int C, long long N, const T* __restrict__ y,
+                                                                 double* __restrict__ valid) {
+    __shared__ int wn[8];
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    int nz = 0;
+    if (p < N) {
+        nz = to_f32(y[p]) != 0.f;
+        for (int c0 = 1; !nz && c0 < C; c0 += kCountGroup) {
+            float v[kCountGroup];
+#pragma unroll
+            for (int j = 0; j < kCountGroup; j++) v[j] = c0 + j < C ? to_f32(y[(size_t)(c0 + j) * N + p]) : 0.f;
+#pragma unroll
+            for (int j = 0; j < kCountGroup; j++) nz |= v[j] != 0.f;
+        }
+    }
+    const int n = __reduce_add_sync(0xffffffffu, nz);
+    if ((threadIdx.x & 31) == 0) wn[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int w = 0; w < 8; w++) t += wn[w];
+        if (t) atomicAdd(valid, (double)t);
+    }
+}
+
+// Cosine loss: CTA = PB = 2^pb_log2 consecutive pixels.  Shared memory holds Xs [Cs][PB] fp32 and, 128-byte aligned
+// after it, Ys [Cs][PB] of the target type, Cs = nbox * box_c >= C (rows past C arrive as zeros and are not read).
+// Thread t reduces pixel t % PB over channels t / PB, t / PB + G, ... (G = 256 / PB); the G partial sums of a pixel
+// are added in a fixed order, so the gradient is bit-reproducible.
+template <typename T>
+__global__ void __launch_bounds__(kFlThreads) feature_cosine_kernel(int C, long long N, int pb_log2, int box_c, int nbox,
+                                                                    const float* __restrict__ render,
+                                                                    const T* __restrict__ target, float* __restrict__ dL,
+                                                                    double* __restrict__ loss,
+                                                                    const __grid_constant__ CUtensorMap xmap,
+                                                                    const __grid_constant__ CUtensorMap ymap, int use_tma) {
+    extern __shared__ __align__(128) unsigned char fl_smem[];
+    __shared__ uint64_t bar;
+    __shared__ float red[3][kFlThreads];
+    __shared__ int nzs[kFlThreads];
+    __shared__ float coef[2][kFlThreads];
+    __shared__ double wsum[kFlThreads / 32];
+    const int PB = 1 << pb_log2, G = kFlThreads >> pb_log2;
+    const int Cs = nbox * box_c;
+    const size_t ys_off = ((size_t)Cs * PB * sizeof(float) + 127) & ~(size_t)127;
+    float* Xs = reinterpret_cast<float*>(fl_smem);
+    T* Ys = reinterpret_cast<T*>(fl_smem + ys_off);
+    const int tid = threadIdx.x;
+    const long long p0 = (long long)blockIdx.x * PB;
+
+    if (use_tma) {
+        if (tid == 0) {
+            mbar_init(&bar, 1);
+            mbar_fence_init();
+        }
+        __syncthreads();
+        if (tid == 0) {
+            mbar_arrive_expect_tx(&bar, (uint32_t)((size_t)Cs * PB * (sizeof(float) + sizeof(T))));
+            for (int k = 0; k < nbox; k++) {
+                tma_tile2d_g2s(Xs + (size_t)k * box_c * PB, &xmap, (int)p0, k * box_c, &bar);
+                tma_tile2d_g2s(Ys + (size_t)k * box_c * PB, &ymap, (int)p0, k * box_c, &bar);
+            }
+        }
+        mbar_wait(&bar, 0);
+    } else {
+        const int npx = (int)min((long long)PB, N - p0);
+#pragma unroll 4
+        for (int e = tid; e < C * PB; e += kFlThreads) {
+            const int c = e >> pb_log2, p = e & (PB - 1);
+            const size_t o = (size_t)c * N + p0 + p;
+            Xs[e] = p < npx ? __ldg(render + o) : 0.f;
+            Ys[e] = p < npx ? target[o] : T(0.f);
+        }
+        __syncthreads();
+    }
+
+    const int tp = tid & (PB - 1), g = tid >> pb_log2;
+    float dot = 0.f, xx = 0.f, yy = 0.f;
+    int nz = 0;
+    for (int c = g; c < C; c += G) {
+        const float x = Xs[c * PB + tp], y = to_f32(Ys[c * PB + tp]);
+        dot = fmaf(x, y, dot);
+        xx = fmaf(x, x, xx);
+        yy = fmaf(y, y, yy);
+        nz |= y != 0.f;
+    }
+    red[0][tid] = dot;
+    red[1][tid] = xx;
+    red[2][tid] = yy;
+    nzs[tid] = nz;
+    __syncthreads();
+
+    double term = 0.0;
+    if (tid < PB) {
+        float d = 0.f, a2 = 0.f, b2 = 0.f;
+        int any = 0;
+        for (int k = 0; k < G; k++) {
+            d += red[0][k * PB + tid];
+            a2 += red[1][k * PB + tid];
+            b2 += red[2][k * PB + tid];
+            any |= nzs[k * PB + tid];
+        }
+        const double nv = loss[1];
+        const float inv_nv = nv > 0.0 ? (float)(1.0 / nv) : 0.f;
+        const float nx = sqrtf(a2), a = fmaxf(nx, 1e-8f), b = fmaxf(sqrtf(b2), 1e-8f);
+        const float cosv = d / (a * b);
+        const bool valid = any && p0 + tid < N;
+        // d cos / dx = y / (a b) - cos x / (a |x|): the norm's own derivative x / |x| is unclamped (torch clamps the
+        // norms under no_grad), and is zero for x = 0
+        coef[0][tid] = valid ? -inv_nv / (a * b) : 0.f;
+        coef[1][tid] = valid && nx > 0.f ? inv_nv * cosv / (a * nx) : 0.f;
+        term = valid ? 1.0 - (double)cosv : 0.0;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) term += __shfl_xor_sync(0xffffffffu, term, o);
+    if ((tid & 31) == 0) wsum[tid >> 5] = term;
+    __syncthreads();
+    if (tid == 0) {
+        double t = 0.0;
+        for (int w = 0; w < kFlThreads / 32; w++) t += wsum[w];
+        const double nv = loss[1];
+        if (nv > 0.0 && t != 0.0) atomicAdd(loss, t / nv);
+    }
+
+    if (p0 + tp >= N) return;
+    const float u = coef[0][tp], v = coef[1][tp];
+    float* out = dL + p0 + tp;
+    for (int c = g; c < C; c += G) out[(size_t)c * N] = fmaf(u, to_f32(Ys[c * PB + tp]), v * Xs[c * PB + tp]);
+}
+
+struct Quad { float v[4]; };
+__device__ __forceinline__ Quad load4(const float* p) {
+    const float4 q = __ldg(reinterpret_cast<const float4*>(p));
+    return {{q.x, q.y, q.z, q.w}};
+}
+__device__ __forceinline__ Quad load4(const __half* p) {
+    const uint2 r = __ldg(reinterpret_cast<const uint2*>(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
+    return {{a.x, a.y, b.x, b.y}};
+}
+
+// l1 / l2 over the M = N*C values: gradient sign(x - y) / M (sign(0) = 0, as abs()'s backward) or 2 (x - y) / M.
+// VEC: render, target and dL start 16-/8-byte aligned, so the first M - M % 4 values go as 4-wide loads.
+template <typename T, bool L2, bool VEC>
+__global__ void __launch_bounds__(256) feature_elementwise_kernel(long long M, long long N, const float* __restrict__ x,
+                                                                  const T* __restrict__ y, float* __restrict__ dL,
+                                                                  double* __restrict__ loss) {
+    const double inv_m = 1.0 / (double)M;
+    const float gs = (float)((L2 ? 2.0 : 1.0) * inv_m);
+    auto term = [&](float xv, float yv, float& g) {
+        const float d = xv - yv;
+        g = L2 ? gs * d : gs * (float)((d > 0.f) - (d < 0.f));
+        return L2 ? d * d : fabsf(d);
+    };
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+    double acc = 0.0;
+    long long tail = 0;
+    if (VEC) {
+        const long long M4 = M >> 2;
+        for (long long i = t0; i < M4; i += stride) {
+            const Quad a = load4(x + 4 * i), b = load4(y + 4 * i);
+            float g[4], s = 0.f;
+#pragma unroll
+            for (int j = 0; j < 4; j++) s += term(a.v[j], b.v[j], g[j]);
+            *reinterpret_cast<float4*>(dL + 4 * i) = make_float4(g[0], g[1], g[2], g[3]);
+            acc += (double)s;
+        }
+        tail = M4 << 2;
+    }
+    for (long long i = tail + t0; i < M; i += stride) {
+        float g;
+        acc += (double)term(__ldg(x + i), to_f32(y[i]), g);
+        dL[i] = g;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    __shared__ double wsum[8];
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < 8; w++) t += wsum[w];
+        atomicAdd(loss, t * inv_m);
+        if (blockIdx.x == 0) loss[1] = (double)N;  // every pixel takes part in the mean
+    }
+}
+
+// Target of the cosine kernel as a (pixel, channel) tensor with a (PB, box_c) box.  False when the layout does not
+// meet the TMA rules (plane pitch and base multiples of 16 bytes, coordinates in int32) or the driver entry point is
+// missing; the kernel then stages with plain loads.
+bool encode_plane_map(CUtensorMap* map, const void* base, CUtensorMapDataType type, size_t es, int C, long long N,
+                      int PB, int box_c) {
+    const TensorMapEncodeFn encode = tensor_map_encoder();
+    memset(map, 0, sizeof(*map));
+    if (!encode || ((size_t)N * es) % 16 != 0 || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || N > 0x7fffffffll)
+        return false;
+    const cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)C};
+    const cuuint64_t strides[1] = {(cuuint64_t)N * es};
+    const cuuint32_t box[2] = {(cuuint32_t)PB, (cuuint32_t)box_c};
+    const cuuint32_t estr[2] = {1, 1};
+    return encode(map, type, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <typename T>
+int launch_cosine(int C, long long N, const float* render, const T* target, float* dL, double* loss, cudaStream_t s) {
+    count_valid_pixels_kernel<T><<<(unsigned)((N + 255) / 256), 256, 0, s>>>(C, N, target, loss + 1);
+    SGB_LAUNCH_CHECK("count_valid_pixels_kernel", 0, s);
+    // channels in nbox TMA boxes of box_c rows; a box after the first starts 128-byte aligned in shared memory
+    const int nbox = (C + kFlMaxBox - 1) / kFlMaxBox;
+    const int box_c = nbox == 1 ? C : ((C + nbox - 1) / nbox + 15) & ~15;
+    const size_t row = sizeof(float) + sizeof(T);
+    // the widest pixel block (a power of two, 16-byte box rows, at least one 32-byte sector of target per row) whose
+    // staged columns fit the per-CTA target
+    const int pb_min = sizeof(T) == 2 ? 16 : 8;
+    int pb_log2 = 8;
+    while ((1 << pb_log2) > pb_min && (size_t)nbox * box_c * (1 << pb_log2) * row > kFlStageTarget) pb_log2--;
+    const int PB = 1 << pb_log2;
+    const size_t xs = ((size_t)nbox * box_c * PB * sizeof(float) + 127) & ~(size_t)127;
+    const size_t smem = xs + (size_t)nbox * box_c * PB * sizeof(T);
+    constexpr size_t kMaxSmem = 96 * 1024 + 128;  // C = 1024, fp16: 16 px x 1024 x 6 B
+    static DeviceOnce attr_set;
+    if (attr_set.first_use_on_device())
+        SGB_CUDA(cudaFuncSetAttribute(feature_cosine_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
+    CUtensorMap xmap, ymap;
+    const CUtensorMapDataType ytype = sizeof(T) == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    const int use_tma = encode_plane_map(&xmap, render, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, sizeof(float), C, N, PB, box_c) &&
+                        encode_plane_map(&ymap, target, ytype, sizeof(T), C, N, PB, box_c);
+    const unsigned blocks = (unsigned)((N + PB - 1) / PB);
+    feature_cosine_kernel<T><<<blocks, kFlThreads, smem, s>>>(C, N, pb_log2, box_c, nbox, render, target, dL, loss, xmap,
+                                                             ymap, use_tma);
+    SGB_LAUNCH_CHECK("feature_cosine_kernel", 0, s);
+    return SGB_OK;
+}
+
+template <typename T, bool L2>
+int launch_elementwise(int C, long long N, const float* render, const T* target, float* dL, double* loss, cudaStream_t s) {
+    const long long M = N * C;
+    const bool vec = (reinterpret_cast<uintptr_t>(render) & 15) == 0 && (reinterpret_cast<uintptr_t>(dL) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(target) & (4 * sizeof(T) - 1)) == 0;
+    const long long work = vec ? M / 4 : M;
+    const unsigned blocks = (unsigned)std::max(1ll, std::min((work + 255) / 256, (long long)kNumSMs * 8));
+    if (vec) feature_elementwise_kernel<T, L2, true><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
+    else feature_elementwise_kernel<T, L2, false><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
+    SGB_LAUNCH_CHECK("feature_elementwise_kernel", 0, s);
+    return SGB_OK;
+}
+
+template <typename T>
+int launch_feature_loss(int loss_type, int C, long long N, const float* render, const T* target, float* dL,
+                        double* loss, cudaStream_t s) {
+    if (loss_type == SGB_FEATLOSS_COSINE) return launch_cosine<T>(C, N, render, target, dL, loss, s);
+    if (loss_type == SGB_FEATLOSS_L1) return launch_elementwise<T, false>(C, N, render, target, dL, loss, s);
+    return launch_elementwise<T, true>(C, N, render, target, dL, loss, s);
+}
+
+}  // namespace
+}  // namespace sgb
+
+using namespace sgb;
+
+extern "C" {
+
+int sgb_feature_map_loss(int32_t C, int64_t N, const float* render, const void* target, int32_t target_dtype,
+                         int32_t loss_type, float* dL_drender, double* loss, void* stream) {
+    static const char* fn = "sgb_feature_map_loss";
+    if (C <= 0 || C > kFlMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kFlMaxC); return SGB_E_INVALID; }
+    if (N < 0) { set_error("%s: N = %lld is negative", fn, (long long)N); return SGB_E_INVALID; }
+    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
+        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
+        return SGB_E_INVALID;
+    }
+    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
+        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
+        return SGB_E_INVALID;
+    }
+    if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
+    if (N > 0 && !render) { set_error("%s: null render", fn); return SGB_E_INVALID; }
+    if (N > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
+    if (N > 0 && !dL_drender) { set_error("%s: null dL_drender", fn); return SGB_E_INVALID; }
+    cudaStream_t s = (cudaStream_t)stream;
+    SGB_CUDA(cudaMemsetAsync(loss, 0, 2 * sizeof(double), s));
+    if (N == 0) return SGB_OK;
+    if (target_dtype == SGB_FEAT_F16)
+        return launch_feature_loss<__half>(loss_type, C, (long long)N, render, (const __half*)target, dL_drender, loss, s);
+    return launch_feature_loss<float>(loss_type, C, (long long)N, render, (const float*)target, dL_drender, loss, s);
+}
+
+}  // extern "C"

@@ -8,7 +8,9 @@ view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:
 ``render_semantic_labels``  label map WITHOUT the (C,H,W) feature image: alpha blending is linear in the
                        blended attribute, so rendering the K per-Gaussian similarities gives the same
                        un-normalised per-pixel similarities; the positive per-pixel normalisation does
-                       not change the arg-max."""
+                       not change the arg-max.
+``distill_loss_and_grad``      training loss against per-pixel class labels and K class embeddings.
+``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2)."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -122,6 +124,50 @@ def distill_loss_and_grad(rendering: torch.Tensor, class_emb: torch.Tensor, labe
         _lib.check(_lib.load().sgb_distill_loss(r.shape[0], e.shape[0], r.shape[1] * r.shape[2], r.data_ptr(),
                                                e.data_ptr(), lab.data_ptr(), int(lab.dtype == torch.int64),
                                                grad.data_ptr(), loss2.data_ptr(), stream), "sgb_distill_loss")
+    return loss2[0], grad
+
+
+_FEATURE_LOSSES = {"cosine": _lib.FEATLOSS_COSINE, "l1": _lib.FEATLOSS_L1, "l2": _lib.FEATLOSS_L2}
+
+
+def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, loss_type: str = "cosine"
+                              ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Distillation loss of a rendered (C,H,W) feature image against a 2D model's (C,H,W) feature map (fp16 or fp32,
+    e.g. the OpenSeg / LSeg map ``fusion.fuse_scene`` consumes) and its gradient, in one pass over both images.
+    With x = rendering.permute(1, 2, 0).reshape(-1, C) and y = target likewise (one row per pixel),
+    the loss types of distill.py:111-124:
+
+        "cosine"  m = y.norm(dim=-1) > 0;  (1 - torch.nn.CosineSimilarity()(x[m], y[m])).mean()   (0 if no m)
+        "l1"      torch.nn.L1Loss()(x, y)
+        "l2"      torch.nn.MSELoss()(x, y)
+
+    Returns (loss: 0-d float64 CUDA tensor, grad: (C,H,W) float32 = d loss / d rendering).  Use as
+    ``rendering.backward(grad)``.  Nothing is synchronised and no full-size temporary is allocated besides grad."""
+    if loss_type not in _FEATURE_LOSSES:
+        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
+    if not isinstance(rendering, torch.Tensor) or not isinstance(target, torch.Tensor):
+        raise ValueError("rendering and target must be tensors")
+    if target.requires_grad:
+        raise ValueError("target must not require grad (the loss gives the gradient of the rendering only)")
+    if target.dtype not in (torch.float16, torch.float32):
+        raise ValueError(f"target must be float16 or float32, got {target.dtype}")
+    if rendering.ndim != 3 or target.shape != rendering.shape:
+        raise ValueError(f"rendering and target must both be (C,H,W), got {tuple(rendering.shape)} and "
+                         f"{tuple(target.shape)}")
+    if not rendering.is_cuda or target.device != rendering.device:
+        raise ValueError(f"rendering and target must be CUDA tensors on one device (the feature-map loss has no CPU "
+                         f"path), got {rendering.device} and {target.device}")
+    r = _check(rendering.detach(), "rendering")
+    y = target.contiguous()
+    C_, H, W = r.shape
+    grad = torch.empty_like(r)
+    loss2 = torch.empty(2, dtype=torch.float64, device=r.device)      # [loss, pixels averaged over]; zeroed by the call
+    dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
+    with torch.cuda.device(r.device):
+        stream = torch.cuda.current_stream(r.device).cuda_stream
+        _lib.check(_lib.load().sgb_feature_map_loss(C_, H * W, r.data_ptr(), y.data_ptr(), dtype,
+                                                   _FEATURE_LOSSES[loss_type], grad.data_ptr(), loss2.data_ptr(),
+                                                   stream), "sgb_feature_map_loss")
     return loss2[0], grad
 
 
