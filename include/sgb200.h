@@ -198,6 +198,37 @@ int sgb_backward_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const
                        const void* const* image_states, const float* const* dL_dpix,
                        const sgb_view_grads* grads /* [V] */, void* stream);
 
+/* ---- differentiable expected depth and accumulated opacity (C <= 4 only).
+ *
+ * Per pixel, over the Gaussians the blend composites, in blend order, with w_i = alpha_i T_i as the forward
+ * computes it and z_i the view-space depth of the Gaussian's centre (the "depths" state field, the value the median
+ * depth uses):
+ *     expected depth  E = sum_i w_i z_i        accumulated opacity  A = sum_i w_i
+ * with no background term.  Both are accumulated with the colour channels' own statement, so they are bit for bit
+ * the blend of a feature [z, 1] over background 0.  A caller's normalised depth is E / max(A, eps).
+ *
+ * sgb_forward_render_batch_ext is sgb_forward_render_batch plus out_exp_depths and out_alphas ([V] arrays of [1,H,W]
+ * planes), given together or both NULL.  sgb_backward_batch_ext is sgb_backward_batch plus the upstream gradients
+ * dL_dexp_depth and dL_dalpha ([V] arrays of [1,H,W] planes, each NULL when absent): E and A are two more channels
+ * with features z_i and 1 over background 0, so their gradients reach means2D, conic and opacity through the colour
+ * channels' paths, and dL/dz_i = sum_p w_ip dL/dE_p reaches dL_dmeans3D through the view transform.  The per-view
+ * dL/dz lives in ctx scratch.  The non-_ext calls are these with NULL arrays.  C > 4 with any of the new arrays
+ * returns SGB_E_INVALID before anything is enqueued. */
+int sgb_forward_render_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                 const int64_t* num_rendered /* [V] host */, void* const* geometry_states,
+                                 void* const* binning_states, void* const* image_states,
+                                 const int32_t* const* radii, float* const* out_colors,
+                                 float* const* out_depths /* NULL or [V] */,
+                                 float* const* out_exp_depths /* NULL or [V] */,
+                                 float* const* out_alphas /* NULL or [V] */, void* stream);
+int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                           const int64_t* num_rendered, const int32_t* const* radii,
+                           const void* const* geometry_states, const void* const* binning_states,
+                           const void* const* image_states, const float* const* dL_dpix,
+                           const float* const* dL_dexp_depth /* NULL or [V] */,
+                           const float* const* dL_dalpha /* NULL or [V] */,
+                           const sgb_view_grads* grads /* [V] */, void* stream);
+
 /* Identity of the build: "<version> src:<sha256 prefix of csrc/ + include/>" (set by build.py; bench.py prints
  * it so that a stale prebuilt library cannot be mistaken for the sources next to it). */
 const char* sgb_build_id(void);

@@ -67,6 +67,7 @@ EXPORTS = (
     "sgb_ctx_set_feature_grad_event", "sgb_semantic_head", "sgb_feature_logits", "sgb_label_argmax", "sgb_ctx_view_stat", "sgb_knn_mean_dist2", "sgb_distill_loss",
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
+    "sgb_forward_render_batch_ext", "sgb_backward_batch_ext",
 )
 
 _lib = None
@@ -111,6 +112,10 @@ def load() -> C.CDLL:
                                                  pvp, pvp, pvp, pvp, pvp, pvp, vp]
         lib.sgb_backward_batch.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), C.POINTER(i64), pvp,
                                            pvp, pvp, pvp, pvp, C.POINTER(ViewGrads), vp]
+        lib.sgb_forward_render_batch_ext.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera),
+                                                     C.POINTER(i64), pvp, pvp, pvp, pvp, pvp, pvp, pvp, pvp, vp]
+        lib.sgb_backward_batch_ext.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), C.POINTER(i64),
+                                               pvp, pvp, pvp, pvp, pvp, pvp, pvp, C.POINTER(ViewGrads), vp]
         lib.sgb_build_id.restype = C.c_char_p
         lib.sgb_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
         lib.sgb_state_field.argtypes = [C.c_char_p, i32, i64, i32, i32, vp, vp, vp, vp, vp]

@@ -106,6 +106,7 @@ void sgb_ctx_destroy(sgb_ctx* c) {
     if (c->bin.p) cudaFree(c->bin.p);
     if (c->misc.p) cudaFree(c->misc.p);
     if (c->work.p) cudaFree(c->work.p);
+    if (c->depth_grad.p) cudaFree(c->depth_grad.p);
     for (PoolSlot& sl : c->pools)
         if (sl.mem.p) cudaFree(sl.mem.p);
     if (c->pinned) cudaFreeHost(c->pinned);
@@ -157,7 +158,7 @@ uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
 
 size_t sgb_ctx_scratch_bytes(const sgb_ctx* c) {
     if (!c) return 0;
-    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap;
+    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap;
     for (const PoolSlot& sl : c->pools) n += sl.mem.cap;
     return n;
 }
@@ -203,7 +204,8 @@ static int forward_geometry_impl(sgb_ctx* ctx, const sgb_view_inputs& in, int V,
 static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, const sgb_camera* cams,
                                const int64_t* num_rendered, void* const* geometry_states, void* const* binning_states,
                                void* const* image_states, const int32_t* const* radii, float* const* out_colors,
-                               float* const* out_depths, cudaStream_t s) {
+                               float* const* out_depths, float* const* out_exp_depths, float* const* out_alphas,
+                               cudaStream_t s) {
     int64_t maxR = 0;
     for (int v = 0; v < V; v++) maxR = num_rendered[v] > maxR ? num_rendered[v] : maxR;
     int rc = reserve_binning(ctx, in_common, in_common.P > 0 ? maxR : 0, s);
@@ -221,7 +223,9 @@ static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, i
         } else {
             StageTimer t(ctx, ST_BLEND_FWD, s);
             ctx->launches += 1;
-            rc = launch_blend_forward(w.in, w.g, w.b, w.im, w.colors, out_colors[v], out_depths ? out_depths[v] : nullptr, s);
+            rc = launch_blend_forward(w.in, w.g, w.b, w.im, w.colors, out_colors[v], out_depths ? out_depths[v] : nullptr,
+                                      out_exp_depths ? out_exp_depths[v] : nullptr, out_alphas ? out_alphas[v] : nullptr,
+                                      s);
             if (rc) return rc;
         }
     }
@@ -240,7 +244,8 @@ static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, i
 static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, const sgb_camera* cams,
                          const int64_t* num_rendered, const int32_t* const* radii, const void* const* geometry_states,
                          const void* const* binning_states, const void* const* image_states,
-                         const float* const* dL_dpix, const sgb_view_grads* grads, cudaStream_t s) {
+                         const float* const* dL_dpix, const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                         const sgb_view_grads* grads, cudaStream_t s) {
     if (in_common.P == 0) {
         if (ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
         return SGB_OK;
@@ -259,6 +264,13 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, 
     }
     const bool wide = in_common.C > 4;
     int rc;
+    // expected depth / alpha: one [P] dL/dz buffer, zeroed before each view's blend and read by its geometry kernel
+    float* dL_ddepth = nullptr;
+    if (dL_dexp_depth || dL_dalpha) {
+        rc = ctx->depth_grad.ensure(sizeof(float) * (size_t)in_common.P);
+        if (rc) return rc;
+        dL_ddepth = (float*)ctx->depth_grad.p;
+    }
     PoolView pv[SGB_MAX_BATCH];
     // dL/dfeature of every view first: it needs only the weight rows and dL/dout, it is the one large gradient and
     // it accumulates across the views of a batch, so a data-parallel caller can start exchanging it while the
@@ -279,17 +291,22 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, 
             rc = blend_backward_v3_chain(ctx, vw[v], pv[v], dL_dpix[v], gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dopacity, s);
             if (rc) return rc;
         } else if (vw[v].R > 0) {
+            if (dL_ddepth) SGB_CUDA(cudaMemsetAsync(dL_ddepth, 0, sizeof(float) * (size_t)in_common.P, s));
             StageTimer t(ctx, ST_BLEND_BWD, s);
             ctx->launches += 1;
             rc = launch_blend_backward(vw[v].in, vw[v].g, vw[v].b, vw[v].im, vw[v].colors, dL_dpix[v], gr.dL_dmeans2D,
-                                       gr.dL_dconic, gr.dL_dopacity, gr.dL_dcolors, s);
+                                       gr.dL_dconic, gr.dL_dopacity, gr.dL_dcolors,
+                                       dL_dexp_depth ? dL_dexp_depth[v] : nullptr, dL_dalpha ? dL_dalpha[v] : nullptr,
+                                       dL_ddepth, s);
             if (rc) return rc;
         }
         if (!wide && v == V - 1 && ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
         const float* cov3D = in_common.cov3D_precomp ? in_common.cov3D_precomp : vw[v].g.cov3D;  // rasterizer_impl.cu:417
         StageTimer t(ctx, ST_GEOM_BWD, s);
         ctx->launches += 1;
-        rc = launch_geom_backward(vw[v].in, vw[v].g, radii[v], cov3D, gr.dL_dcolors, gr, s);
+        // a view without instances has no blend and so no depth gradient
+        rc = launch_geom_backward(vw[v].in, vw[v].g, radii[v], cov3D, gr.dL_dcolors, gr, vw[v].R > 0 ? dL_ddepth : nullptr,
+                                  s);
         if (rc) return rc;
     }
     return SGB_OK;
@@ -330,6 +347,15 @@ int sgb_forward_render_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V,
                              const int64_t* num_rendered, void* const* geometry_states, void* const* binning_states,
                              void* const* image_states, const int32_t* const* radii, float* const* out_colors,
                              float* const* out_depths, void* stream) {
+    return sgb_forward_render_batch_ext(ctx, in, V, cams, num_rendered, geometry_states, binning_states, image_states,
+                                        radii, out_colors, out_depths, nullptr, nullptr, stream);
+}
+
+int sgb_forward_render_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                 const int64_t* num_rendered, void* const* geometry_states,
+                                 void* const* binning_states, void* const* image_states, const int32_t* const* radii,
+                                 float* const* out_colors, float* const* out_depths, float* const* out_exp_depths,
+                                 float* const* out_alphas, void* stream) {
     int rc = check_batch(in, V, cams);
     if (rc) return rc;
     if (!ctx || !num_rendered || !geometry_states || !binning_states || !image_states || !radii || !out_colors) {
@@ -340,14 +366,22 @@ int sgb_forward_render_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V,
         set_error("out_depth is only produced by the 3-channel RGB-D path (C <= 4)");
         return SGB_E_INVALID;
     }
+    if (in->C > 4 && (out_exp_depths || out_alphas)) {
+        set_error("expected depth and alpha are only produced by the C <= 4 path");
+        return SGB_E_INVALID;
+    }
+    if ((out_exp_depths == nullptr) != (out_alphas == nullptr)) {
+        set_error("out_exp_depths and out_alphas are given together or not at all");
+        return SGB_E_INVALID;
+    }
     for (int v = 0; v < V; v++)
         if (!image_states[v] || !out_colors[v] || (in->P > 0 && (!geometry_states[v] || !radii[v])) ||
-            (num_rendered[v] > 0 && !binning_states[v])) {
+            (num_rendered[v] > 0 && !binning_states[v]) || (out_exp_depths && (!out_exp_depths[v] || !out_alphas[v]))) {
             set_error("sgb_forward_render_batch: null state/output of view %d", v);
             return SGB_E_INVALID;
         }
     return forward_render_impl(ctx, *in, V, cams, num_rendered, geometry_states, binning_states, image_states, radii,
-                               out_colors, out_depths, (cudaStream_t)stream);
+                               out_colors, out_depths, out_exp_depths, out_alphas, (cudaStream_t)stream);
 }
 
 int sgb_backward(sgb_ctx* ctx, const sgb_view_inputs* in, int64_t num_rendered, const int32_t* radii,
@@ -365,12 +399,31 @@ int sgb_backward_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const
                        const int64_t* num_rendered, const int32_t* const* radii, const void* const* geometry_states,
                        const void* const* binning_states, const void* const* image_states,
                        const float* const* dL_dpix, const sgb_view_grads* grads, void* stream) {
+    return sgb_backward_batch_ext(ctx, in, V, cams, num_rendered, radii, geometry_states, binning_states, image_states,
+                                  dL_dpix, nullptr, nullptr, grads, stream);
+}
+
+int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                           const int64_t* num_rendered, const int32_t* const* radii,
+                           const void* const* geometry_states, const void* const* binning_states,
+                           const void* const* image_states, const float* const* dL_dpix,
+                           const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                           const sgb_view_grads* grads, void* stream) {
     int rc = check_batch(in, V, cams);
     if (rc) return rc;
+    if (in->C > 4 && (dL_dexp_depth || dL_dalpha)) {
+        set_error("expected depth and alpha are only produced by the C <= 4 path");
+        return SGB_E_INVALID;
+    }
     if (!ctx || !num_rendered || !radii || !geometry_states || !binning_states || !image_states || !dL_dpix || !grads) {
         set_error("sgb_backward_batch: null argument");
         return SGB_E_INVALID;
     }
+    for (int v = 0; v < V; v++)
+        if ((dL_dexp_depth && !dL_dexp_depth[v]) || (dL_dalpha && !dL_dalpha[v])) {
+            set_error("sgb_backward_batch: null dL_dexp_depth / dL_dalpha of view %d", v);
+            return SGB_E_INVALID;
+        }
     // with SH colours the geometry kernel of view v reads dL_dcolors as view v's RGB gradient, after view v's blend
     // has added into it: a buffer shared with an earlier view would carry that view's gradient too
     if (in->shs)
@@ -382,7 +435,7 @@ int sgb_backward_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const
                     return SGB_E_INVALID;
                 }
     return backward_impl(ctx, *in, V, cams, num_rendered, radii, geometry_states, binning_states, image_states, dL_dpix,
-                         grads, (cudaStream_t)stream);
+                         dL_dexp_depth, dL_dalpha, grads, (cudaStream_t)stream);
 }
 
 int64_t sgb_ctx_view_stat(const sgb_ctx* ctx, int which) {

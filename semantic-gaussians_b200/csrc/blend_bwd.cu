@@ -12,6 +12,10 @@
 //   * the transmittance chain T <- T / (1 - alpha) walks back from final_T exactly like :498;
 //   * per-pair atomics become: warp shuffle reductions -> warp-private shared-memory partials ->
 //     one block-level sum per staged Gaussian -> one red.global.add per (Gaussian, tile, channel).
+// With EXP_ALPHA the expected depth E and accumulated opacity A of blend_fwd.cu are two more channels with features
+// z_i and 1 over background 0: their upstream gradients join s and A (bgdot is unchanged), and
+// dL/dz_i = sum_p alpha_i T_i dL/dE_p is reduced like a seventh geometry partial into dL_ddepth [P], which the
+// geometry backward carries into dL/dmeans3D.
 #include <cstdlib>
 #include "common.cuh"
 
@@ -40,12 +44,15 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+template <bool EXP_ALPHA>
 __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int C,
     const float* __restrict__ bg_color, const SplatRec* __restrict__ rec, const float* __restrict__ colors,
     const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib,
     const uint32_t* __restrict__ tile_last, const float* __restrict__ dL_dpixels, float* __restrict__ dL_dmean2D,
-    float* __restrict__ dL_dconic2D, float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors) {
+    float* __restrict__ dL_dconic2D, float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolors,
+    const float* __restrict__ dL_dexp_depth, const float* __restrict__ dL_dalpha, float* __restrict__ dL_ddepth) {
+    constexpr int kGeo = EXP_ALPHA ? 7 : 6;  // geometry partials per Gaussian: means2D xy, conic 3, opacity[, z]
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BwdSmem& sm = *reinterpret_cast<BwdSmem*>(smem_raw);
 
@@ -102,6 +109,9 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
         dL[k] = (inside && k < nch) ? __ldg(dL_dpixels + (size_t)(ch0 + k) * plane + pix_id) : 0.f;
         if (k < nch) bgdot += bg_color[ch0 + k] * dL[k];  // backward.cu:527-529, chunk partial
     }
+    // dL/dE and dL/dA of this pixel (an absent plane has zero gradient)
+    const float dLE = (EXP_ALPHA && inside && dL_dexp_depth) ? __ldg(dL_dexp_depth + pix_id) : 0.f;
+    const float dLA = (EXP_ALPHA && inside && dL_dalpha) ? __ldg(dL_dalpha + pix_id) : 0.f;
     const float T_final = inside ? final_Ts[pix_id] : 0.f;
     float T = T_final;
     const int last_contributor = inside ? (int)n_contrib[pix_id] : 0;
@@ -129,13 +139,18 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
             const bool contributes = (pos < last_contributor) && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
             if (!__any_sync(0xffffffffu, contributes)) continue;
 
-            float w = 0.f, g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f, g4 = 0.f, g5 = 0.f;
+            float w = 0.f, g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f, g4 = 0.f, g5 = 0.f, g6 = 0.f;
             if (contributes) {
                 T = T / (1.f - alpha);  // backward.cu:498
                 w = alpha * T;          // dchannel_dcolor, :499
                 float s = 0.f;
 #pragma unroll
                 for (int k = 0; k < CH; k++) s += sm.feat[st][j][k] * dL[k];
+                if (EXP_ALPHA) {
+                    s += a.z * dLE;
+                    s += 1.0f * dLA;
+                    g6 = w * dLE;
+                }
                 A = last_alpha * s_last + (1.f - last_alpha) * A;  // :511 in dot-product form
                 s_last = s;
                 float dL_dalpha = (s - A) * T;                           // :515, :521
@@ -159,6 +174,10 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
                 *reinterpret_cast<float4*>(gp) = make_float4(g0, g1, g2, g3);
                 *reinterpret_cast<float2*>(gp + 4) = make_float2(g4, g5);
             }
+            if (EXP_ALPHA) {
+                g6 = warp_sum(g6);
+                if (lane == 0) sm.geo[warp][j][6] = g6;
+            }
 #pragma unroll
             for (int k = 0; k < CH; k++) {
                 const float t = warp_sum(w * dL[k]);  // :519
@@ -180,8 +199,8 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
                 if (sm.active[wv] >> j & 1u) { t += sm.dF[wv][j][k]; any = true; }
             if (any) red_add_f32(dL_dcolors + (size_t)sm.ids[st][j] * C + ch0 + k, t);
         }
-        for (int e = tid; e < cnt * 6; e += kThreads) {
-            const int j = e / 6, q = e - j * 6;
+        for (int e = tid; e < cnt * kGeo; e += kThreads) {
+            const int j = e / kGeo, q = e - j * kGeo;
             float t = 0.f;
             bool any = false;
 #pragma unroll
@@ -191,7 +210,8 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
                 const size_t id = sm.ids[st][j];
                 float* dst = q < 2 ? dL_dmean2D + id * 3 + q                        // float3 .x .y
                            : q < 5 ? dL_dconic2D + id * 4 + (q == 4 ? 3 : q - 2)    // float4 .x .y .w
-                                   : dL_dopacity + id;
+                           : q == 5 ? dL_dopacity + id
+                                    : dL_ddepth + id;
                 red_add_f32(dst, t);
             }
         }
@@ -202,7 +222,8 @@ __global__ void __launch_bounds__(kThreads) blend_backward_kernel(
 
 int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
                           const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
-                          float* dL_dcolors, cudaStream_t s) {
+                          float* dL_dcolors, const float* dL_dexp_depth, const float* dL_dalpha, float* dL_ddepth,
+                          cudaStream_t s) {
     if (in.C > 4) {  // wider rasters: blend_v3.cu
         set_error("launch_blend_backward handles C <= 4 only");
         return SGB_E_INVALID;
@@ -210,13 +231,15 @@ int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgV
     const int tiles = ((in.W + SGB_TILE - 1) / SGB_TILE) * ((in.H + SGB_TILE - 1) / SGB_TILE);
     const int chunks = (in.C + CH - 1) / CH;
     const size_t smem = sizeof(BwdSmem);
-    static DeviceOnce attr_set;
-    if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(blend_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const bool exp_alpha = dL_ddepth != nullptr;
+    auto kern = exp_alpha ? blend_backward_kernel<true> : blend_backward_kernel<false>;
+    static DeviceOnce attr_set[2];
+    if (attr_set[exp_alpha].first_use_on_device()) {
+        SGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    blend_backward_kernel<<<dim3(tiles, chunks), kThreads, smem, s>>>(
+    kern<<<dim3(tiles, chunks), kThreads, smem, s>>>(
         im.ranges, b.point_list, in.W, in.H, in.C, in.background, g.rec, colors, im.final_T, im.n_contrib,
-        im.tile_last, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors);
+        im.tile_last, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, dL_dexp_depth, dL_dalpha, dL_ddepth);
     SGB_LAUNCH_CHECK("blend_backward_kernel", in.debug, s);
     return SGB_OK;
 }

@@ -5,6 +5,10 @@
 // reference.  The per-pixel alpha / transmittance chain and the accumulation `C[ch] += f*alpha*T`
 // are the reference's statement sequence verbatim, so pixels, depth, final_T and n_contrib are
 // bit-identical.  Wider rasters go through blend_v3.cu.
+//
+// With EXP_ALPHA the walk also accumulates, with the colour channels' own statement, the expected depth
+// E = sum_i z_i alpha_i T_i and the accumulated opacity A = sum_i alpha_i T_i (no background term): E and A are
+// bit for bit what the same walk gives for a feature [z, 1] over background 0.
 #include <cstdlib>
 #include "common.cuh"
 
@@ -22,12 +26,13 @@ struct __align__(16) FwdStage {
     float feat[kBatch][CH];  // feature slice [ch0, ch0+CH) of each staged Gaussian
 };
 
-template <bool DEPTH>
+template <bool DEPTH, bool EXP_ALPHA>
 __global__ void __launch_bounds__(kThreads) blend_forward_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int C,
     const SplatRec* __restrict__ rec, const float* __restrict__ features, const float* __restrict__ bg_color,
     float* __restrict__ final_T, uint32_t* __restrict__ n_contrib, uint32_t* __restrict__ tile_last,
-    float* __restrict__ out_color, float* __restrict__ out_depth) {
+    float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_exp_depth,
+    float* __restrict__ out_alpha) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     FwdStage* stage = reinterpret_cast<FwdStage*>(smem_raw);
     __shared__ uint32_t s_last;
@@ -76,6 +81,7 @@ __global__ void __launch_bounds__(kThreads) blend_forward_kernel(
     float acc[CH];
 #pragma unroll
     for (int k = 0; k < CH; k++) acc[k] = 0.f;
+    float acc_z = 0.f, acc_w = 0.f;  // E and A
 
     if (nbatches > 0) issue(0);
 
@@ -111,6 +117,10 @@ __global__ void __launch_bounds__(kThreads) blend_forward_kernel(
             if (DEPTH) {
                 if (T > 0.5f && test_T < 0.5) D = a.z;  // rgbd forward.cu:368-372: median depth
             }
+            if (EXP_ALPHA) {
+                acc_z += a.z * alpha * T;
+                acc_w += 1.0f * alpha * T;
+            }
             T = test_T;
             last_contributor = contributor;
         }
@@ -121,6 +131,10 @@ __global__ void __launch_bounds__(kThreads) blend_forward_kernel(
             final_T[pix_id] = T;
             n_contrib[pix_id] = last_contributor;
             if (DEPTH) out_depth[pix_id] = D;
+            if (EXP_ALPHA) {
+                out_exp_depth[pix_id] = acc_z;
+                out_alpha[pix_id] = acc_w;
+            }
             atomicMax(&s_last, last_contributor);
         }
         __syncthreads();
@@ -134,20 +148,20 @@ __global__ void __launch_bounds__(kThreads) blend_forward_kernel(
     }
 }
 
-template <bool DEPTH>
+template <bool DEPTH, bool EXP_ALPHA>
 int launch_one(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
-               float* out_color, float* out_depth, cudaStream_t s) {
+               float* out_color, float* out_depth, float* out_exp_depth, float* out_alpha, cudaStream_t s) {
     const int tiles = ((in.W + SGB_TILE - 1) / SGB_TILE) * ((in.H + SGB_TILE - 1) / SGB_TILE);
     const int chunks = (in.C + CH - 1) / CH;
     const size_t smem = 2 * sizeof(FwdStage);
-    auto kern = blend_forward_kernel<DEPTH>;
+    auto kern = blend_forward_kernel<DEPTH, EXP_ALPHA>;
     static DeviceOnce attr_set;
     if (attr_set.first_use_on_device()) {
         SGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     kern<<<dim3(tiles, chunks), kThreads, smem, s>>>(im.ranges, b.point_list, in.W, in.H, in.C, g.rec, colors,
                                                     in.background, im.final_T, im.n_contrib, im.tile_last,
-                                                    out_color, out_depth);
+                                                    out_color, out_depth, out_exp_depth, out_alpha);
     SGB_LAUNCH_CHECK("blend_forward_kernel", in.debug, s);
     return SGB_OK;
 }
@@ -155,15 +169,19 @@ int launch_one(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, con
 }  // namespace
 
 int launch_blend_forward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
-                         float* out_color, float* out_depth, cudaStream_t s) {
+                         float* out_color, float* out_depth, float* out_exp_depth, float* out_alpha, cudaStream_t s) {
     // RGB / RGB-D path (C <= 4): the reference's accumulation order, bit for bit.  Wider rasters go
     // through the weights-once pipeline in blend_v3.cu.
     if (in.C > 4) {
         set_error("launch_blend_forward handles C <= 4 only");
         return SGB_E_INVALID;
     }
-    if (out_depth) return launch_one<true>(in, g, b, im, colors, out_color, out_depth, s);
-    return launch_one<false>(in, g, b, im, colors, out_color, nullptr, s);
+    if (out_exp_depth) {  // E and A come together (api.cu)
+        if (out_depth) return launch_one<true, true>(in, g, b, im, colors, out_color, out_depth, out_exp_depth, out_alpha, s);
+        return launch_one<false, true>(in, g, b, im, colors, out_color, nullptr, out_exp_depth, out_alpha, s);
+    }
+    if (out_depth) return launch_one<true, false>(in, g, b, im, colors, out_color, out_depth, nullptr, nullptr, s);
+    return launch_one<false, false>(in, g, b, im, colors, out_color, nullptr, nullptr, nullptr, s);
 }
 
 }  // namespace sgb

@@ -177,6 +177,7 @@ struct sgb_ctx {
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
     sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
+    sgb::Scratch depth_grad;  // [P] dL/d(view-space z) of the view being differentiated (expected-depth backward)
     // Per-tile weight rows of the C-channel blend (blend_v3.cu).  As many slots as views per batch: the backward
     // resolves the rows of all V views before its first kernel, and V <= slots guarantees that rebuilding one view
     // cannot evict another view of the same batch.
@@ -251,11 +252,15 @@ int run_depth_order_and_scan(sgb_ctx* ctx, const sgb_view_inputs& in, int V, con
 int reserve_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, cudaStream_t s);
 int run_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int view_slot, int64_t R, GeomView g, BinView b, ImgView im,
                 const int32_t* radii, cudaStream_t s);
+// C <= 4 blend.  out_exp_depth / out_alpha (given together or not at all): expected depth and accumulated opacity.
+// dL_ddepth non-null selects the backward with those two extra channels (either upstream plane may be null = zero);
+// it accumulates dL/dz per Gaussian into dL_ddepth, which the caller zeroes and passes on to launch_geom_backward.
 int launch_blend_forward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
-                         float* out_color, float* out_depth, cudaStream_t s);
+                         float* out_color, float* out_depth, float* out_exp_depth, float* out_alpha, cudaStream_t s);
 int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
                           const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
-                          float* dL_dcolors, cudaStream_t s);
+                          float* dL_dcolors, const float* dL_dexp_depth, const float* dL_dalpha, float* dL_ddepth,
+                          cudaStream_t s);
 struct PoolView;
 // C > 4 blend.  The weight pool of a view (blend_pool.cuh) is built by its alpha pass; blend_v3.cu owns the slots:
 //   weight_pool_build         enqueue the alpha pass of one view into its slot (no sync), so that a batch enqueues
@@ -276,7 +281,7 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView&
 int blend_backward_v3_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
                             float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, cudaStream_t s);
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,
-                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, cudaStream_t s);
+                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, const float* dL_ddepth, cudaStream_t s);
 
 // ------------------------------------------------------------------ device helpers
 #ifdef __CUDACC__

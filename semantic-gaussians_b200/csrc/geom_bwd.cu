@@ -19,7 +19,7 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
     const float tan_fovx, const float tan_fovy, const float* __restrict__ campos, const float* __restrict__ dL_dmean2D,
     const float* __restrict__ dL_dconics, float* __restrict__ dL_dmeans, const float* __restrict__ dL_dcolor,
     float* __restrict__ dL_dcov, float* __restrict__ dL_dsh, float* __restrict__ dL_dscale,
-    float* __restrict__ dL_drot) {
+    float* __restrict__ dL_drot, const float* __restrict__ dL_ddepth) {
     __shared__ float cam[35];  // view (16) | proj (16) | campos (3): read by every thread, staged once per CTA
     if (threadIdx.x < 16) {
         cam[threadIdx.x] = view_matrix[threadIdx.x];
@@ -49,6 +49,12 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
         for (int c = 0; c < 3; c++) g_rgb[c] = clamped[3 * g + c] ? 0.f : dL_dcolor[3 * g + c];
         geomgrad::colour_grad(D, p, cam + 32, shs + g * (size_t)M * 3, g_rgb, dL_dsh + g * (size_t)M * 3, g_mean);
     }
+    if (dL_ddepth) {  // view-space z = V[2] x + V[6] y + V[10] z + V[14] (transformPoint4x3), as blended into E
+        const float gz = dL_ddepth[g];
+        g_mean[0] += gz * cam[2];
+        g_mean[1] += gz * cam[6];
+        g_mean[2] += gz * cam[10];
+    }
 #pragma unroll
     for (int i = 0; i < 3; i++) dL_dmeans[3 * g + i] = g_mean[i];
 
@@ -69,14 +75,14 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
 }  // namespace
 
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,
-                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, cudaStream_t s) {
+                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, const float* dL_ddepth, cudaStream_t s) {
     const float focal_y = in.H / (2.0f * in.tan_fovy);
     const float focal_x = in.W / (2.0f * in.tan_fovx);
     geom_backward_kernel<<<(in.P + 255) / 256, 256, 0, s>>>(
         in.P, in.D, in.M, in.means3D, radii, in.shs, g.clamped, in.scales,
         in.rotations, in.scale_modifier, cov3D, in.viewmatrix, in.projmatrix, focal_x, focal_y,
         in.tan_fovx, in.tan_fovy, in.campos, gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dmeans3D, dL_dcolor_rgb,
-        gr.dL_dcov3D, gr.dL_dsh, gr.dL_dscales, gr.dL_drotations);
+        gr.dL_dcov3D, gr.dL_dsh, gr.dL_dscales, gr.dL_drotations, dL_ddepth);
     SGB_LAUNCH_CHECK("geom_backward_kernel", in.debug, s);
     return SGB_OK;
 }

@@ -97,11 +97,12 @@ def _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, 
 
 
 def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opacity, scales, rotations,
-             scale_modifier, cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, num_channels):
-    """V = len(cams) views of the same Gaussians through sgb_forward_geometry_batch / sgb_forward_render_batch: one
-    stream sync for all instance counts, one for all weight-pool checks.  Returns the marshalled inputs (None for an
-    empty scene), which _backward takes, and the per-view lists
-    (R, color, radii, geometry state, binning state, image state, depth or None)."""
+             scale_modifier, cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, num_channels,
+             want_exp_alpha=False):
+    """V = len(cams) views of the same Gaussians through sgb_forward_geometry_batch / sgb_forward_render_batch_ext:
+    one stream sync for all instance counts, one for all weight-pool checks.  Returns the marshalled inputs (None for
+    an empty scene), which _backward takes, and the per-view lists (R, color, radii, geometry state, binning state,
+    image state, depth or None, expected depth or None, alpha or None)."""
     lib = _lib.load()
     V = len(cams)
     if means3D.ndimension() == 2 and means3D.size(0) == 0 and means3D.is_cuda:
@@ -112,7 +113,9 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
         return None, ([0] * V, z(num_channels, image_height, image_width), z(0, dtype=torch.int32),
                       z(0, dtype=torch.uint8), z(0, dtype=torch.uint8),
                       z(lib.sgb_image_bytes(image_width, image_height), dtype=torch.uint8),
-                      z(1, image_height, image_width) if want_depth else None)
+                      z(1, image_height, image_width) if want_depth else None,
+                      z(1, image_height, image_width) if want_exp_alpha else None,
+                      z(1, image_height, image_width) if want_exp_alpha else None)
     native = _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                           image_height, image_width, sh, degree, prefiltered, debug, num_channels)
     inp, cameras, _, dev = native
@@ -123,7 +126,8 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
         # every pixel / every radius is written by the kernels: no zero fill (the reference's
         # torch::full of out_color is pure waste, rasterize_points.cu:73)
         out_color = [torch.empty((Cn, H, W), dtype=torch.float32, device=dev) for _ in range(V)]
-        out_depth = [torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(V)] if want_depth else None
+        plane = lambda want: [torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(V)] if want else None
+        out_depth, out_exp_depth, out_alpha = plane(want_depth), plane(want_exp_alpha), plane(want_exp_alpha)
         radii = [torch.empty((P,), dtype=torch.int32, device=dev) for _ in range(V)]
         geom = [torch.empty((lib.sgb_geometry_bytes(P),), **u8) for _ in range(V)]
         img = [torch.empty((lib.sgb_image_bytes(W, H),), **u8) for _ in range(V)]
@@ -131,17 +135,20 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
         # the geometry call waits for the instance counts: only the binning states are left for after it
         geom_p, radii_p, img_p, color_p = _ptrs(geom), _ptrs(radii), _ptrs(img), _ptrs(out_color)
         depth_p = _ptrs(out_depth) if want_depth else None
+        exp_p, alpha_p = (_ptrs(out_exp_depth), _ptrs(out_alpha)) if want_exp_alpha else (None, None)
         _lib.check(lib.sgb_forward_geometry_batch(ctx, C.byref(inp), V, cameras, geom_p, radii_p, R, stream),
                    f"{what} (geometry)")
         binning = [torch.empty((lib.sgb_binning_bytes(R[v]),), **u8) for v in range(V)]
-        _lib.check(lib.sgb_forward_render_batch(ctx, C.byref(inp), V, cameras, R, geom_p, _ptrs(binning), img_p,
-                                                radii_p, color_p, depth_p, stream), f"{what} (render)")
-    return native, (list(R), out_color, radii, geom, binning, img, out_depth)
+        _lib.check(lib.sgb_forward_render_batch_ext(ctx, C.byref(inp), V, cameras, R, geom_p, _ptrs(binning), img_p,
+                                                    radii_p, color_p, depth_p, exp_p, alpha_p, stream),
+                   f"{what} (render)")
+    return native, (list(R), out_color, radii, geom, binning, img, out_depth, out_exp_depth, out_alpha)
 
 
-def _backward(what: str, native, radii, dL_dout, geom, R, binning, img):
-    """sgb_backward_batch over the views of one forward: ``native`` is what _make_inputs returned for it, the other
-    arguments are per-view lists of its states and of dL/dout.  Returns (the per-view list of dL_dmeans2D, then the
+def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_depth=None, dL_dalpha=None):
+    """sgb_backward_batch_ext over the views of one forward: ``native`` is what _make_inputs returned for it, the other
+    arguments are per-view lists of its states and of dL/dout (dL/d expected depth and dL/d alpha: per-view lists of
+    (1, H, W) planes, or None when absent).  Returns (the per-view list of dL_dmeans2D, then the
     colour, opacity, means3D, cov3D, SH, scale and rotation gradients summed over the views).  Precomputed colours /
     features accumulate over the views in ONE (P, C) buffer inside the kernels; on the SH path the per-view RGB
     gradient is an input of that view's SH backward (backward.cu:385-386), so every view gets its own (P, 3)."""
@@ -157,6 +164,8 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img):
         torch.zeros(lead + s, **z) for s in ((P, 3), (P, 2, 2), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4))]
     bufs = [g_means2D, g_conic, g_opacity, g_colors, g_means3D, g_cov3D, g_sh, g_scales, g_rot]  # sgb_view_grads order
     gouts = [_f32(g, dev, "dL_dout_color") for g in dL_dout]
+    planes = lambda gs, name: None if gs is None else [_f32(g, dev, name).reshape(inp.H, inp.W) for g in gs]
+    g_exp, g_alpha = planes(dL_dexp_depth, "dL_dexp_depth"), planes(dL_dalpha, "dL_dalpha")
     if P != 0:
         # view v's slice of every buffer, by address; the shared colour buffer is the same for all views
         base = [t.data_ptr() for t in bufs]
@@ -167,8 +176,11 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img):
         with torch.cuda.device(dev):
             stream, ctx = _stream_ctx(dev)
             num_rendered = (C.c_int64 * V)(*map(int, R))
-            _lib.check(lib.sgb_backward_batch(ctx, C.byref(inp), V, cameras, num_rendered, _ptrs(radii), _ptrs(geom),
-                                              _ptrs(binning), _ptrs(img), _ptrs(gouts), grads, stream), what)
+            _lib.check(lib.sgb_backward_batch_ext(ctx, C.byref(inp), V, cameras, num_rendered, _ptrs(radii),
+                                                  _ptrs(geom), _ptrs(binning), _ptrs(img), _ptrs(gouts),
+                                                  None if g_exp is None else _ptrs(g_exp),
+                                                  None if g_alpha is None else _ptrs(g_alpha), grads, stream),
+                       what)
     summed = [g_colors, g_opacity, g_means3D, g_cov3D, g_sh, g_scales, g_rot]
     if V == 1:
         return ([g_means2D], *summed)
@@ -332,26 +344,43 @@ def make_module(variant: str):
                 is_chn and rs.debug, rs.num_channels if is_chn else 3)
 
     def views_forward(ctx, what, settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
-                      cov3Ds_precomp):
-        """Forward of _RasterizeGaussians (one view) and _RasterizeGaussiansBatch: (*colors, *radii[, *depths])."""
-        native, (R, color, radii, geom, binning, img, depth) = _forward(
+                      cov3Ds_precomp, expected_depth):
+        """Forward of _RasterizeGaussians (one view) and _RasterizeGaussiansBatch:
+        (*colors, *radii[, *depths][, *expected depths, *alphas]), the last two when ``expected_depth``."""
+        native, (R, color, radii, geom, binning, img, depth, exp_depth, alpha) = _forward(
             not is_chn, what, *native_args(settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
-                                           cov3Ds_precomp))
+                                           cov3Ds_precomp), want_exp_alpha=expected_depth)
         # the backward reuses the marshalled inputs; they also hold any contiguous copies their pointers refer to
-        ctx.settings_list, ctx.R, ctx.native = settings_list, R, native
+        ctx.settings_list, ctx.R, ctx.native, ctx.expected_depth = settings_list, R, native, expected_depth
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, *radii, *geom, *binning,
                               *img)
         ctx.mark_non_differentiable(*radii)
-        if is_chn:
-            return (*color, *radii)
-        ctx.mark_non_differentiable(*depth)  # no depth gradient in the reference (backward ignores it)
-        return (*color, *radii, *depth)
+        outs = (*color, *radii)
+        if not is_chn:
+            ctx.mark_non_differentiable(*depth)  # no median-depth gradient in the reference (backward ignores it)
+            outs += (*depth,)
+        if not expected_depth:
+            return outs
+        # gradients arrive as None for outputs the loss does not use: a loss on E / A alone runs no colour gradient
+        # through the blend, and one on the colours alone runs the plain backward
+        ctx.set_materialize_grads(False)
+        return outs + (*exp_depth, *alpha)
 
-    def views_backward(ctx, what, saved, grad_colors):
+    def views_backward(ctx, what, saved, grad_outputs):
         """(per-view list of dL_dmeans2D, then the gradients of means3D, sh, colors_precomp, opacities, scales,
         rotations, cov3Ds_precomp summed over the views; None for an absent optional input).  ``saved`` is
-        ctx.saved_tensors."""
+        ctx.saved_tensors, ``grad_outputs`` the gradients of views_forward's outputs."""
         V = len(ctx.settings_list)
+        grad_colors, g_exp, g_alpha = grad_outputs[:V], None, None
+        if ctx.expected_depth:
+            k = (2 if is_chn else 3) * V
+            g_exp, g_alpha = grad_outputs[k:k + V], grad_outputs[k + V:k + 2 * V]
+            rs = ctx.settings_list[0]
+            H, W = rs.image_height, rs.image_width
+            fill = lambda gs, *shape: [torch.zeros(shape, device=saved[1].device) if g is None else g for g in gs]
+            grad_colors = fill(grad_colors, rs.num_channels if is_chn else 3, H, W)
+            g_exp = None if all(g is None for g in g_exp) else fill(g_exp, 1, H, W)
+            g_alpha = None if all(g is None for g in g_alpha) else fill(g_alpha, 1, H, W)
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, *states = saved
         radii, geom, binning, img = states[:V], states[V:2 * V], states[2 * V:3 * V], states[3 * V:]
         native = ctx.native
@@ -359,7 +388,7 @@ def make_module(variant: str):
             native = _make_inputs(*native_args(ctx.settings_list, means3D, sh, colors_precomp, means3D, scales,
                                                rotations, cov3Ds_precomp))
         g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = _backward(
-            what, native, radii, grad_colors[:V], geom, ctx.R, binning, img)
+            what, native, radii, grad_colors, geom, ctx.R, binning, img, g_exp, g_alpha)
 
         def present(t, g):  # absent optional inputs were empty tensors; they get no gradient
             return g if t.numel() != 0 else None
@@ -369,11 +398,11 @@ def make_module(variant: str):
     class _RasterizeGaussians(torch.autograd.Function):
         @staticmethod
         def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                    raster_settings):
+                    raster_settings, expected_depth=False):
             rs = raster_settings
             try:
                 return views_forward(ctx, "rasterize_gaussians", [rs], means3D, sh, colors_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp)
+                                     rotations, cov3Ds_precomp, expected_depth)
             except Exception:
                 if rs.debug:
                     args = [rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
@@ -384,27 +413,29 @@ def make_module(variant: str):
                 raise
 
         @staticmethod
-        def backward(ctx, grad_out_color, *_unused):
+        def backward(ctx, *grad_outputs):
             saved = ctx.saved_tensors
             try:
                 g_means2D, g_means3D, *grads = views_backward(ctx, "rasterize_gaussians_backward", saved,
-                                                              (grad_out_color,))
+                                                              grad_outputs)
             except Exception:
                 rs = ctx.settings_list[0]
                 if rs.debug:
                     colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, radii, geom, binning, img = saved
                     args = [rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier,
-                            cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, sh,
+                            cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_outputs[0], sh,
                             rs.sh_degree, rs.campos, geom, ctx.R[0], binning, img]
                     _dump(args + [rs.debug] if is_chn else args, "snapshot_bw.dump")
                     print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
                 raise
-            return (g_means3D, g_means2D[0], *grads, None)
+            return (g_means3D, g_means2D[0], *grads, None, None)
 
     def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                            raster_settings):
+                            raster_settings, *, expected_depth=False):
+        """The reference's rasterize_gaussians; with ``expected_depth`` the outputs gain the expected depth
+        E = sum_i w_i z_i and the accumulated opacity A = sum_i w_i, (1, H, W) each and differentiable (C <= 4)."""
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                         cov3Ds_precomp, raster_settings)
+                                         cov3Ds_precomp, raster_settings, expected_depth)
 
     class _RasterizeGaussiansBatch(torch.autograd.Function):
         """V views of the same Gaussians in one native call each way (the reference loops over
@@ -414,23 +445,24 @@ def make_module(variant: str):
 
         @staticmethod
         def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings_list,
-                    *means2D):
+                    expected_depth, *means2D):
             _check_batch_settings(settings_list)
             return views_forward(ctx, "rasterize_gaussians_batch", settings_list, means3D, sh, colors_precomp,
-                                 opacities, scales, rotations, cov3Ds_precomp)
+                                 opacities, scales, rotations, cov3Ds_precomp, expected_depth)
 
         @staticmethod
         def backward(ctx, *grad_outputs):
             g_means2D, *grads = views_backward(ctx, "rasterize_gaussians_backward_batch", ctx.saved_tensors,
                                                grad_outputs)
-            return (*grads, None, *g_means2D)
+            return (*grads, None, None, *g_means2D)
 
     def rasterize_gaussians_batch(means3D, means2D_list, opacities, settings_list, shs=None, colors_precomp=None,
-                                  scales=None, rotations=None, cov3D_precomp=None):
+                                  scales=None, rotations=None, cov3D_precomp=None, expected_depth=False):
         """Batched counterpart of GaussianRasterizer.forward: ``settings_list`` holds one
         GaussianRasterizationSettings per view (same image size / background tensor / channel count; only the
         cameras differ), ``means2D_list`` one screen-space tensor per view.  Returns a list of per-view tuples
-        (color, radii[, depth]).  Batches larger than the native limit are split."""
+        (color, radii[, depth][, expected depth, alpha]), the last two with ``expected_depth`` (see
+        rasterize_gaussians).  Batches larger than the native limit are split."""
         shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
                                                                                  rotations, cov3D_precomp)
         results = []
@@ -438,10 +470,13 @@ def make_module(variant: str):
             sl = list(settings_list[lo:lo + _lib.MAX_BATCH])
             m2 = list(means2D_list[lo:lo + _lib.MAX_BATCH])
             out = _RasterizeGaussiansBatch.apply(means3D, shs, colors_precomp, opacities, scales, rotations,
-                                                 cov3D_precomp, sl, *m2)
+                                                 cov3D_precomp, sl, expected_depth, *m2)
             V = len(sl)
+            per_view = 2 if is_chn else 3
+            if expected_depth:
+                per_view += 2
             for v in range(V):
-                results.append((out[v], out[V + v]) if is_chn else (out[v], out[V + v], out[2 * V + v]))
+                results.append(tuple(out[i * V + v] for i in range(per_view)))
         return results
 
     class GaussianRasterizer(nn.Module):  # channel_rasterization/__init__.py:232-289
@@ -460,6 +495,14 @@ def make_module(variant: str):
                                                                                      rotations, cov3D_precomp)
             return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, self.raster_settings)
+
+        def forward_expected_depth(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
+                                   rotations=None, cov3D_precomp=None):
+            """forward() followed by the differentiable expected depth and alpha (see rasterize_gaussians)."""
+            shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
+                                                                                     rotations, cov3D_precomp)
+            return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
+                                       cov3D_precomp, self.raster_settings, expected_depth=True)
 
     GaussianRasterizationSettings.__qualname__ = "GaussianRasterizationSettings"
     GaussianRasterizer.__qualname__ = "GaussianRasterizer"

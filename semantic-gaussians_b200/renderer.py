@@ -8,6 +8,14 @@ Differences from the reference, all on purpose:
   * tensors are created on ``pc.get_xyz.device`` instead of the literal "cuda";
   * render_chn() honours ``pipe.debug`` instead of hard-coding debug=True
     (model/renderer.py:181), which made every call deep-copy all inputs to the CPU.
+
+Addition: render_with_depth() (render()'s parameters; render() keeps the reference's exact signature) and
+render_batch(..., differentiable_depth=True) also return, from the same pass,
+  "expected_depth"  E = sum_i w_i z_i  (1, H, W)   w_i = alpha_i T_i, z_i the view-space depth of Gaussian i
+  "alpha"           A = sum_i w_i      (1, H, W)
+with gradients (to means3D through z and through the blend weights, to opacity, scales / rotations or cov3D, and
+the screen-space points).  No background term: the normalised depth is E / A.clamp_min(eps).  "depth" stays the
+reference's non-differentiable median depth.
 """
 import math
 
@@ -73,13 +81,32 @@ def _prepare(viewpoint_camera, pc, pipe, scaling_modifier, override_color, overr
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            override_shape=None, foreground=None, world_rotate=None):
     """RGB + median depth (rgbd rasterizer).  Background tensor (bg_color) must be on the GPU."""
+    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, override_shape, foreground,
+                   world_rotate, False)
+
+
+def render_with_depth(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
+                      override_shape=None, foreground=None, world_rotate=None):
+    """render()'s dict plus the differentiable "expected_depth" and "alpha" of the same pass (module docstring)."""
+    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, override_shape, foreground,
+                   world_rotate, True)
+
+
+def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, override_shape, foreground,
+            world_rotate, differentiable_depth):
     screenspace_points, common, call = _prepare(viewpoint_camera, pc, pipe, scaling_modifier, override_color,
                                                 override_shape, foreground, world_rotate)
     raster_settings = GaussianRasterizationSettings(bg=bg_color, debug=pipe.debug, **common)
     rasterizer = GaussianRasterizer(raster_settings=raster_settings)
-    rendered_image, radii, depth = rasterizer(**call)
-    return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
-            "radii": radii, "depth": depth}
+    if differentiable_depth:
+        rendered_image, radii, depth, exp_depth, alpha = rasterizer.forward_expected_depth(**call)
+    else:
+        rendered_image, radii, depth = rasterizer(**call)
+    out = {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
+           "radii": radii, "depth": depth}
+    if differentiable_depth:
+        out.update(expected_depth=exp_depth, alpha=alpha)
+    return out
 
 
 def render_chn(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, num_channels=3,
@@ -96,14 +123,14 @@ def render_chn(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modif
 
 
 def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_channels, override_color, override_shape,
-                  foreground, world_rotate):
+                  foreground, world_rotate, differentiable_depth=False):
     """Shared body of render_batch / render_chn_batch: the Gaussian-side tensors are prepared ONCE (the reference's
     per-view loop, eval_segmentation.py:146-157 / fusion.py:106-120, re-evaluates the activations for every view),
     the views go through the batched native calls (rasterizer.rasterize_gaussians_batch)."""
     cameras = list(cameras)
     if not cameras:
         return []
-    single = render if variant == "rgbd" else (
+    single = (render_with_depth if differentiable_depth else render) if variant == "rgbd" else (
         lambda cam, *a, **k: render_chn(cam, *a, num_channels=num_channels, **k))
     per_view_colors = override_color is None and pipe.convert_shs_python   # python SH -> colours depend on the camera
     if per_view_colors:
@@ -137,21 +164,24 @@ def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_ch
     Rast = mod.GaussianRasterizer if variant == "chn" else GaussianRasterizer
     outs = Rast.rasterize_batch(call["means3D"], points, call["opacities"], settings, shs=call["shs"],
                                 colors_precomp=call["colors_precomp"], scales=call["scales"],
-                                rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"])
+                                rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
+                                expected_depth=differentiable_depth)
     res = []
     for pts, o in zip(points, outs):
         d = {"render": o[0], "viewspace_points": pts, "visibility_filter": o[1] > 0, "radii": o[1]}
         if variant == "rgbd":
             d["depth"] = o[2]
+        if differentiable_depth:
+            d.update(expected_depth=o[3], alpha=o[4])
         res.append(d)
     return res
 
 
 def render_batch(cameras, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-                 override_shape=None, foreground=None, world_rotate=None):
+                 override_shape=None, foreground=None, world_rotate=None, *, differentiable_depth=False):
     """``[render(cam, ...) for cam in cameras]`` through the batched native path: same per-view dicts."""
     return _render_batch("rgbd", cameras, pc, pipe, bg_color, scaling_modifier, 3, override_color, override_shape,
-                         foreground, world_rotate)
+                         foreground, world_rotate, differentiable_depth)
 
 
 def render_chn_batch(cameras, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, num_channels=3,
