@@ -325,6 +325,23 @@ int sgb_feature_map_loss(int32_t C, int64_t N, const float* render, const void* 
                          int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type,
                          float* dL_drender, double* loss /* [2] device: loss, Nv; zeroed by the call */,
                          void* stream);
+/* The same loss on a compact rendered field through a per-pixel linear decoder (a 1x1 conv / nn.Linear(c, C)), with
+ * every gradient, without materialising the decoded (C, N) image.  render / dL_drender (c, N) planar fp32, weight /
+ * dL_dweight (C, c) row-major fp32 (nn.Linear(c, C).weight), bias / dL_dbias (C) fp32 or both NULL, target (C, N)
+ * planar, SGB_FEAT_F16 or SGB_FEAT_F32.  Per pixel x_p = weight render[:, p] + bias, and the loss on x against the
+ * target is exactly that of sgb_feature_map_loss (same loss_type values, the same loss[2] output).  With g_p = dLoss/dx_p:
+ *     dL_drender[:, p] = weight^T g_p      dL_dweight = sum_p g_p render[:, p]^T      dL_dbias = sum_p g_p
+ * dL_dweight and dL_dbias are overwritten, not added to.  workspace: caller-allocated device scratch of
+ * sgb_decoded_feature_loss_workspace_bytes(C, c, N) bytes, 16-byte aligned (it depends on C and c only).  Every output
+ * is bitwise identical from call to call (no float atomics).  1 <= C <= 1024, 1 <= c <= 128; a bad argument returns
+ * SGB_E_INVALID before anything is enqueued.  Asynchronous on `stream`, no host copy, no ctx; N == 0 only zeroes loss,
+ * dL_dweight and dL_dbias.  The workspace-size call returns 0 for C, c or N outside those limits. */
+size_t sgb_decoded_feature_loss_workspace_bytes(int32_t C, int32_t c, int64_t N);
+int sgb_decoded_feature_loss(int32_t C, int32_t c, int64_t N, const float* render, const float* weight,
+                             const float* bias /* NULL */, const void* target,
+                             int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type,
+                             float* dL_drender, float* dL_dweight, float* dL_dbias /* NULL iff bias NULL */,
+                             void* workspace, double* loss /* [2] device: loss, pixels averaged over */, void* stream);
 int sgb_semantic_head(sgb_ctx* ctx, int32_t C, int32_t K, int64_t N, const float* render, const float* text,
                       int32_t first_class, float* sim, int64_t* label, void* stream);
 int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const float* features, const float* text,

@@ -67,7 +67,8 @@ EXPORTS = (
     "sgb_ctx_set_feature_grad_event", "sgb_semantic_head", "sgb_feature_logits", "sgb_label_argmax", "sgb_ctx_view_stat", "sgb_knn_mean_dist2", "sgb_distill_loss",
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
-    "sgb_forward_render_batch_ext", "sgb_backward_batch_ext",
+    "sgb_forward_render_batch_ext", "sgb_backward_batch_ext", "sgb_decoded_feature_loss",
+    "sgb_decoded_feature_loss_workspace_bytes",
 )
 
 _lib = None
@@ -141,6 +142,9 @@ def load() -> C.CDLL:
         lib.sgb_photometric_backward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp, i64, i64, vp]
         lib.sgb_confusion_accumulate.argtypes = [i64, vp, i32, vp, i32, i32, i32, vp, vp, vp]
         lib.sgb_feature_map_loss.argtypes = [i32, i64, vp, vp, i32, i32, vp, vp, vp]
+        lib.sgb_decoded_feature_loss.argtypes = [i32, i32, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
+        lib.sgb_decoded_feature_loss_workspace_bytes.argtypes = [i32, i32, i64]
+        lib.sgb_decoded_feature_loss_workspace_bytes.restype = C.c_size_t
         _lib = lib
         return lib
 

@@ -22,6 +22,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "feature_loss.cuh"
 
 namespace sgb {
 namespace {
@@ -257,8 +258,8 @@ bool encode_plane_map(CUtensorMap* map, const void* base, CUtensorMapDataType ty
 
 template <typename T>
 int launch_cosine(int C, long long N, const float* render, const T* target, float* dL, double* loss, cudaStream_t s) {
-    count_valid_pixels_kernel<T><<<(unsigned)((N + 255) / 256), 256, 0, s>>>(C, N, target, loss + 1);
-    SGB_LAUNCH_CHECK("count_valid_pixels_kernel", 0, s);
+    const int rc = count_valid_pixels<T>(C, N, target, loss + 1, s);
+    if (rc != SGB_OK) return rc;
     // channels in nbox TMA boxes of box_c rows; a box after the first starts 128-byte aligned in shared memory
     const int nbox = (C + kFlMaxBox - 1) / kFlMaxBox;
     const int box_c = nbox == 1 ? C : ((C + nbox - 1) / nbox + 15) & ~15;
@@ -308,6 +309,16 @@ int launch_feature_loss(int loss_type, int C, long long N, const float* render, 
 }
 
 }  // namespace
+
+template <typename T>
+int count_valid_pixels(int C, long long N, const T* target, double* valid, cudaStream_t s) {
+    count_valid_pixels_kernel<T><<<(unsigned)((N + 255) / 256), 256, 0, s>>>(C, N, target, valid);
+    SGB_LAUNCH_CHECK("count_valid_pixels_kernel", 0, s);
+    return SGB_OK;
+}
+template int count_valid_pixels<float>(int, long long, const float*, double*, cudaStream_t);
+template int count_valid_pixels<__half>(int, long long, const __half*, double*, cudaStream_t);
+
 }  // namespace sgb
 
 using namespace sgb;

@@ -10,7 +10,8 @@ view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:
                        un-normalised per-pixel similarities; the positive per-pixel normalisation does
                        not change the arg-max.
 ``distill_loss_and_grad``      training loss against per-pixel class labels and K class embeddings.
-``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2)."""
+``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2).
+``decoded_feature_map_loss_and_grads``  the same loss for a compact field through a per-pixel linear decoder."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -169,6 +170,68 @@ def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, los
                                                    _FEATURE_LOSSES[loss_type], grad.data_ptr(), loss2.data_ptr(),
                                                    stream), "sgb_feature_map_loss")
     return loss2[0], grad
+
+
+def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Tensor, target: torch.Tensor,
+                                       bias: Optional[torch.Tensor] = None, loss_type: str = "cosine"
+                                       ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+    """``feature_map_loss_and_grad`` for a compact field: the rendered (c,H,W) image is lifted per pixel to the C
+    channels of the (C,H,W) target (fp16 or fp32) by a linear decoder, ``x = weight @ r + bias`` (weight (C,c) as
+    ``nn.Linear(c, C).weight``, or a 1x1 ``nn.Conv2d`` weight viewed as (C,c)), and the loss of
+    ``feature_map_loss_and_grad`` is taken on x.  The decoded (C,H,W) image is never materialised.
+
+    Returns (loss: 0-d float64 CUDA tensor, g_render (c,H,W), g_weight (C,c), g_bias (C,) or None when bias is None),
+    all gradients of the loss.  Use as ``rendering.backward(g_render)``, ``decoder.weight.grad = g_weight``,
+    ``decoder.bias.grad = g_bias``.  weight and bias are read detached (they may be nn.Parameters).  1 <= C <= 1024,
+    1 <= c <= 128.  Nothing is synchronised; besides the outputs only a scratch buffer that depends on C and c alone
+    is allocated, and every output is bitwise reproducible."""
+    if loss_type not in _FEATURE_LOSSES:
+        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
+    for name, t in (("rendering", rendering), ("weight", weight), ("target", target), ("bias", bias)):
+        if not isinstance(t, torch.Tensor) and not (name == "bias" and t is None):
+            raise ValueError(f"{name} must be a tensor")
+    if target.requires_grad:
+        raise ValueError("target must not require grad (the loss gives the gradients of the rendering and decoder)")
+    if target.dtype not in (torch.float16, torch.float32):
+        raise ValueError(f"target must be float16 or float32, got {target.dtype}")
+    if weight.dtype != torch.float32 or (bias is not None and bias.dtype != torch.float32):
+        raise ValueError(f"weight and bias must be float32, got {weight.dtype} and "
+                         f"{None if bias is None else bias.dtype}")
+    if rendering.ndim != 3 or weight.ndim != 2 or weight.shape[1] != rendering.shape[0] or \
+            target.shape != (weight.shape[0],) + tuple(rendering.shape[1:]) or \
+            (bias is not None and tuple(bias.shape) != (weight.shape[0],)):
+        raise ValueError(f"rendering must be (c,H,W), weight (C,c), target (C,H,W) and bias (C,), got "
+                         f"{tuple(rendering.shape)}, {tuple(weight.shape)}, {tuple(target.shape)} and "
+                         f"{None if bias is None else tuple(bias.shape)}")
+    C_, c = weight.shape
+    if not (1 <= C_ <= 1024 and 1 <= c <= 128):
+        raise ValueError(f"the decoder must have 1 <= C <= 1024 outputs and 1 <= c <= 128 inputs, got ({C_}, {c})")
+    tensors = [rendering, weight, target] + ([bias] if bias is not None else [])
+    if not rendering.is_cuda or any(t.device != rendering.device for t in tensors):
+        raise ValueError(f"rendering, weight, target and bias must be CUDA tensors on one device (the decoded "
+                         f"feature-map loss has no CPU path), got {', '.join(str(t.device) for t in tensors)}")
+    r = _check(rendering.detach(), "rendering")
+    w = weight.detach().contiguous()
+    b = bias.detach().contiguous() if bias is not None else None
+    y = target.contiguous()
+    _, H, W = r.shape
+    N = H * W
+    lib = _lib.load()
+    g_render = torch.empty_like(r)
+    g_weight = torch.empty_like(w)
+    g_bias = torch.empty_like(b) if b is not None else None
+    workspace = torch.empty(lib.sgb_decoded_feature_loss_workspace_bytes(C_, c, N), dtype=torch.uint8, device=r.device)
+    loss2 = torch.empty(2, dtype=torch.float64, device=r.device)      # [loss, pixels averaged over]; zeroed by the call
+    dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
+    with torch.cuda.device(r.device):
+        stream = torch.cuda.current_stream(r.device).cuda_stream
+        _lib.check(lib.sgb_decoded_feature_loss(C_, c, N, r.data_ptr(), w.data_ptr(),
+                                                b.data_ptr() if b is not None else None, y.data_ptr(), dtype,
+                                                _FEATURE_LOSSES[loss_type], g_render.data_ptr(), g_weight.data_ptr(),
+                                                g_bias.data_ptr() if g_bias is not None else None,
+                                                workspace.data_ptr(), loss2.data_ptr(), stream),
+                   "sgb_decoded_feature_loss")
+    return loss2[0], g_render, g_weight, g_bias
 
 
 def render_semantic_labels(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, text_features: torch.Tensor,
