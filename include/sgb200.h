@@ -373,6 +373,31 @@ int sgb_confusion_accumulate(int64_t N, const void* pred, int32_t pred_dtype, co
                              int32_t pred_offset, int32_t num_classes, uint64_t* counts, uint32_t* invalid,
                              void* stream);
 
+/* ---- voxelization: Voxelizer.voxelize + sparse_quantize of dataset/fusion_utils.py, bit for bit, on the device.
+ *
+ * For every point p of xyz (P,3) fp32 and the row-major 3x4 fp64 transform T (host memory, 12 doubles):
+ *     v[a]  = floor(((x T[4a] + y T[4a+1]) + z T[4a+2]) + T[4a+3])     fp64, every product and sum rounded alone
+ *     u[a]  = v[a] - min_p v[a]                                         origin-aligned voxel coordinate
+ *     key   = FNV-1a 64 of (u[0], u[1], u[2]): h = 14695981039346656037; per axis h *= 1099511628211, h ^= u[a]
+ * and then np.unique(key, return_index=True, return_inverse=True):
+ *     first_index[0..M)  the first point of each distinct key, in ascending key order (return_index)
+ *     inverse[p]         the rank of p's key among the M distinct keys (return_inverse)
+ *     coords[0..M)       (M,3) int32 u of the point first_index[r]
+ * Two voxels whose keys collide are one voxel here, as in the reference (the first point's coordinates win).
+ *
+ * counts (device, 3 int64) receives [0] M, [1] the number of points with a non-finite v (the reference's result is
+ * undefined then) and [2] SGB_E_OVERFLOW when an axis spans 2^31 voxels or more (coords are int32), else SGB_OK.
+ * The outputs are only meaningful when counts[1] == 0 and counts[2] == SGB_OK; they never index out of range
+ * otherwise.  The status words live on the device because the call never synchronises.
+ *
+ * workspace: device scratch of sgb_voxelize_workspace_bytes(P) bytes, 16-byte aligned.  1 <= P <= 2^31 - 1; a bad
+ * argument returns SGB_E_INVALID before anything is enqueued.  Asynchronous on `stream`, no host copy, no ctx; the
+ * same inputs give bitwise identical outputs.  The workspace-size call returns 0 for P outside those limits. */
+size_t sgb_voxelize_workspace_bytes(int64_t P);
+int sgb_voxelize(int64_t P, const float* xyz, const double* transform /* [12] host */, void* workspace,
+                 int64_t* first_index /* (P) */, int64_t* inverse /* (P) */, int32_t* coords /* (P,3) */,
+                 int64_t* counts /* [3] */, void* stream);
+
 /* ---- 3-nearest-neighbour mean squared distance: `distCUDA2` of the reference's
  * simple-knn extension (submodules/simple-knn/simple_knn.cu:185-220, spatial.cu), used by
  * GaussianModel.create_from_pcd (model/gaussian_model.py:150-186).  points (P,3) fp32 device, mean_dist2 (P) fp32

@@ -68,7 +68,7 @@ EXPORTS = (
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
     "sgb_forward_render_batch_ext", "sgb_backward_batch_ext", "sgb_decoded_feature_loss",
-    "sgb_decoded_feature_loss_workspace_bytes",
+    "sgb_decoded_feature_loss_workspace_bytes", "sgb_voxelize", "sgb_voxelize_workspace_bytes",
 )
 
 _lib = None
@@ -145,6 +145,9 @@ def load() -> C.CDLL:
         lib.sgb_decoded_feature_loss.argtypes = [i32, i32, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
         lib.sgb_decoded_feature_loss_workspace_bytes.argtypes = [i32, i32, i64]
         lib.sgb_decoded_feature_loss_workspace_bytes.restype = C.c_size_t
+        lib.sgb_voxelize.argtypes = [i64, vp, C.POINTER(C.c_double), vp, vp, vp, vp, vp, vp]
+        lib.sgb_voxelize_workspace_bytes.argtypes = [i64]
+        lib.sgb_voxelize_workspace_bytes.restype = C.c_size_t
         _lib = lib
         return lib
 

@@ -134,6 +134,22 @@ class GaussianModel(DensifyMixin):
         self._features_semantic = torch.zeros((P, dim), dtype=torch.float32, device=dev)
         self._times = torch.zeros((P, 1), dtype=torch.float32, device=dev)
 
+    def get_locs_and_features(self, feature_type="all", device=False):
+        """model/gaussian_model.py:400-418: the raw xyz (P,3) and the per-Gaussian features the 3D network reads,
+        ``"all"``: opacity, SH dc, SH rest, scale, rotation (56 columns at degree 3), ``"color"``: SH dc and rest
+        (48).  numpy arrays as the reference returns them, or with ``device=True`` the tensors on the model's
+        device with no host copy (voxelize.voxelize_gaussians)."""
+        parts = {"all": (self._opacity, self._features_dc, self._features_rest, self._scaling, self._rotation),
+                 "color": (self._features_dc, self._features_rest)}
+        if feature_type not in parts:
+            raise ValueError(f"feature_type must be 'all' or 'color', got {feature_type!r}")
+        P = self._xyz.shape[0]
+        locs = self._xyz.detach()
+        features = torch.cat([t.detach().reshape(P, -1) for t in parts[feature_type]], dim=-1)
+        if device:
+            return locs, features
+        return locs.cpu().numpy().copy(), features.cpu().numpy()
+
     # --- on-disk formats (model/gaussian_model.py:265-281, :288-344, :346-378) without plyfile
     def save_ply(self, path):
         from .io_formats import save_gaussian_ply
