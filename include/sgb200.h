@@ -283,6 +283,32 @@ int sgb_fusion_accumulate(sgb_ctx* ctx, const sgb_fusion_view* v, const void* fe
 /* fusion.py:146-147: count[count==0] = 1e-5; feat_sum /= count (in place). */
 int sgb_fusion_normalize(int32_t P, int32_t C, float* feat_sum, float* count, void* stream);
 
+/* ---- lifting feature maps onto the Gaussians by their blend weights (the adjoint of rendering).
+ *
+ * For V views of the same Gaussians (V <= SGB_MAX_BATCH), with w_i^v(p) = alpha_i T_i as the forward blend computes it
+ * (0 where the walk skips Gaussian i at pixel p or has stopped) and no background term:
+ *     feat_sum[i][c] += sum_v sum_p w_i^v(p) map_v[c][p]          weight_sum[i] += sum_v sum_p w_i^v(p)
+ * feat_sum is what sgb_backward's dL_dcolors would receive with dL/dout = map_v.  sgb_fusion_normalize(P, C,
+ * feat_sum, weight_sum) then gives each Gaussian the weighted mean of the pixels it shows in, a convex combination of
+ * map values (0 for a Gaussian that no pixel shows).  Occlusion comes from the transmittance: no depth test.
+ *
+ * in: P, W, H, C (the map channels, any C >= 1), means3D, opacities, scales + rotations or cov3D_precomp,
+ * scale_modifier, prefiltered, debug; shs, colors_precomp and background must be NULL; the camera fields are ignored
+ * (cams[v] is view v).  maps[v]: (C, H, W) contiguous, SGB_FEAT_F16 or SGB_FEAT_F32, any 2-byte / 4-byte alignment
+ * (fp16 maps are read as fp16 and widened on chip; sums are fp32).  feat_sum (P, C) and weight_sum (P) fp32 are
+ * accumulated into: the caller zero-fills them once and may lift any number of calls into them.
+ * Per view: geometry, binning and the alpha pass (weight pool) of the C > 4 blend, then the dL/dfeature contraction
+ * with the map as dL/dout and a pass over the weight rows; never the colour blend, the chain or the geometry backward.
+ * The per-view states live in ctx scratch and nothing outlives the call; the weight-pool slots it took are left empty,
+ * and a later sgb_backward_batch rebuilds the rows of any forward whose slot it took.  The host synchronises twice, as
+ * sgb_forward_geometry_batch + sgb_forward_render_batch do: once for the V instance counts, once for the V weight-pool
+ * checks (plus one per rebuilt pool when a pool overflows).  Bad arguments return SGB_E_INVALID before anything is
+ * enqueued: V outside 1..SGB_MAX_BATCH, C < 1, an unknown map_dtype, a null array or map, shs / colors_precomp /
+ * background given, or the forward's scale/rotation-versus-cov3D_precomp rule. */
+int sgb_lift_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                   const void* const* maps /* [V] (C,H,W) */, int32_t map_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */,
+                   float* feat_sum /* (P,C) */, float* weight_sum /* (P) */, void* stream);
+
 /* ---- semantic head: what every render_chn caller runs on the rendered feature image.
  *
  * sgb_semantic_head: render (C, N) planar fp32 with N = H*W, text (K, C) row-major:

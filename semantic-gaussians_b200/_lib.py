@@ -68,7 +68,7 @@ EXPORTS = (
     "sgb_forward_geometry_batch", "sgb_forward_render_batch", "sgb_backward_batch", "sgb_build_id",
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
     "sgb_forward_render_batch_ext", "sgb_backward_batch_ext", "sgb_decoded_feature_loss",
-    "sgb_decoded_feature_loss_workspace_bytes", "sgb_voxelize", "sgb_voxelize_workspace_bytes",
+    "sgb_decoded_feature_loss_workspace_bytes", "sgb_voxelize", "sgb_voxelize_workspace_bytes", "sgb_lift_batch",
 )
 
 _lib = None
@@ -124,6 +124,7 @@ def load() -> C.CDLL:
         lib.sgb_fusion_map.argtypes = [vp, C.POINTER(FusionView), vp, vp]
         lib.sgb_fusion_accumulate.argtypes = [vp, C.POINTER(FusionView), vp, i32, i32, vp, vp, vp, vp]
         lib.sgb_fusion_normalize.argtypes = [i32, i32, vp, vp, vp]
+        lib.sgb_lift_batch.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), pvp, i32, vp, vp, vp]
         lib.sgb_profile_enable.argtypes = [vp, C.c_int]
         lib.sgb_profile_read.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(i32)]
         lib.sgb_profile_stage_name.argtypes = [C.c_int]

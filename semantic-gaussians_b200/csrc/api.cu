@@ -107,6 +107,8 @@ void sgb_ctx_destroy(sgb_ctx* c) {
     if (c->misc.p) cudaFree(c->misc.p);
     if (c->work.p) cudaFree(c->work.p);
     if (c->depth_grad.p) cudaFree(c->depth_grad.p);
+    if (c->lift_state.p) cudaFree(c->lift_state.p);
+    if (c->lift_bin.p) cudaFree(c->lift_bin.p);
     for (PoolSlot& sl : c->pools)
         if (sl.mem.p) cudaFree(sl.mem.p);
     if (c->pinned) cudaFreeHost(c->pinned);
@@ -149,7 +151,7 @@ int sgb_profile_num_stages(void) { return ST_COUNT; }
 const char* sgb_profile_stage_name(int st) {
     static const char* names[ST_COUNT] = {"preprocess", "depth_sort", "scan", "emit", "tile_sort", "ranges",
                                           "blend_fwd", "blend_bwd", "geom_bwd", "fusion_project",
-                                          "fusion_sort", "fusion_gather", "alpha_pass", "dfeature"};
+                                          "fusion_sort", "fusion_gather", "alpha_pass", "dfeature", "weight_sum"};
     return (st >= 0 && st < ST_COUNT) ? names[st] : "";
 }
 uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
@@ -158,7 +160,8 @@ uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
 
 size_t sgb_ctx_scratch_bytes(const sgb_ctx* c) {
     if (!c) return 0;
-    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap;
+    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap + c->lift_state.cap +
+               c->lift_bin.cap;
     for (const PoolSlot& sl : c->pools) n += sl.mem.cap;
     return n;
 }
@@ -436,6 +439,98 @@ int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, c
                 }
     return backward_impl(ctx, *in, V, cams, num_rendered, radii, geometry_states, binning_states, image_states, dL_dpix,
                          dL_dexp_depth, dL_dalpha, grads, (cudaStream_t)stream);
+}
+
+// ---- lifting feature maps onto the Gaussians by their blend weights ------------------------------------------
+// Per view: geometry, binning and the alpha pass (the weight pool) into ctx scratch, then the dL/dfeature contraction
+// with the map as dL/dout and the per-Gaussian weight-row sums.  No colour blend, no chain or geometry backward.
+static int lift_impl(sgb_ctx* ctx, const sgb_view_inputs& in, int V, const sgb_camera* cams, const void* const* maps,
+                     int32_t map_dtype, float* feat_sum, float* weight_sum, cudaStream_t s) {
+    const int P = in.P;
+    const size_t geom_b = sgb_geometry_bytes(P), radii_b = align_up(sizeof(int32_t) * (size_t)P),
+                 img_b = sgb_image_bytes(in.W, in.H), per_view = geom_b + radii_b + img_b;
+    int rc = ctx->lift_state.ensure((size_t)V * per_view);
+    if (rc) return rc;
+    void* geom[SGB_MAX_BATCH];
+    void* img[SGB_MAX_BATCH];
+    int32_t* radii[SGB_MAX_BATCH];
+    for (int v = 0; v < V; v++) {
+        char* base = (char*)ctx->lift_state.p + (size_t)v * per_view;
+        geom[v] = base;
+        radii[v] = (int32_t*)(base + geom_b);
+        img[v] = base + geom_b + radii_b;
+    }
+    int64_t R[SGB_MAX_BATCH];
+    rc = forward_geometry_impl(ctx, in, V, cams, geom, radii, R, s);  // the first sync: the V instance counts
+    if (rc) return rc;
+    int64_t maxR = 0;
+    size_t bin_total = 0;
+    for (int v = 0; v < V; v++) {
+        maxR = R[v] > maxR ? R[v] : maxR;
+        bin_total += sgb_binning_bytes(R[v]);
+    }
+    if (maxR == 0) return SGB_OK;
+    rc = reserve_binning(ctx, in, maxR, s);
+    if (rc) return rc;
+    rc = ctx->lift_bin.ensure(bin_total);
+    if (rc) return rc;
+    ViewState vw[SGB_MAX_BATCH];
+    int nv = 0;  // views with instances, compacted to the front of vw
+    size_t bin_off = 0;
+    for (int v = 0; v < V; v++) {
+        if (R[v] == 0) continue;
+        ViewState& w = vw[nv];
+        w = ViewState::carve(in, cams[v], R[v], geom[v], (char*)ctx->lift_bin.p + bin_off, img[v]);
+        bin_off += sgb_binning_bytes(R[v]);
+        rc = run_binning(ctx, w.in, v, w.R, w.g, w.b, w.im, radii[v], s);
+        if (!rc) rc = weight_pool_build(ctx, w, s);
+        if (rc) {
+            weight_pool_release(ctx, nv + 1, vw);
+            return rc;
+        }
+        nv++;
+    }
+    PoolView pv[SGB_MAX_BATCH];
+    rc = weight_pool_settle(ctx, nv, vw, pv, s);  // the second sync: the weight-pool checks
+    for (int k = 0, v = 0; !rc && v < V; v++) {
+        if (R[v] == 0) continue;
+        if (map_dtype == SGB_FEAT_F16)
+            rc = blend_backward_v3_dfeature(ctx, vw[k], pv[k], static_cast<const __half*>(maps[v]), feat_sum, s);
+        else
+            rc = blend_backward_v3_dfeature(ctx, vw[k], pv[k], static_cast<const float*>(maps[v]), feat_sum, s);
+        if (!rc) rc = pool_weight_sums(ctx, vw[k], pv[k], weight_sum, s);
+        k++;
+    }
+    weight_pool_release(ctx, nv, vw);
+    return rc;
+}
+
+int sgb_lift_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                   const void* const* maps, int32_t map_dtype, float* feat_sum, float* weight_sum, void* stream) {
+    if (!ctx || !in || !cams || !maps || !feat_sum || !weight_sum) {
+        set_error("sgb_lift_batch: null argument");
+        return SGB_E_INVALID;
+    }
+    if (V < 1 || V > SGB_MAX_BATCH) { set_error("batch of %d views: need 1 <= V <= %d", V, SGB_MAX_BATCH); return SGB_E_INVALID; }
+    if (map_dtype != SGB_FEAT_F16 && map_dtype != SGB_FEAT_F32) {
+        set_error("sgb_lift_batch: unknown map dtype %d", map_dtype);
+        return SGB_E_INVALID;
+    }
+    if (in->shs || in->colors_precomp || in->background) {
+        set_error("sgb_lift_batch: shs, colors_precomp and background must be NULL (the maps are the features)");
+        return SGB_E_INVALID;
+    }
+    for (int v = 0; v < V; v++)
+        if (!maps[v]) { set_error("sgb_lift_batch: null map of view %d", v); return SGB_E_INVALID; }
+    // the forward's argument rules with placeholders for the absent colours and background; preprocess only tests
+    // colors_precomp against NULL (to skip the SH colours) and nothing here reads either
+    sgb_view_inputs g = *in;
+    g.colors_precomp = in->means3D;
+    g.background = in->means3D;
+    int rc = check_batch(&g, V, cams);
+    if (rc) return rc;
+    if (in->P == 0) return SGB_OK;
+    return lift_impl(ctx, g, V, cams, maps, map_dtype, feat_sum, weight_sum, (cudaStream_t)stream);
 }
 
 int64_t sgb_ctx_view_stat(const sgb_ctx* ctx, int which) {

@@ -565,8 +565,9 @@ __global__ void __launch_bounds__(kThreads, 2) blend_forward_tma_kernel(
 // costs one claim.  Warp 8 is the producer and warps 0-7 only compute:
 //   * the dL tile of an item, [16 rows][64 ch][16 px] = 64 KB, is ONE 3-D TMA box into one of two buffers.  The
 //     producer issues the next item's box while the current item is being contracted (at its 5th weight slab, when
-//     every warp has provably released the buffer).  Layouts TMA cannot take (W % 4 != 0 or a misaligned base) are
-//     staged by the producer warp with 4-byte cp.async into the same (swizzled) layout, on the same mbarrier;
+//     every warp has provably released the buffer).  Layouts TMA cannot take (a row pitch or base that is not a
+//     multiple of 16 bytes: W % 4 != 0 in fp32, W % 8 != 0 in fp16) are staged by the producer warp into the same
+//     (swizzled) layout on the same mbarrier, with 4-byte cp.async (fp32) or plain loads (fp16);
 //   * the weight rows of a pass (up to 128 entries) stream as 32-pixel slabs, one 3-D TMA box [16 rows][32 px] per
 //     16-entry pool chunk, through a ring of kDfStages stages.
 // Every hand-off is a full/empty mbarrier pair; there is no CTA-wide barrier after the set-up.  Warp w owns channels
@@ -583,7 +584,6 @@ constexpr int kDfStages = 4;                // weight-slab ring depth
 constexpr int kDfThreads = kThreads + 32;   // 8 compute warps + 1 producer warp
 constexpr int kDfPass = 128;                // entries per pass (8 pool chunks)
 constexpr int kDfSlabs = SGB_TILE_PIX / 32;  // 32-pixel K slabs per pass
-constexpr uint32_t kDfTileBytes = SGB_TILE_PIX * kDfCH * 4;
 
 struct DfHdr {  // one weight-ring stage's description, written by the producer before the stage is armed
     int end;            // no more work
@@ -595,14 +595,38 @@ struct DfHdr {  // one weight-ring stage's description, written by the producer 
     int ch0, nch;
     uint32_t gid[kDfPass];  // Gaussian ids of the pass (written for the last slab of a pass)
 };
+// T: element type of dL/dout as it sits in global memory (float, or __half for an fp16 feature map that is lifted
+// onto the Gaussians); the dL tile keeps it in shared memory and is widened to fp32 in the compute warps' loads.
+template <typename T>
 struct DfSmem {  // at a 1024-byte aligned offset of the dynamic shared memory (TMA swizzle atoms)
-    float dl[2][SGB_TILE_PIX * kDfCH];
+    T dl[2][SGB_TILE_PIX * kDfCH];
     float w[kDfStages][kDfPass * 32];
     DfHdr hdr[kDfStages];
     uint64_t wfull[kDfStages], wempty[kDfStages], dfull[2], dempty[2];
 };
-constexpr size_t kDfSmemBytes = sizeof(DfSmem) + 1024;
-static_assert(kDfSmemBytes <= 227 * 1024, "dL/dfeature shared memory exceeds the sm_90 opt-in limit");
+template <typename T>
+constexpr size_t kDfSmemBytes = sizeof(DfSmem<T>) + 1024;
+template <typename T>
+constexpr uint32_t kDfTileBytes = SGB_TILE_PIX * kDfCH * sizeof(T);
+static_assert(kDfSmemBytes<float> <= 227 * 1024, "dL/dfeature shared memory exceeds the sm_90 opt-in limit");
+
+// Pixels 4 (Q & 3) .. 4 (Q & 3) + 3 of tile row Q >> 2, channel cl + k, of an item's dL tile; dl points at channel cl
+// (a multiple of 4) and swz = df_swz<T>(cl).  The tile is the TMA box under its swizzle, 16 px per channel row:
+//   fp32, 64 B rows, SWIZZLE_64B: 4-px quad p of channel c sits at p ^ ((c >> 1) & 3);
+//   fp16, 32 B rows, SWIZZLE_32B: 8-px half h of channel c sits at h ^ ((c >> 2) & 1).
+// Either way channels c and c + 4, the two halves of a warp's load, land in different banks.
+template <typename T>
+__device__ __forceinline__ int df_swz(int cl) { return sizeof(T) == 4 ? (cl >> 1) & 3 : (cl >> 2) & 1; }
+__device__ __forceinline__ float4 df_dl4(const float* dl, int Q, int k, int swz) {
+    return *reinterpret_cast<const float4*>(dl + (Q >> 2) * (kDfCH * 16) + k * 16 + (((Q & 3) ^ swz ^ (k >> 1)) << 2));
+}
+__device__ __forceinline__ float4 df_dl4(const __half* dl, int Q, int k, int swz) {
+    const uint2 r = *reinterpret_cast<const uint2*>(dl + (Q >> 2) * (kDfCH * 16) + k * 16 +
+                                                    ((((Q & 3) >> 1) ^ swz) << 3) + ((Q & 1) << 2));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
 
 __device__ __forceinline__ void cp_async4(void* dst_smem, const void* src, int src_bytes) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes)
@@ -614,18 +638,16 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
 }
 
 // One 32-pixel slab of a pass: acc[j][k] += sum over the slab of w[eg + 16j][px] * dL[px][cl + k].
-// dl points at channel cl of the item's dL buffer, ws at the stage's weight rows; swz = (cl >> 1) & 3.
-template <int R>
-__device__ __forceinline__ void df_slab(float (&acc)[8][4], const float* __restrict__ ws, const float* __restrict__ dl,
+// dl points at channel cl of the item's dL buffer, ws at the stage's weight rows; swz = df_swz<T>(cl).
+template <int R, typename T>
+__device__ __forceinline__ void df_slab(float (&acc)[8][4], const float* __restrict__ ws, const T* __restrict__ dl,
                                         int slab, int eg, int swz) {
 #pragma unroll
     for (int q = 0; q < 8; q++) {
         const int Q = slab * 8 + q;  // pixel quad of the tile: row Q >> 2, quad Q & 3 of the row
         float4 d[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++)
-            d[k] = *reinterpret_cast<const float4*>(dl + (Q >> 2) * (kDfCH * 16) + k * 16 +
-                                                    (((Q & 3) ^ swz ^ (k >> 1)) << 2));
+        for (int k = 0; k < 4; k++) d[k] = df_dl4(dl, Q, k, swz);
 #pragma unroll
         for (int j = 0; j < R; j++) {
             const float4 wv = *reinterpret_cast<const float4*>(ws + (eg + 16 * j) * 32 + ((q ^ (eg & 7)) << 2));
@@ -640,12 +662,13 @@ __device__ __forceinline__ void df_slab(float (&acc)[8][4], const float* __restr
     }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
-    int W, int H, int C, const float* __restrict__ dL_dpixels, PoolView pool, float* __restrict__ dL_dcolors,
+    int W, int H, int C, const T* __restrict__ dL_dpixels, PoolView pool, float* __restrict__ dL_dcolors,
     int* __restrict__ work_counter, const __grid_constant__ CUtensorMap dl_map,
     const __grid_constant__ CUtensorMap w_map, const int use_tma) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    DfSmem& sm = *reinterpret_cast<DfSmem*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+    DfSmem<T>& sm = *reinterpret_cast<DfSmem<T>*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int kComputeWarps = kThreads / 32;
     if (tid == 0) {
@@ -682,17 +705,17 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
             }
             if (warp * 8 < nch) {
                 const float* ws = sm.w[st];
-                const float* dl = sm.dl[dbuf] + cl * 16;
-                const int swz = (cl >> 1) & 3;
+                const T* dl = sm.dl[dbuf] + cl * 16;
+                const int swz = df_swz<T>(cl);
                 switch (R) {
-                    case 1: df_slab<1>(acc, ws, dl, slab, eg, swz); break;
-                    case 2: df_slab<2>(acc, ws, dl, slab, eg, swz); break;
-                    case 3: df_slab<3>(acc, ws, dl, slab, eg, swz); break;
-                    case 4: df_slab<4>(acc, ws, dl, slab, eg, swz); break;
-                    case 5: df_slab<5>(acc, ws, dl, slab, eg, swz); break;
-                    case 6: df_slab<6>(acc, ws, dl, slab, eg, swz); break;
-                    case 7: df_slab<7>(acc, ws, dl, slab, eg, swz); break;
-                    default: df_slab<8>(acc, ws, dl, slab, eg, swz); break;
+                    case 1: df_slab<1, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 2: df_slab<2, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 3: df_slab<3, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 4: df_slab<4, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 5: df_slab<5, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 6: df_slab<6, T>(acc, ws, dl, slab, eg, swz); break;
+                    case 7: df_slab<7, T>(acc, ws, dl, slab, eg, swz); break;
+                    default: df_slab<8, T>(acc, ws, dl, slab, eg, swz); break;
                 }
                 if (slab == kDfSlabs - 1 && cl < nch) {
                     const int ch0 = h.ch0;
@@ -752,12 +775,23 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
         if (items >= 2) mbar_wait(&sm.dempty[it.dbuf], ((items >> 1) - 1) & 1u);  // item `items - 2` released it
         items++;
         const int x0 = (it.tile % tiles_x) * SGB_TILE, y0 = (it.tile / tiles_x) * SGB_TILE;
-        float* dst = sm.dl[it.dbuf];
+        T* dst = sm.dl[it.dbuf];
         if (use_tma) {
             if (lane == 0) {
-                mbar_arrive_expect_tx(&sm.dfull[it.dbuf], kDfTileBytes);
+                mbar_arrive_expect_tx(&sm.dfull[it.dbuf], kDfTileBytes<T>);
                 tma_tile3d_g2s(dst, &dl_map, x0, it.ch0, y0, &sm.dfull[it.dbuf]);
             }
+        } else if constexpr (sizeof(T) == 2) {
+            // cp.async has no 2-byte size: plain loads into the TMA layout, then one release-arrive per lane
+#pragma unroll 8
+            for (int idx = lane; idx < SGB_TILE_PIX * kDfCH; idx += 32) {
+                const int x = idx & (SGB_TILE - 1), r = (idx >> 4) & (SGB_TILE - 1), c = idx >> 8;
+                const int gx = x0 + x, gy = y0 + r;
+                const bool ok = it.ch0 + c < C && gx < W && gy < H;
+                dst[r * (kDfCH * 16) + c * 16 + ((((x >> 3) ^ ((c >> 2) & 1)) << 3) | (x & 7))] =
+                    ok ? dL_dpixels[(size_t)(it.ch0 + c) * plane + (size_t)W * gy + gx] : T(0.f);
+            }
+            mbar_arrive(&sm.dfull[it.dbuf]);
         } else {
             for (int idx = lane; idx < SGB_TILE_PIX * kDfCH; idx += 32) {
                 const int x = idx & (SGB_TILE - 1), r = (idx >> 4) & (SGB_TILE - 1), c = idx >> 8;
@@ -828,6 +862,29 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
     if (lane == 0) {
         sm.hdr[st].end = 1;
         mbar_arrive(&sm.wfull[st]);
+    }
+}
+
+// weight_sum[g] += sum over the tile's pixels of w[entry][px], for every entry of every tile of a view's pool: the
+// denominator of a lift (sgb_lift_batch).  CTA = tile, warp = one 16-entry chunk at a time; every row is read once,
+// by all 32 lanes (two coalesced float4 per lane), and reduced across the warp.
+__global__ void __launch_bounds__(kThreads) pool_weight_sum_kernel(PoolView pool, float* __restrict__ weight_sum) {
+    const int tile = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t n = pool.count[tile];
+    const uint32_t dbase = pool.dirbase[tile];
+    const int nck = (int)((n + kChunkEntries - 1) / kChunkEntries);
+    for (int k = warp; k < nck; k += kThreads / 32) {
+        const WChunk* ck = pool.chunks + chunk_of(pool, dbase, k);
+        const int m = (int)min((uint32_t)kChunkEntries, n - (uint32_t)k * kChunkEntries);
+#pragma unroll 4
+        for (int s = 0; s < m; s++) {
+            const float4 a = __ldg(reinterpret_cast<const float4*>(&ck->w[s][4 * lane]));
+            const float4 b = __ldg(reinterpret_cast<const float4*>(&ck->w[s][128 + 4 * lane]));
+            float t = ((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w));
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+            if (lane == 0) red_add_f32(weight_sum + __ldg(&ck->meta[s].x), t);
+        }
     }
 }
 
@@ -1341,6 +1398,16 @@ int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView*
     return weight_pool_settle(ctx, V, vw, pv, s, miss);
 }
 
+// A lift keeps nothing for a backward: its slots are emptied (not left valid under a scratch address that a later
+// binning state could reuse) and are the first a later build takes, ahead of any training forward's slot.
+void weight_pool_release(sgb_ctx* ctx, int V, const ViewState* vw) {
+    for (int v = 0; v < V; v++)
+        if (PoolSlot* sl = slot_of(ctx, vw[v])) {
+            sl->valid = false;
+            sl->key_bin = nullptr;
+        }
+}
+
 // Forward GEMM of one view.  The host waited for the alpha passes only, so the caller keeps enqueueing the rest of
 // its step while the GEMM runs.
 int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s) {
@@ -1370,20 +1437,24 @@ int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float
     return SGB_OK;
 }
 
-// dL/dout (C, H, W) fp32 for dfeature_persistent_kernel, described with its dimensions in the order (x, channel, y) so
-// that one [16 px][64 ch][16 rows] box lands as [row][ch][16 px] under the 64-byte swizzle.  Returns false (the kernel
-// then stages the tile with cp.async) when the layout does not meet the TMA rules (base and row pitch multiples of 16
-// bytes) or the driver entry point is not available.
-static bool encode_dfeature_dl_map(CUtensorMap* map, const float* dL_dpix, int W, int H, int C) {
+// dL/dout (C, H, W), fp32 or fp16, for dfeature_persistent_kernel<T>, described with its dimensions in the order
+// (x, channel, y) so that one [16 px][64 ch][16 rows] box lands as [row][ch][16 px] under the swizzle df_dl4 reads
+// (64-byte rows of fp32, 32-byte rows of fp16).  Returns false (the kernel then stages the tile itself) when the layout
+// does not meet the TMA rules (base and row pitch multiples of 16 bytes: W % 4 == 0 in fp32, W % 8 == 0 in fp16) or
+// the driver entry point is not available.
+template <typename T>
+static bool encode_dfeature_dl_map(CUtensorMap* map, const T* dL_dpix, int W, int H, int C) {
     const TensorMapEncodeFn encode = tensor_map_encoder();
     memset(map, 0, sizeof(*map));
-    if (!encode || (W & 3) != 0 || (reinterpret_cast<uintptr_t>(dL_dpix) & 15) != 0) return false;
+    if (!encode || ((size_t)W * sizeof(T)) % 16 != 0 || (reinterpret_cast<uintptr_t>(dL_dpix) & 15) != 0) return false;
     const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)C, (cuuint64_t)H};
-    const cuuint64_t strides[2] = {(cuuint64_t)W * H * sizeof(float), (cuuint64_t)W * sizeof(float)};
+    const cuuint64_t strides[2] = {(cuuint64_t)W * H * sizeof(T), (cuuint64_t)W * sizeof(T)};
     const cuuint32_t box[3] = {SGB_TILE, kDfCH, SGB_TILE};
     const cuuint32_t estr[3] = {1, 1, 1};
-    return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(dL_dpix), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+    const bool f32 = sizeof(T) == 4;
+    return encode(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+                  const_cast<T*>(dL_dpix), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  f32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -1402,7 +1473,8 @@ static bool encode_dfeature_w_map(CUtensorMap* map, const PoolView& pv) {
                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+template <typename T>
+int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const T* dL_dpix,
                                float* dL_dcolors, cudaStream_t s) {
     const sgb_view_inputs& in = w.in;
     const int items = num_tiles(in) * ((in.C + kDfCH - 1) / kDfCH);
@@ -1422,11 +1494,11 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView&
     SGB_CUDA(cudaGetDevice(&dev));
     int& grid = grid_of_device[dev < 64 ? dev : 63];
     if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(dfeature_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)kDfSmemBytes));
+        SGB_CUDA(cudaFuncSetAttribute(dfeature_persistent_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)kDfSmemBytes<T>));
         int per_sm = 0, sms = 0;
-        SGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dfeature_persistent_kernel, kDfThreads,
-                                                               kDfSmemBytes));
+        SGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dfeature_persistent_kernel<T>, kDfThreads,
+                                                               kDfSmemBytes<T>));
         SGB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         grid = per_sm * sms > 0 ? per_sm * sms : 1;
     }
@@ -1434,9 +1506,22 @@ int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView&
     StageTimer t(ctx, ST_DFEATURE, s);
     SGB_CUDA(cudaMemsetAsync(counter, 0, sizeof(int), s));
     ctx->launches += 1;
-    dfeature_persistent_kernel<<<grid < items ? grid : items, kDfThreads, kDfSmemBytes, s>>>(
+    dfeature_persistent_kernel<T><<<grid < items ? grid : items, kDfThreads, kDfSmemBytes<T>, s>>>(
         in.W, in.H, in.C, dL_dpix, pv, dL_dcolors, counter, dl_map, w_map, use_tma);
     SGB_LAUNCH_CHECK("dfeature_persistent_kernel", in.debug, s);
+    return SGB_OK;
+}
+
+template int blend_backward_v3_dfeature<float>(sgb_ctx*, const ViewState&, const PoolView&, const float*, float*,
+                                               cudaStream_t);
+template int blend_backward_v3_dfeature<__half>(sgb_ctx*, const ViewState&, const PoolView&, const __half*, float*,
+                                                cudaStream_t);
+
+int pool_weight_sums(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* weight_sum, cudaStream_t s) {
+    StageTimer t(ctx, ST_WEIGHT_SUM, s);
+    ctx->launches += 1;
+    pool_weight_sum_kernel<<<num_tiles(w.in), kThreads, 0, s>>>(pv, weight_sum);
+    SGB_LAUNCH_CHECK("pool_weight_sum_kernel", w.in.debug, s);
     return SGB_OK;
 }
 

@@ -3,6 +3,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include "../../include/sgb200.h"
 
@@ -139,7 +140,7 @@ namespace sgb {
 enum Stage {
     ST_PREPROCESS = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_TILE_SORT, ST_RANGES, ST_BLEND_FWD,
     ST_BLEND_BWD, ST_GEOM_BWD, ST_FUSION_PROJECT, ST_FUSION_SORT, ST_FUSION_GATHER, ST_ALPHA, ST_DFEATURE,
-    ST_COUNT
+    ST_WEIGHT_SUM, ST_COUNT
 };
 constexpr int kProfRing = 320;
 struct Profiler {
@@ -178,6 +179,8 @@ struct sgb_ctx {
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
     sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
     sgb::Scratch depth_grad;  // [P] dL/d(view-space z) of the view being differentiated (expected-depth backward)
+    sgb::Scratch lift_state;  // sgb_lift_batch: geometry state, radii and image state of every view of the call
+    sgb::Scratch lift_bin;    // sgb_lift_batch: binning states of the views
     // Per-tile weight rows of the C-channel blend (blend_v3.cu).  As many slots as views per batch: the backward
     // resolves the rows of all V views before its first kernel, and V <= slots guarantees that rebuilding one view
     // cannot evict another view of the same batch.
@@ -275,9 +278,14 @@ int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s);
 int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s,
                        const bool* only = nullptr);
 int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s);
+void weight_pool_release(sgb_ctx* ctx, int V, const ViewState* vw);
 int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s);
-int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
+// dL_dcolors[g][c] += sum_px w * dL_dpix[c][px]; T = float for a backward, float or __half for a lift's feature map
+template <typename T>
+int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const T* dL_dpix,
                                float* dL_dcolors, cudaStream_t s);
+// weight_sum[g] += sum_px w over every entry of the view's pool (the denominator of a lift)
+int pool_weight_sums(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* weight_sum, cudaStream_t s);
 int blend_backward_v3_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
                             float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, cudaStream_t s);
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,

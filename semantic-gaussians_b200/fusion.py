@@ -4,6 +4,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Union
 
 import numpy as np
@@ -204,3 +205,137 @@ def fuse_scene(gaussians, views, feature_maps, pipe, background, img_dim, visibi
         mask = count > 0
         normalize_fused(gaussians._features_semantic, count)
     return {"features": gaussians._features_semantic, "mask": mask, "views": fused}
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Fusion by blend weights: the adjoint of rendering (sgb_lift_batch, include/sgb200.h)
+
+def _lift_map(m, idx, Cn, dev, hw):
+    """The (C, h, w) map of view idx as the native call reads it; raises on anything it would misread."""
+    if not isinstance(m, torch.Tensor):
+        raise TypeError(f"feature map {idx} must be a torch.Tensor, got {type(m).__name__}")
+    if m.dtype not in (torch.float16, torch.float32):
+        raise TypeError(f"feature map {idx} must be float16 or float32, got {m.dtype}")
+    if m.device != dev:
+        raise ValueError(f"feature map {idx} is on {m.device}, expected {dev}")
+    if m.ndim != 3 or m.shape[0] != Cn or m.shape[1] < 1 or m.shape[2] < 1:
+        raise ValueError(f"feature map {idx} must be (C={Cn}, h, w), got {tuple(m.shape)}")
+    if hw is not None and tuple(m.shape[1:]) != hw:
+        raise ValueError(f"feature map {idx} is {tuple(m.shape[1:])}, the other maps of the call are {hw}: the "
+                         f"views of one call share the render size")
+    return m.contiguous()
+
+
+def lift_views(gaussians, views, feature_maps, pipe, feat_sum: torch.Tensor, weight_sum: torch.Tensor,
+               scaling_modifier: float = 1.0) -> int:
+    """Lift 2D feature maps onto the Gaussians by their blend weights, accumulating
+
+        feat_sum[i]  += sum_v sum_p w_i^v(p) F_v[:, p]          weight_sum[i] += sum_v sum_p w_i^v(p)
+
+    where w_i^v(p) = alpha_i T_i is the weight with which the render of view v composites Gaussian i into pixel p (0
+    where it is occluded or outside its footprint).  feat_sum is the feature gradient a render_chn backward with the
+    map as dL/dout would give, without the colour blend and the rest of the backward; normalize_fused(feat_sum,
+    weight_sum) turns it into the weighted mean of the map over the pixels each Gaussian shows in.
+
+    gaussians     GaussianModel-like (get_xyz, get_opacity, get_scaling, get_rotation, get_covariance)
+    views         cameras (FoVx, FoVy, world_view_transform, full_proj_transform, camera_center)
+    feature_maps  sequence, or callable idx -> map, of (C, h, w) float16 / float32 tensors on the Gaussians' device;
+                  views are rendered at the map size (render()'s override_shape), which all maps of a call share
+    pipe          compute_cov3d_python and debug are honoured as in render_chn_batch
+    feat_sum      (P, C) and weight_sum (P,) or (P, 1): contiguous float32 on the Gaussians' device, added into
+
+    The views go to the native call in batches of at most 8 consecutive views whose maps share a dtype.  A sequence
+    of maps is checked in full before the first native call, a callable's maps batch by batch as they are fetched:
+    TypeError for a non-tensor or a dtype other than float16 / float32, ValueError for a wrong shape or device or a
+    map size that differs from the call's first map.  Returns the number of views lifted."""
+    from . import channel_rasterization as chn
+    from .rasterizer import _cameras, _make_inputs, _ptrs, _stream_ctx
+    from .renderer import _prepare
+    views = list(views)
+    xyz = gaussians.get_xyz
+    dev, P = xyz.device, xyz.shape[0]
+    for name, t, shape in (("feat_sum", feat_sum, None), ("weight_sum", weight_sum, (P,))):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+            raise TypeError(f"{name} must be a float32 tensor")
+        if t.device != dev:
+            raise ValueError(f"{name} is on {t.device}, expected {dev}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be contiguous (it is accumulated in place)")
+    if feat_sum.ndim != 2 or feat_sum.shape[0] != P:
+        raise ValueError(f"feat_sum must be (P={P}, C), got {tuple(feat_sum.shape)}")
+    if weight_sum.numel() != P:
+        raise ValueError(f"weight_sum must hold P={P} entries, got {tuple(weight_sum.shape)}")
+    Cn = feat_sum.shape[1]
+    fetch = feature_maps if callable(feature_maps) else feature_maps.__getitem__
+    hw = None
+    if not callable(feature_maps):
+        if len(feature_maps) < len(views):
+            raise ValueError(f"{len(views)} views but {len(feature_maps)} feature maps")
+        for i in range(len(views)):
+            hw = tuple(_lift_map(feature_maps[i], i, Cn, dev, hw).shape[1:])
+    if not xyz.is_cuda:
+        raise ValueError(f"the Gaussians are on {dev}: lifting runs on a CUDA device only (there is no CPU path)")
+    if not views:
+        return 0
+    lib = _lib.load()
+    debug = bool(getattr(pipe, "debug", False))
+    with torch.no_grad(), torch.cuda.device(dev):
+        i = 0
+        bg = carry = None   # carry: a fetched map of the other dtype, the first of the next batch
+        while i < len(views):
+            maps = [carry if carry is not None else _lift_map(fetch(i), i, Cn, dev, hw)]
+            carry = None
+            hw = tuple(maps[0].shape[1:])
+            while i + len(maps) < len(views) and len(maps) < _lib.MAX_BATCH:
+                m = _lift_map(fetch(i + len(maps)), i + len(maps), Cn, dev, hw)
+                if m.dtype != maps[0].dtype:
+                    carry = m
+                    break
+                maps.append(m)
+            h, w = hw
+            batch = views[i:i + len(maps)]
+            if bg is None:
+                # the Gaussian-side tensors once per call, as render_chn_batch prepares them; any override colour
+                # keeps _prepare from evaluating SH colours, which a lift does not read
+                _, common0, call = _prepare(batch[0], gaussians, pipe, scaling_modifier, override_color=feat_sum,
+                                            override_shape=(w, h), foreground=None, world_rotate=None)
+                bg = torch.zeros(Cn, device=dev)   # _make_inputs wants a background; the native call takes none
+            settings = [chn.GaussianRasterizationSettings(
+                bg=bg, debug=debug, num_channels=Cn,
+                **dict(common0, tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5),
+                       viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform,
+                       campos=cam.camera_center)) for cam in batch]
+            inp, cameras, keep, _ = _make_inputs(_cameras(settings), bg, call["means3D"], None,
+                                                 call["opacities"], call["scales"], call["rotations"], scaling_modifier,
+                                                 call["cov3D_precomp"], h, w, None, 0, False, debug, Cn)
+            inp.background = None
+            stream, ctx = _stream_ctx(dev)
+            dt = _lib.FEAT_F16 if maps[0].dtype == torch.float16 else _lib.FEAT_F32
+            _lib.check(lib.sgb_lift_batch(ctx, C.byref(inp), len(maps), cameras, _ptrs(maps), dt,
+                                          feat_sum.data_ptr(), weight_sum.data_ptr(), stream), "sgb_lift_batch")
+            i += len(maps)
+    return len(views)
+
+
+def lift_scene(gaussians, views, feature_maps, pipe, every: int = 5) -> dict:
+    """The counterpart of fuse_scene that needs no depth map, visibility threshold or boundary cut: every view
+    ``idx % every == 0`` is lifted with lift_views (occlusion comes from the render's transmittance), and each
+    Gaussian gets the weighted mean of the feature-map pixels it shows in.
+
+    Writes the means into ``gaussians._features_semantic`` (create_semantic(C) first) and the weight sums into
+    ``gaussians._times``.  Returns {"features": (P, C) float32, "mask": (P,) bool, weight sum > 0 (a Gaussian no
+    lifted pixel shows has features 0), "views": number of lifted views, "weights": (P,) float32 weight sums}, which
+    io_formats.save_fused_features and the evaluation code take as they take fuse_scene's result."""
+    if getattr(gaussians, "_features_semantic", None) is None or gaussians._features_semantic.numel() == 0:
+        raise ValueError("call gaussians.create_semantic(C) first")
+    views = list(views)
+    sel = list(range(0, len(views), every))
+    maps = (lambda k: feature_maps(sel[k])) if callable(feature_maps) else [feature_maps[i] for i in sel]
+    feats, weights = gaussians._features_semantic, gaussians._times.view(-1)
+    with torch.no_grad():
+        feats.zero_()
+        weights.zero_()
+        n = lift_views(gaussians, [views[i] for i in sel], maps, pipe, feats, weights)
+        mask = weights > 0
+        normalize_fused(feats, weights.clone())   # the normaliser marks zero sums 1e-5; the weights stay as summed
+    return {"features": feats, "mask": mask, "views": n, "weights": weights}
