@@ -459,6 +459,45 @@ int sgb_photometric_backward(int32_t planes, int32_t h, int32_t w, const float* 
                              const float* partials, const float* coef, float* dL_dx, int64_t dx_plane_stride,
                              int64_t dx_row_stride, void* stream);
 
+/* ---- optimizer step: torch.optim.Adam (no amsgrad, no weight_decay, maximize=False) over up to
+ * SGB_ADAM_MAX_TENSORS parameter tables in ONE kernel launch, with an optional per-row visibility mask.
+ *
+ * A tensor is `rows` rows of `row_len` contiguous fp32 values (for a Gaussian table: one row per Gaussian).  Per
+ * element of a row that is stepped, in fp32:
+ *     m = m + (g - m) * (1 - beta1)          v = beta2 * v + (1 - beta2) * g * g
+ *     p = p - step_size * (m / (sqrtf(v) / bias_correction2_sqrt + eps))
+ * with IEEE sqrtf and division.  step_size = lr / (1 - beta1^t) and bias_correction2_sqrt = sqrt(1 - beta2^t) are
+ * the caller's, computed in double from its step count t.
+ *
+ * visible: NULL steps every row.  Otherwise row r is stepped where visible[r] != 0; of a row with visible[r] == 0
+ * only that byte is read: no element of param / grad / exp_avg / exp_avg_sq is loaded or stored (so they stay
+ * bitwise as they were, and a NaN in such a row's gradient is never seen).  This is 3DGS's `sparse_adam` rule, with
+ * the bias corrections kept.
+ *
+ * The descriptors are host memory and travel as kernel parameters: nothing is copied to the device.  Rows are
+ * accessed 16 bytes wide where row_len % 4 == 0 and the four base pointers are 16-byte aligned (a tensor without a
+ * mask is one flat run, so there rows * row_len % 4 == 0 is enough); any other layout takes a scalar path with the
+ * same result.  No ctx, no scratch, no host synchronisation; asynchronous on `stream`; the same inputs give bitwise
+ * identical outputs.  Tensors with rows == 0 are skipped and a call with no work launches nothing.
+ *
+ * SGB_E_INVALID, before anything is enqueued: n outside [0, SGB_ADAM_MAX_TENSORS]; tensors NULL with n > 0; and per
+ * tensor rows < 0, row_len < 1, a NULL param / grad / exp_avg / exp_avg_sq with rows > 0, beta1 or beta2 outside
+ * [0, 1), eps < 0, a non-finite step_size, bias_correction2_sqrt outside (0, 1]. */
+#define SGB_ADAM_MAX_TENSORS 8
+typedef struct sgb_adam_tensor {
+    float* param;                /* (rows, row_len) */
+    const float* grad;           /* (rows, row_len) */
+    float* exp_avg;              /* (rows, row_len) first moment m */
+    float* exp_avg_sq;           /* (rows, row_len) second moment v */
+    const uint8_t* visible;      /* [rows], 0 = skip the row; NULL = every row */
+    int64_t rows;
+    int32_t row_len;
+    double beta1, beta2, eps;    /* double as torch holds them: the kernel uses fp32(1 - beta), not 1 - fp32(beta) */
+    float step_size;             /* lr / (1 - beta1^t) */
+    float bias_correction2_sqrt; /* sqrt(1 - beta2^t) */
+} sgb_adam_tensor;
+int sgb_adam_step(const sgb_adam_tensor* tensors_host, int32_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -58,6 +58,17 @@ class FusionView(C.Structure):
     ]
 
 
+ADAM_MAX_TENSORS = 8
+
+
+class AdamTensor(C.Structure):
+    """sgb_adam_tensor: one (rows, row_len) fp32 parameter table of an sgb_adam_step call."""
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
+                ("visible", C.c_void_p), ("rows", C.c_int64), ("row_len", C.c_int32),
+                ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+                ("step_size", C.c_float), ("bias_correction2_sqrt", C.c_float)]
+
+
 EXPORTS = (
     "sgb_last_error", "sgb_version", "sgb_ctx_create", "sgb_ctx_destroy", "sgb_ctx_scratch_bytes",
     "sgb_geometry_bytes", "sgb_binning_bytes", "sgb_image_bytes", "sgb_forward_geometry",
@@ -69,6 +80,7 @@ EXPORTS = (
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
     "sgb_forward_render_batch_ext", "sgb_backward_batch_ext", "sgb_decoded_feature_loss",
     "sgb_decoded_feature_loss_workspace_bytes", "sgb_voxelize", "sgb_voxelize_workspace_bytes", "sgb_lift_batch",
+    "sgb_adam_step",
 )
 
 _lib = None
@@ -149,6 +161,7 @@ def load() -> C.CDLL:
         lib.sgb_voxelize.argtypes = [i64, vp, C.POINTER(C.c_double), vp, vp, vp, vp, vp, vp]
         lib.sgb_voxelize_workspace_bytes.argtypes = [i64]
         lib.sgb_voxelize_workspace_bytes.restype = C.c_size_t
+        lib.sgb_adam_step.argtypes = [C.POINTER(AdamTensor), i32, vp]
         _lib = lib
         return lib
 

@@ -56,7 +56,14 @@ class DensifyMixin:
             p = nn.Parameter(getattr(self, attr).detach().clone().requires_grad_(True))
             setattr(self, attr, p)
             groups.append({"params": [p], "lr": lrs[name], "name": name})
-        self.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+        optimizer_type = getattr(training_args, "optimizer_type", "default")
+        if optimizer_type == "default":
+            self.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+        elif optimizer_type == "sparse_adam":  # 3DGS's name: step(visibility=...) leaves unseen Gaussians alone
+            from .optim import GaussianAdam
+            self.optimizer = GaussianAdam([dict(g, row_sparse=True) for g in groups], lr=0.0, eps=1e-15)
+        else:
+            raise ValueError(f"optimizer_type must be 'default' or 'sparse_adam', got {optimizer_type!r}")
         self._xyz_lr = expon_lr(training_args.position_lr_init * scale, training_args.position_lr_final * scale,
                                 training_args.position_lr_max_steps, delay_mult=training_args.position_lr_delay_mult)
 
