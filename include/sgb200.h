@@ -34,6 +34,11 @@
  *     geomBuffer/binningBuffer/imgBuffer (rasterize_points.cu:28-36,73-80), but sized up
  *     front through sgb_*_bytes() instead of std::function resize callbacks.  Scratch that does
  *     not outlive a call (sort double-buffers, CUB temp storage) lives in the sgb_ctx.
+ *   - Render and backward read only the states, radii and num_rendered they are given, which must
+ *     come from one geometry call for the same inputs (as in the reference).  Calls may interleave
+ *     on a ctx, and a render may run on another ctx than its geometry call.  The one thing a ctx
+ *     carries from call to call is the weight-pool cache of the C > 4 blend: keyed by binning
+ *     state, checked on use and rebuilt on a miss.
  *   - A ctx is bound to one device and must not be used by two streams concurrently.
  */
 #ifndef SGB200_H_INCLUDED

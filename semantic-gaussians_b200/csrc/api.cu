@@ -191,8 +191,6 @@ static int forward_geometry_impl(sgb_ctx* ctx, const sgb_view_inputs& in, int V,
                                  void* const* geometry_states, int32_t* const* radii, int64_t* num_rendered_host,
                                  cudaStream_t s) {
     for (int v = 0; v < V; v++) num_rendered_host[v] = 0;
-    ctx->last_P = 0;
-    ctx->last_V = 0;
     if (in.P == 0) return SGB_OK;  // rasterize_points.cu:84: nothing to do for an empty scene
     int rc = run_depth_order_and_scan(ctx, in, V, cams, geometry_states, radii, num_rendered_host, s);
     if (rc) return rc;
@@ -218,7 +216,7 @@ static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, i
     for (int v = 0; v < V; v++) {
         ViewState& w = vw[v];
         w = ViewState::carve(in_common, cams[v], num_rendered[v], geometry_states[v], binning_states[v], image_states[v]);
-        rc = run_binning(ctx, w.in, v, w.R, w.g, w.b, w.im, radii[v], s);
+        rc = run_binning(ctx, w.in, w.R, w.g, w.b, w.im, radii[v], s);
         if (rc) return rc;
         if (wide) {
             rc = weight_pool_build(ctx, w, s);
@@ -482,7 +480,7 @@ static int lift_impl(sgb_ctx* ctx, const sgb_view_inputs& in, int V, const sgb_c
         ViewState& w = vw[nv];
         w = ViewState::carve(in, cams[v], R[v], geom[v], (char*)ctx->lift_bin.p + bin_off, img[v]);
         bin_off += sgb_binning_bytes(R[v]);
-        rc = run_binning(ctx, w.in, v, w.R, w.g, w.b, w.im, radii[v], s);
+        rc = run_binning(ctx, w.in, w.R, w.g, w.b, w.im, radii[v], s);
         if (!rc) rc = weight_pool_build(ctx, w, s);
         if (rc) {
             weight_pool_release(ctx, nv + 1, vw);

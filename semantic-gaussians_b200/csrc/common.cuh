@@ -46,6 +46,8 @@ struct GeomView {  // carved out of geometry_state (caller-owned, P-sized)
     float* rgb;              // [P,3]   SH path only
     uint8_t* clamped;        // [P,3]
     uint32_t* tiles_touched; // [P]
+    uint32_t* perm;          // [P] Gaussian ids in (depth bits, id) order
+    uint32_t* offsets;       // [P] inclusive scan of tiles_touched in that order (GeometryState::point_offsets)
     size_t bytes;
     static GeomView carve(void* base, int64_t P) {
         GeomView g;
@@ -56,6 +58,8 @@ struct GeomView {  // carved out of geometry_state (caller-owned, P-sized)
         g.rgb = (float*)(p + off); off += align_up(sizeof(float) * 3 * P);
         g.clamped = (uint8_t*)(p + off); off += align_up(3 * (size_t)P);
         g.tiles_touched = (uint32_t*)(p + off); off += align_up(sizeof(uint32_t) * P);
+        g.perm = (uint32_t*)(p + off); off += align_up(sizeof(uint32_t) * P);
+        g.offsets = (uint32_t*)(p + off); off += align_up(sizeof(uint32_t) * P);
         g.bytes = off;
         return g;
     }
@@ -174,7 +178,7 @@ struct sgb_ctx {
     sgb::Profiler prof;
     uint64_t launches = 0;       // kernels of this library launched through this ctx
     uint64_t lib_launches = 0;   // CUB device-wide calls (each several kernels)
-    sgb::Scratch geom;     // depth-sort keys/values, offsets, CUB temp (one slice per view of a batch)
+    sgb::Scratch geom;     // depth-sort keys, iota values, CUB temp, 64-bit instance total (shared by a batch's views)
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
     sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
@@ -191,11 +195,6 @@ struct sgb_ctx {
     int64_t stat_blended_pairs = 0;  // last alpha pass: blended (pixel, Gaussian) pairs
     int64_t stat_pool_chunks = 0;    // last alpha pass: 16-entry weight-row chunks in use
     cudaEvent_t feature_grad_event = nullptr;  // caller-owned; recorded when dL_dcolors is final (sgb200.h)
-    // cached layout of the last sgb_forward_geometry[_batch] call (consumed by sgb_forward_render[_batch])
-    int64_t last_P = 0;
-    int last_V = 0;
-    uint32_t* d_perm[SGB_MAX_BATCH] = {};     // [P] Gaussian ids in (depth bits, id) order, per view of the batch
-    uint32_t* d_offsets[SGB_MAX_BATCH] = {};  // [P] inclusive scan of tiles_touched in that order
 };
 
 namespace sgb {
@@ -248,12 +247,12 @@ inline TensorMapEncodeFn tensor_map_encoder() {
 int launch_preprocess(const sgb_view_inputs& in, GeomView g, int32_t* radii, uint32_t* depth_keys,
                       cudaStream_t s);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t s);
-// Depth order + scan of V views of the same Gaussians (cams[v] replaces the camera fields of `in`): everything is
-// enqueued back to back, ONE stream sync reads all R.
+// Depth order + scan of V views of the same Gaussians (cams[v] replaces the camera fields of `in`) into each view's
+// geometry state: everything is enqueued back to back, ONE stream sync reads all R.
 int run_depth_order_and_scan(sgb_ctx* ctx, const sgb_view_inputs& in, int V, const sgb_camera* cams,
                              void* const* geometry_states, int32_t* const* radii, int64_t* R_host, cudaStream_t s);
 int reserve_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, cudaStream_t s);
-int run_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int view_slot, int64_t R, GeomView g, BinView b, ImgView im,
+int run_binning(sgb_ctx* ctx, const sgb_view_inputs& in, int64_t R, GeomView g, BinView b, ImgView im,
                 const int32_t* radii, cudaStream_t s);
 // C <= 4 blend.  out_exp_depth / out_alpha (given together or not at all): expected depth and accumulated opacity.
 // dL_ddepth non-null selects the backward with those two extra channels (either upstream plane may be null = zero);

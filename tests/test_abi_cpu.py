@@ -40,7 +40,7 @@ def test_library_contains_sm90a_code_with_bulk_and_tensor_copies():
 
 def test_state_sizes_are_sane():
     lib = _lib.load()
-    assert lib.sgb_geometry_bytes(1_000_000) >= 1_000_000 * (32 + 24 + 12 + 3 + 4)
+    assert lib.sgb_geometry_bytes(1_000_000) >= 1_000_000 * (32 + 24 + 12 + 3 + 4 + 4 + 4)
     assert lib.sgb_geometry_bytes(1_000_000) < 1_000_000 * 100          # reference: ~79 B / Gaussian + scan temp
     assert lib.sgb_binning_bytes(10_000_000) >= 40_000_000              # 4 B / instance (reference: 24 B + temp)
     assert lib.sgb_binning_bytes(10_000_000) < 41_000_000
