@@ -3,7 +3,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "common.cuh"
-#include "blend_pool.cuh"
+#include "chn_blend.cuh"
 
 namespace sgb {
 
@@ -87,9 +87,10 @@ int sgb_ctx_create(sgb_ctx** out, int device) {
     SGB_CUDA(cudaSetDevice(device));
     sgb_ctx* c = new sgb_ctx();
     c->device = device;
-    cudaError_t e = cudaMallocHost(&c->pinned, 1024);
+    c->pools = new WeightPools();
+    cudaError_t e = cudaMallocHost(&c->pinned, sizeof(Readback));
     if (prev >= 0 && prev != device) cudaSetDevice(prev);
-    if (e != cudaSuccess) { delete c; return cuda_fail(e, "cudaMallocHost"); }
+    if (e != cudaSuccess) { sgb_ctx_destroy(c); return cuda_fail(e, "cudaMallocHost"); }
     *out = c;
     return SGB_OK;
 }
@@ -109,8 +110,7 @@ void sgb_ctx_destroy(sgb_ctx* c) {
     if (c->depth_grad.p) cudaFree(c->depth_grad.p);
     if (c->lift_state.p) cudaFree(c->lift_state.p);
     if (c->lift_bin.p) cudaFree(c->lift_bin.p);
-    for (PoolSlot& sl : c->pools)
-        if (sl.mem.p) cudaFree(sl.mem.p);
+    delete c->pools;
     if (c->pinned) cudaFreeHost(c->pinned);
     delete c;
 }
@@ -160,10 +160,8 @@ uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
 
 size_t sgb_ctx_scratch_bytes(const sgb_ctx* c) {
     if (!c) return 0;
-    size_t n = c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap + c->lift_state.cap +
-               c->lift_bin.cap;
-    for (const PoolSlot& sl : c->pools) n += sl.mem.cap;
-    return n;
+    return c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap + c->lift_state.cap +
+           c->lift_bin.cap + c->pools->bytes();
 }
 
 size_t sgb_geometry_bytes(int32_t P) { return GeomView::carve(nullptr, P > 0 ? P : 1).bytes; }
@@ -236,7 +234,7 @@ static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, i
     rc = weight_pool_settle(ctx, V, vw, pv, s);
     if (rc) return rc;
     for (int v = 0; v < V; v++) {
-        rc = blend_forward_v3(ctx, vw[v], pv[v], out_colors[v], s);
+        rc = chn_forward(ctx, vw[v], pv[v], out_colors[v], s);
         if (rc) return rc;
     }
     return SGB_OK;
@@ -281,7 +279,7 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, 
         if (rc) return rc;
         for (int v = 0; v < V; v++) {
             if (vw[v].R <= 0) continue;
-            rc = blend_backward_v3_dfeature(ctx, vw[v], pv[v], dL_dpix[v], grads[v].dL_dcolors, s);
+            rc = chn_dfeature(ctx, vw[v], pv[v], dL_dpix[v], grads[v].dL_dcolors, s);
             if (rc) return rc;
         }
         if (ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
@@ -289,7 +287,7 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in_common, int V, 
     for (int v = 0; v < V; v++) {
         const sgb_view_grads& gr = grads[v];
         if (vw[v].R > 0 && wide) {
-            rc = blend_backward_v3_chain(ctx, vw[v], pv[v], dL_dpix[v], gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dopacity, s);
+            rc = chn_chain(ctx, vw[v], pv[v], dL_dpix[v], gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dopacity, s);
             if (rc) return rc;
         } else if (vw[v].R > 0) {
             if (dL_ddepth) SGB_CUDA(cudaMemsetAsync(dL_ddepth, 0, sizeof(float) * (size_t)in_common.P, s));
@@ -493,9 +491,9 @@ static int lift_impl(sgb_ctx* ctx, const sgb_view_inputs& in, int V, const sgb_c
     for (int k = 0, v = 0; !rc && v < V; v++) {
         if (R[v] == 0) continue;
         if (map_dtype == SGB_FEAT_F16)
-            rc = blend_backward_v3_dfeature(ctx, vw[k], pv[k], static_cast<const __half*>(maps[v]), feat_sum, s);
+            rc = chn_dfeature(ctx, vw[k], pv[k], static_cast<const __half*>(maps[v]), feat_sum, s);
         else
-            rc = blend_backward_v3_dfeature(ctx, vw[k], pv[k], static_cast<const float*>(maps[v]), feat_sum, s);
+            rc = chn_dfeature(ctx, vw[k], pv[k], static_cast<const float*>(maps[v]), feat_sum, s);
         if (!rc) rc = pool_weight_sums(ctx, vw[k], pv[k], weight_sum, s);
         k++;
     }
@@ -533,7 +531,7 @@ int sgb_lift_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb
 
 int64_t sgb_ctx_view_stat(const sgb_ctx* ctx, int which) {
     if (!ctx) return -1;
-    return which == 0 ? ctx->stat_blended_pairs : which == 1 ? ctx->stat_pool_chunks : -1;
+    return which == 0 ? ctx->pools->stat_blended_pairs : which == 1 ? ctx->pools->stat_pool_chunks : -1;
 }
 
 int sgb_ctx_set_feature_grad_event(sgb_ctx* ctx, void* cuda_event) {

@@ -14,6 +14,7 @@
 // result is identical while the R-sized traffic drops from ~6x(12+12) B to 2x(8+8) B per instance.
 #include <cub/cub.cuh>
 #include "common.cuh"
+#include "weight_pool.cuh"
 
 namespace sgb {
 
@@ -162,7 +163,7 @@ int run_depth_order_and_scan(sgb_ctx* ctx, const sgb_view_inputs& in_common, int
     uint32_t* vals_in = (uint32_t*)(base + 2 * arr);
     void* cub_tmp = base + 3 * arr;
     unsigned long long* total64 = (unsigned long long*)(base + 3 * arr + tmp);
-    unsigned long long* h = (unsigned long long*)ctx->pinned;
+    unsigned long long* h = ctx->pinned->num_rendered;
     for (int v = 0; v < V; v++) {
         const sgb_view_inputs in = with_camera(in_common, cams[v]);
         GeomView g = GeomView::carve(geometry_states[v], P);

@@ -4,7 +4,7 @@
 // One CTA per 16x16 tile, thread = pixel, Gaussians staged in shared memory per batch like the
 // reference.  The per-pixel alpha / transmittance chain and the accumulation `C[ch] += f*alpha*T`
 // are the reference's statement sequence verbatim, so pixels, depth, final_T and n_contrib are
-// bit-identical.  Wider rasters go through blend_v3.cu.
+// bit-identical.  Wider rasters go through the weights-once pipeline (chn_blend.cuh).
 //
 // With EXP_ALPHA the walk also accumulates, with the colour channels' own statement, the expected depth
 // E = sum_i z_i alpha_i T_i and the accumulated opacity A = sum_i alpha_i T_i (no background term): E and A are
@@ -171,7 +171,7 @@ int launch_one(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, con
 int launch_blend_forward(const sgb_view_inputs& in, GeomView g, BinView b, ImgView im, const float* colors,
                          float* out_color, float* out_depth, float* out_exp_depth, float* out_alpha, cudaStream_t s) {
     // RGB / RGB-D path (C <= 4): the reference's accumulation order, bit for bit.  Wider rasters go
-    // through the weights-once pipeline in blend_v3.cu.
+    // through the weights-once pipeline (chn_blend.cuh).
     if (in.C > 4) {
         set_error("launch_blend_forward handles C <= 4 only");
         return SGB_E_INVALID;

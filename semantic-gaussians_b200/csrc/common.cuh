@@ -2,7 +2,6 @@
 #pragma once
 #include <cstdint>
 #include <cstdio>
-#include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include "../../include/sgb200.h"
@@ -135,9 +134,7 @@ struct Scratch {
     int ensure(size_t n);  // grows (cudaFree + cudaMalloc); returns SGB_OK / SGB_E_NOMEM
 };
 
-}  // namespace sgb
-
-namespace sgb {
+// ------------------------------------------------------------------ stage tracing
 // Built-in stage tracing (the reference has none; its only timing hook is train.py's per-iteration
 // event pair).  When enabled, every stage is bracketed by a CUDA event pair recorded on the
 // caller's stream; sgb_profile_read() sums the pairs recorded since the last read.
@@ -153,24 +150,11 @@ struct Profiler {
     int n[ST_COUNT];
     bool created = false;
 };
-}  // namespace sgb
 
-namespace sgb {
 constexpr int kNumSMs = 132;  // H100 SXM: sizes the grids of the grid-stride kernels
 
-// One weight pool (blend_v3.cu) = the per-tile alpha*T rows of ONE view.  A ctx keeps SGB_MAX_BATCH of them so
-// that the backward of each view of a batch (or of a forward-forward-...-backward-backward sequence) finds the
-// rows its forward built.  A slot is identified by the view's binning-state pointer: a new forward through the
-// same pointer necessarily overwrites that slot, so a slot can never describe a different view's instance list.
-struct PoolSlot {
-    Scratch mem;
-    bool valid = false;
-    const void* key_bin = nullptr;
-    int64_t key_R = 0;
-    int key_W = 0, key_H = 0, key_P = 0;
-    uint32_t chunks = 0;   // capacity the slot was carved with
-    uint64_t stamp = 0;    // LRU clock
-};
+struct WeightPools;  // weight_pool.cuh
+struct Readback;
 }  // namespace sgb
 
 struct sgb_ctx {
@@ -181,19 +165,14 @@ struct sgb_ctx {
     sgb::Scratch geom;     // depth-sort keys, iota values, CUB temp, 64-bit instance total (shared by a batch's views)
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
-    sgb::Scratch work;     // work-item counters of the persistent kernels (blend_v3.cu)
+    sgb::Scratch work;     // work-item counters of the persistent kernels (chn_dfeature.cu)
     sgb::Scratch depth_grad;  // [P] dL/d(view-space z) of the view being differentiated (expected-depth backward)
     sgb::Scratch lift_state;  // sgb_lift_batch: geometry state, radii and image state of every view of the call
     sgb::Scratch lift_bin;    // sgb_lift_batch: binning states of the views
-    // Per-tile weight rows of the C-channel blend (blend_v3.cu).  As many slots as views per batch: the backward
-    // resolves the rows of all V views before its first kernel, and V <= slots guarantees that rebuilding one view
-    // cannot evict another view of the same batch.
-    sgb::PoolSlot pools[SGB_MAX_BATCH];
-    uint64_t pool_clock = 0;
-    uint64_t pool_chunks_hint = 0;  // high-water mark of the pool demand (chunks)
-    int64_t* pinned = nullptr;  // host-pinned readback slots (1 KB)
-    int64_t stat_blended_pairs = 0;  // last alpha pass: blended (pixel, Gaussian) pairs
-    int64_t stat_pool_chunks = 0;    // last alpha pass: 16-entry weight-row chunks in use
+    // What the ctx carries from one call to the next: the weight rows of the C-channel blend, one pool per view of a
+    // batch.  Owned; its layout is the weight-pool module's (weight_pool.cuh).
+    sgb::WeightPools* pools = nullptr;
+    sgb::Readback* pinned = nullptr;  // host-pinned readback buffer (weight_pool.cuh)
     cudaEvent_t feature_grad_event = nullptr;  // caller-owned; recorded when dL_dcolors is final (sgb200.h)
 };
 
@@ -227,22 +206,6 @@ struct DeviceOnce {
     }
 };
 
-using TensorMapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no libcuda link); nullptr when unavailable.
-inline TensorMapEncodeFn tensor_map_encoder() {
-    static const TensorMapEncodeFn encode = [] {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            fn = nullptr;
-        return (TensorMapEncodeFn)fn;
-    }();
-    return encode;
-}
-
 // ------------------------------------------------------------------ stage launchers
 int launch_preprocess(const sgb_view_inputs& in, GeomView g, int32_t* radii, uint32_t* depth_keys,
                       cudaStream_t s);
@@ -263,74 +226,12 @@ int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgV
                           const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,
                           float* dL_dcolors, const float* dL_dexp_depth, const float* dL_dalpha, float* dL_ddepth,
                           cudaStream_t s);
-struct PoolView;
-// C > 4 blend.  The weight pool of a view (blend_pool.cuh) is built by its alpha pass; blend_v3.cu owns the slots:
-//   weight_pool_build         enqueue the alpha pass of one view into its slot (no sync), so that a batch enqueues
-//                             the alpha passes of all its views before the one sync that checks their pools
-//   weight_pool_settle        one stream sync, then the pool check of views [0, V) (of those with only[v], when
-//                             given); a view whose pool overflowed is grown and built again; fills pv[v]
-//   weight_rows_for_backward  pv[v] of every view with R > 0: the slot its forward filled, else rebuilt (all misses
-//                             under one sync)
-// The blend kernels take the PoolView and look up nothing.  A batched backward runs all dL/dfeature kernels first,
-// records the feature-gradient event, then the chain kernels.
-int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s);
-int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s,
-                       const bool* only = nullptr);
-int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s);
-void weight_pool_release(sgb_ctx* ctx, int V, const ViewState* vw);
-int blend_forward_v3(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s);
-// dL_dcolors[g][c] += sum_px w * dL_dpix[c][px]; T = float for a backward, float or __half for a lift's feature map
-template <typename T>
-int blend_backward_v3_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const T* dL_dpix,
-                               float* dL_dcolors, cudaStream_t s);
-// weight_sum[g] += sum_px w over every entry of the view's pool (the denominator of a lift)
-int pool_weight_sums(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* weight_sum, cudaStream_t s);
-int blend_backward_v3_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float* dL_dpix,
-                            float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, cudaStream_t s);
+// C > 4 blend: weight_pool.cuh (the alpha pass and the pools it fills) and chn_blend.cuh (the contraction stages).
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,
                          const float* dL_dcolor_rgb, const sgb_view_grads& gr, const float* dL_ddepth, cudaStream_t s);
 
 // ------------------------------------------------------------------ device helpers
 #ifdef __CUDACC__
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Waits for the phase with the given parity.  try_wait sleeps in hardware between polls; a bounded
-// spin turns a protocol bug into a trap (launch failure) instead of a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0;
-    for (uint32_t spins = 0; !done; spins++) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if (spins > (1u << 24)) __trap();
-    }
-}
-// 1-D bulk copy global -> shared through the TMA engine (SASS: UBLKCP); dst/src 16-B aligned,
-// bytes a multiple of 16; completion is signalled on `bar` as transaction bytes.
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst_smem)),
-                 "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
 // d.xy = a.xy * b.xy + c.xy as two round-to-nearest FMAs (sm_90 has no packed fp32 FMA).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
     return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));

@@ -23,6 +23,7 @@
 
 #include "common.cuh"
 #include "feature_loss.cuh"
+#include "tma.cuh"
 
 namespace sgb {
 namespace {
@@ -34,16 +35,6 @@ constexpr size_t kFlStageTarget = 48 * 1024;  // staged bytes per CTA aimed at: 
 
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-
-// 2-D tensor tile global -> shared (SASS: UTMALDG): box corner (x, y) in elements, out-of-range elements arrive as
-// zeros; completion is signalled on `bar` as the box's bytes.
-__device__ __forceinline__ void tma_tile2d_g2s(void* dst_smem, const CUtensorMap* map, int x, int y, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-            smem_u32(dst_smem)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
-        : "memory");
-}
 
 // loss[1] = number of pixels whose target column has a non-zero element (features_gt.norm(dim=-1) > 0).  Thread =
 // one pixel.  Channel 0 decides almost every pixel of a real feature map; the rest of a column is read in groups of
@@ -243,17 +234,12 @@ __global__ void __launch_bounds__(256) feature_elementwise_kernel(long long M, l
 // missing; the kernel then stages with plain loads.
 bool encode_plane_map(CUtensorMap* map, const void* base, CUtensorMapDataType type, size_t es, int C, long long N,
                       int PB, int box_c) {
-    const TensorMapEncodeFn encode = tensor_map_encoder();
     memset(map, 0, sizeof(*map));
-    if (!encode || ((size_t)N * es) % 16 != 0 || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || N > 0x7fffffffll)
-        return false;
+    if (((size_t)N * es) % 16 != 0 || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || N > 0x7fffffffll) return false;
     const cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)C};
     const cuuint64_t strides[1] = {(cuuint64_t)N * es};
     const cuuint32_t box[2] = {(cuuint32_t)PB, (cuuint32_t)box_c};
-    const cuuint32_t estr[2] = {1, 1};
-    return encode(map, type, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return encode_tiled_map(map, type, 2, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 template <typename T>

@@ -11,6 +11,7 @@
 // the channel planes with 16-byte loads and keeps K running dot products plus the squared norm in
 // registers; the class embeddings sit transposed in shared memory and are read as broadcasts.
 #include "common.cuh"
+#include "tma.cuh"
 
 namespace sgb {
 

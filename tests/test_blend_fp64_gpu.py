@@ -2,7 +2,7 @@
 count, image shape, list length and pointer layout the kernels branch on.  The restatement runs on the kernel's own
 per-Gaussian state and tile lists (sgb_state_field), so the only error measured is the kernel's arithmetic.
 
-Which case reaches which branch (C <= 4: blend_fwd.cu / blend_bwd.cu; C > 4: blend_v3.cu):
+Which case reaches which branch (C <= 4: blend_fwd.cu / blend_bwd.cu; C > 4: weight_pool.cu + chn_*.cu):
   C = 1, 2, 4 ................ the C <= 4 feature path with colors_precomp
   C = 5 .. 768 ............... 16-channel slabs of the chain kernel and 64-channel items of the dL/dfeature kernel,
                                on both sides of every multiple of 16 and 64 (plain loads when C % 4 != 0)
@@ -14,7 +14,7 @@ Which case reaches which branch (C <= 4: blend_fwd.cu / blend_bwd.cu; C > 4: ble
                                remainder R = 1..8 of the 128-entry dL/dfeature passes, weight pool overflow and
                                retry on a fresh ctx
   dl_offset4 ................. dL/dout 4 bytes off 16-byte alignment with W % 4 == 0: non-TMA dL paths
-  feat_offset4 ............... feature rows not 16-byte aligned with C % 4 == 0: blend_forward_v3_kernel and
+  feat_offset4 ............... feature rows not 16-byte aligned with C % 4 == 0: blend_forward_ldg_kernel and
                                chain_backward_warp_kernel<false>
   dcolors_offset4 ............ dL_dcolors not 16-byte aligned: red16 off
   zero_bg .................... the bg_nonzero == 0 branch of the chain kernel (C = 17, 64, 257)

@@ -31,7 +31,7 @@ from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
 from semantic_gaussians_b200.renderer import render_chn  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene, room_cameras  # noqa: E402
 
-WCHUNK_BYTES = 16 + 16 * 8 + 16 * 256 * 4   # one 16-entry weight-pool chunk (csrc/blend_pool.cuh)
+WCHUNK_BYTES = 16 + 16 * 8 + 16 * 256 * 4   # one 16-entry weight-pool chunk (csrc/weight_pool.cuh)
 
 
 class Pipe:
