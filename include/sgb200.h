@@ -503,6 +503,67 @@ typedef struct sgb_adam_tensor {
 } sgb_adam_tensor;
 int sgb_adam_step(const sgb_adam_tensor* tensors_host, int32_t n, void* stream);
 
+/* ---- sparse 3D convolution: the coordinate maps, kernel maps and products of MinkowskiEngine's
+ * MinkowskiConvolution / MinkowskiConvolutionTranspose as MinkUNet uses them (sparse.py, mink_unet.py).
+ *
+ * Coordinates are (N,4) int32 rows (b, x, y, z), 16-byte aligned, 1 <= N <= 2^31 - 1.  A coordinate map at tensor
+ * stride t holds rows whose x, y, z are multiples of t.  Its hash table (sgb_coord_map_bytes(N) bytes of device
+ * memory) is keyed on all four values: two different rows never share an entry.
+ *
+ * sgb_coord_map_build: builds the table of `coords`.  status (device, 2 int64, zeroed by the call) receives [0] the
+ * number of rows equal to an earlier-inserted row and [1] the number of rows with a negative x, y or z.  The map is
+ * only valid when both are 0.
+ *
+ * sgb_coord_stride: the map at stride 2t from the map at stride t (`stride` = t): rows (b, floor(x / 2t) * 2t, ...),
+ * unique, in the order in which their first child row appears in `coords`.  out_coords has room for N rows;
+ * out_count (device, 1 int64) receives the row count.  workspace: sgb_coord_stride_workspace_bytes(N) bytes.
+ *
+ * sgb_kernel_map_count / sgb_kernel_map_fill: the (input row, output row) pairs of kernel size k in {2, 3, 5} over an
+ * input map at stride t (`stride`).  Offset index d = jx + k jy + k^2 jz, offset per axis lb + j t with
+ * lb = -((k - 1) / 2) t (C division): {-t, 0, t} for k = 3, {0, t} for k = 2.  Output row o pairs with input row i
+ * at d when coord(i) = coord(o) + offset and the b values are equal.  count writes offsets (device, k^3 + 1 int64):
+ * offset d's pairs are pairs[offsets[d] .. offsets[d+1]).  The caller reads offsets[k^3] to size `pairs` (int32
+ * (in, out) pairs, 8 bytes each) and then calls fill with the same arguments and the workspace
+ * (sgb_kernel_map_workspace_bytes(N_out, k) bytes) the count call left.  Within an offset the pairs ascend in the
+ * output row.  A transposed layer uses the pairs of the matching stride-2 layer with the roles swapped.
+ *
+ * Products (kernel (K, C_in, C_out) fp32 row-major, 1 <= K <= SGB_SPARSE_MAX_K, C_in, C_out >= 1; offsets_host is
+ * the host copy of the kernel map's offsets, pairs may be NULL when offsets_host[K] == 0).  transposed = 0:
+ *     forward   out[o] = sum_d x[i] W_d                 over offset d's pairs (i, o)
+ *     input     dx[i]  = sum_d dy[o] W_d^T
+ *     weight    dW_d   = sum over d's pairs of x[i]^T dy[o]
+ * transposed = 1 swaps the roles of i and o (x and dx then live on the pairs' output-row side).  n_in / C_in describe
+ * x and dx, n_out / C_out describe out and dy.  out, dx and dkernel are overwritten.  The weight gradient needs
+ * sgb_sparse_conv_backward_weight_workspace_bytes(...) bytes of 16-byte aligned workspace.  No float atomics: the
+ * same inputs give bitwise identical outputs.
+ *
+ * Every call validates its arguments (SGB_E_INVALID) before anything is enqueued, is asynchronous on `stream` and
+ * never synchronises; the workspace-size calls return 0 for arguments the calls would reject. */
+#define SGB_SPARSE_MAX_K 125
+size_t sgb_coord_map_bytes(int64_t N);
+int sgb_coord_map_build(int64_t N, const int32_t* coords, void* table, int64_t* status /* [2] */, void* stream);
+size_t sgb_coord_stride_workspace_bytes(int64_t N);
+int sgb_coord_stride(int64_t N, const int32_t* coords, int32_t stride, void* workspace, int32_t* out_coords,
+                     int64_t* out_count /* [1] */, void* stream);
+size_t sgb_kernel_map_workspace_bytes(int64_t N_out, int32_t k);
+int sgb_kernel_map_count(int64_t N_in, const int32_t* in_coords, const void* in_table, int64_t N_out,
+                         const int32_t* out_coords, int32_t k, int32_t stride, void* workspace,
+                         int64_t* offsets /* [k^3 + 1] */, void* stream);
+int sgb_kernel_map_fill(int64_t N_in, const int32_t* in_coords, const void* in_table, int64_t N_out,
+                        const int32_t* out_coords, int32_t k, int32_t stride, const void* workspace,
+                        int32_t* pairs /* (offsets[k^3], 2) */, void* stream);
+int sgb_sparse_conv_forward(int32_t K, const int64_t* offsets_host, const int32_t* pairs, int32_t transposed,
+                            int64_t n_in, int32_t C_in, const float* x, const float* kernel, int64_t n_out,
+                            int32_t C_out, float* out, void* stream);
+int sgb_sparse_conv_backward_input(int32_t K, const int64_t* offsets_host, const int32_t* pairs, int32_t transposed,
+                                   int64_t n_in, int32_t C_in, float* dx, const float* kernel, int64_t n_out,
+                                   int32_t C_out, const float* dy, void* stream);
+size_t sgb_sparse_conv_backward_weight_workspace_bytes(int32_t K, const int64_t* offsets_host, int32_t C_in,
+                                                       int32_t C_out);
+int sgb_sparse_conv_backward_weight(int32_t K, const int64_t* offsets_host, const int32_t* pairs, int32_t transposed,
+                                    int64_t n_in, int32_t C_in, const float* x, int64_t n_out, int32_t C_out,
+                                    const float* dy, void* workspace, float* dkernel, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -80,7 +80,10 @@ EXPORTS = (
     "sgb_photometric_forward", "sgb_photometric_backward", "sgb_confusion_accumulate", "sgb_feature_map_loss",
     "sgb_forward_render_batch_ext", "sgb_backward_batch_ext", "sgb_decoded_feature_loss",
     "sgb_decoded_feature_loss_workspace_bytes", "sgb_voxelize", "sgb_voxelize_workspace_bytes", "sgb_lift_batch",
-    "sgb_adam_step",
+    "sgb_adam_step", "sgb_coord_map_bytes", "sgb_coord_map_build", "sgb_coord_stride_workspace_bytes",
+    "sgb_coord_stride", "sgb_kernel_map_workspace_bytes", "sgb_kernel_map_count", "sgb_kernel_map_fill",
+    "sgb_sparse_conv_forward", "sgb_sparse_conv_backward_input", "sgb_sparse_conv_backward_weight_workspace_bytes",
+    "sgb_sparse_conv_backward_weight",
 )
 
 _lib = None
@@ -162,6 +165,21 @@ def load() -> C.CDLL:
         lib.sgb_voxelize_workspace_bytes.argtypes = [i64]
         lib.sgb_voxelize_workspace_bytes.restype = C.c_size_t
         lib.sgb_adam_step.argtypes = [C.POINTER(AdamTensor), i32, vp]
+        pi64 = C.POINTER(i64)
+        for name in ("sgb_coord_map_bytes", "sgb_coord_stride_workspace_bytes"):
+            getattr(lib, name).argtypes = [i64]
+            getattr(lib, name).restype = C.c_size_t
+        lib.sgb_coord_map_build.argtypes = [i64, vp, vp, vp, vp]
+        lib.sgb_coord_stride.argtypes = [i64, vp, i32, vp, vp, vp, vp]
+        lib.sgb_kernel_map_workspace_bytes.argtypes = [i64, i32]
+        lib.sgb_kernel_map_workspace_bytes.restype = C.c_size_t
+        lib.sgb_kernel_map_count.argtypes = [i64, vp, vp, i64, vp, i32, i32, vp, vp, vp]
+        lib.sgb_kernel_map_fill.argtypes = [i64, vp, vp, i64, vp, i32, i32, vp, vp, vp]
+        lib.sgb_sparse_conv_forward.argtypes = [i32, pi64, vp, i32, i64, i32, vp, vp, i64, i32, vp, vp]
+        lib.sgb_sparse_conv_backward_input.argtypes = [i32, pi64, vp, i32, i64, i32, vp, vp, i64, i32, vp, vp]
+        lib.sgb_sparse_conv_backward_weight_workspace_bytes.argtypes = [i32, pi64, i32, i32]
+        lib.sgb_sparse_conv_backward_weight_workspace_bytes.restype = C.c_size_t
+        lib.sgb_sparse_conv_backward_weight.argtypes = [i32, pi64, vp, i32, i64, i32, vp, i64, i32, vp, vp, vp, vp]
         _lib = lib
         return lib
 

@@ -1,0 +1,223 @@
+"""Sparse 3D convolution and MinkUNet on the GPU against the float64 restatement (tests/sparse_ref.py): coordinate and
+kernel maps bit for bit, the products within 1e-5 of sum |x||w|, MinkUNet on a voxelized `room` scene, call-to-call
+reproducibility and a short distillation loop."""
+import numpy as np
+import pytest
+import torch
+
+import sparse_ref as ref
+from semantic_gaussians_b200 import sparse as sp
+from semantic_gaussians_b200.gaussian_model import GaussianModel
+from semantic_gaussians_b200.mink_unet import mink_unet
+from semantic_gaussians_b200.scene_synth import make_scene
+from semantic_gaussians_b200.voxelize import distill_targets, voxelize_gaussians
+
+pytestmark = pytest.mark.gpu
+DEV = torch.device("cuda:0")
+
+
+def _rows(kind, N, batches, seed=0):
+    rng = np.random.default_rng(seed)
+    if kind == "box":
+        side = max(4, int(round((N / batches / 0.3) ** (1 / 3))))        # ~30 % occupancy
+        pts = rng.integers(0, side, (3 * N, 3))
+    elif kind == "near_2_30":
+        pts = (1 << 30) - 1024 + rng.integers(0, 64, (3 * N, 3)) * 32 + rng.integers(0, 3, (3 * N, 3))
+    else:   # low_bits: rows that differ only above bit 20
+        pts = (rng.integers(0, 64, (3 * N, 3)) << 20) + rng.integers(0, 2, (3 * N, 3))
+    b = rng.integers(0, batches, (3 * N, 1))
+    rows = np.unique(np.concatenate([b, pts], 1), axis=0)
+    rows = rows[rng.permutation(len(rows))[:N]]
+    assert len(rows) == N
+    return rows.astype(np.int32)
+
+
+def _pairs(km):
+    return [[tuple(p) for p in km.pairs[a:b].tolist()]
+            for a, b in zip(km.offsets_host[:km.K], km.offsets_host[1:km.K + 1])]
+
+
+@pytest.mark.parametrize("kind,N,batches", [("box", 1, 1), ("box", 127, 2), ("box", 128, 3), ("box", 129, 4),
+                                            ("box", 50_000, 2), ("near_2_30", 5_000, 3), ("low_bits", 5_000, 1)])
+def test_coordinate_and_kernel_maps_equal_the_restatement(kind, N, batches):
+    rows = _rows(kind, N, batches, seed=N)
+    mgr = sp.CoordinateManager(torch.from_numpy(rows).to(DEV))
+    maps = ref.Maps(rows.tolist())
+    for t in (1, 2, 4, 8, 16):
+        assert [tuple(r) for r in mgr.map(t).coords.tolist()] == maps.at(t), t
+    for t in (1, 2, 4, 8, 16):
+        for k in ((3, 5) if t == 1 else (3,)):
+            assert _pairs(mgr.kernel_map(t, t, k)) == maps.kmap(t, t, k), (t, k)
+        if t < 16:
+            assert _pairs(mgr.kernel_map(t, 2 * t, 2)) == maps.kmap(t, 2 * t, 2), (t, 2)
+
+
+def test_duplicate_and_negative_coordinates_raise():
+    rows = torch.tensor([[1, 0, 0, 0], [1, 5, 6, 7], [1, 0, 0, 0]], dtype=torch.int32, device=DEV)
+    with pytest.raises(ValueError, match="1 coordinate rows repeat"):
+        sp.SparseTensor(torch.zeros(3, 2, device=DEV), rows)
+    rows = torch.tensor([[1, 0, 0, 0], [1, 5, -6, 7]], dtype=torch.int32, device=DEV)
+    with pytest.raises(ValueError, match="negative"):
+        sp.SparseTensor(torch.zeros(2, 2, device=DEV), rows)
+    # rows equal in x, y, z but not in b are distinct
+    rows = torch.tensor([[0, 1, 2, 3], [1, 1, 2, 3]], dtype=torch.int32, device=DEV)
+    assert sp.SparseTensor(torch.zeros(2, 2, device=DEV), rows).C.shape == (2, 4)
+
+
+# ---------------------------------------------------------------- products
+
+_CONV_ROWS = _rows("box", 1500, 2, seed=7)
+
+
+def _layer_case(k, stride, transposed, rows=_CONV_ROWS, t=1):
+    """(kernel map, restatement pairs per offset, rows of x, rows of the output) of one layer at stride t."""
+    mgr = sp.CoordinateManager(torch.from_numpy(rows).to(DEV))
+    maps = ref.Maps(rows.tolist())
+    if transposed:
+        km, rk = mgr.kernel_map(t, 2 * t, 2), maps.kmap(t, 2 * t, 2)
+        return km, rk, mgr.map(2 * t).n, mgr.map(t).n
+    to = t * stride
+    return mgr.kernel_map(t, to, k), maps.kmap(t, to, k), mgr.map(t).n, mgr.map(to).n
+
+
+def _bound_ok(got, want, bound, what):
+    err = (got.double().cpu() - want).abs()
+    ok = err <= 1e-5 * bound + 1e-30
+    assert bool(ok.all()), f"{what}: worst err {err.max().item():.3g}, worst ratio {(err / bound.clamp_min(1e-30)).max().item():.3g}"
+
+
+@pytest.mark.parametrize("cin", [1, 3, 32, 56, 96, 384])
+@pytest.mark.parametrize("cout", [1, 32, 64, 256])
+@pytest.mark.parametrize("k,stride,transposed", [(3, 1, False), (5, 1, False), (2, 2, False), (2, 2, True)])
+def test_products_match_float64(cin, cout, k, stride, transposed):
+    km, rk, n_in, n_out = _layer_case(k, stride, transposed)
+    g = torch.Generator().manual_seed(cin * 1000 + cout)
+    x = torch.randn(n_in, cin, generator=g, dtype=torch.float64)
+    W = torch.randn(km.K, cin, cout, generator=g, dtype=torch.float64) / cin ** 0.5
+    dy = torch.randn(n_out, cout, generator=g, dtype=torch.float64)
+    xg = x.float().to(DEV).requires_grad_(True)
+    Wg = W.float().to(DEV).requires_grad_(True)
+    out = sp._SparseConvFunction.apply(xg, Wg, km, transposed, n_out)
+    out.backward(dy.float().to(DEV))
+    x32, W32, dy32 = xg.detach().double().cpu(), Wg.detach().double().cpu(), dy.float().double()
+    want = ref.conv(x32, W32, rk, n_out, transposed)
+    _bound_ok(out.detach(), want, ref.conv(x32.abs(), W32.abs(), rk, n_out, transposed), "forward")
+    # dx = conv of dy with W^T over the swapped roles
+    Wt = W32.transpose(1, 2)
+    want_dx = ref.conv(dy32, Wt, rk, n_in, not transposed)
+    _bound_ok(xg.grad, want_dx, ref.conv(dy32.abs(), Wt.abs(), rk, n_in, not transposed), "dx")
+    dW = torch.zeros_like(W32)
+    bW = torch.zeros_like(W32)
+    for d, pairs in enumerate(rk):
+        if pairs:
+            p = torch.tensor(pairs)
+            xs, ys = (p[:, 1], p[:, 0]) if transposed else (p[:, 0], p[:, 1])
+            dW[d] = x32[xs].T @ dy32[ys]
+            bW[d] = x32[xs].abs().T @ dy32[ys].abs()
+    _bound_ok(Wg.grad, dW, bW, "dW")
+
+
+def test_layer_with_empty_offsets_and_skipped_input_gradient():
+    rows = np.array([[0, 0, 0, 0], [0, 10, 0, 0], [0, 11, 0, 0], [1, 0, 0, 0]], np.int32)  # 2 of 27 offsets filled
+    km, rk, n_in, n_out = _layer_case(3, 1, False, rows)
+    assert sum(1 for c in km.counts if c) == 3 and km.counts[13] == 4
+    x = torch.randn(n_in, 5, device=DEV)
+    W = torch.randn(27, 5, 7, device=DEV, requires_grad=True)
+    out = sp._SparseConvFunction.apply(x, W, km, False, n_out)
+    out.sum().backward()
+    want = ref.conv(x.double().cpu(), W.detach().double().cpu(), rk, n_out)
+    assert torch.allclose(out.detach().double().cpu(), want, rtol=1e-5, atol=1e-5)
+    empty = [d for d in range(27) if not km.counts[d]]
+    assert (W.grad[empty] == 0).all() and W.grad[13].abs().sum() > 0
+
+
+# ---------------------------------------------------------------- MinkUNet
+
+def _room_input(P=20_000):
+    scene = make_scene(P, 0, kind="room", sh=True)
+    m = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, shs=scene.shs, device=DEV)
+    locs, feats, vox_ind = voxelize_gaussians(m, 0.02, "all")
+    return locs, feats, vox_ind
+
+
+def _float64_params(model):
+    return {n: p.detach().double().cpu().requires_grad_(True) for n, p in model.named_parameters()}
+
+
+@pytest.mark.parametrize("arch", ["MinkUNet14A", "MinkUNet34A"])
+def test_minkunet_matches_float64(arch):
+    torch.manual_seed(0)
+    locs, feats, _ = _room_input()
+    assert 15_000 < locs.shape[0] <= 20_000
+    model = mink_unet(56, 768, arch=arch).to(DEV)
+    params = _float64_params(model)
+    out = model(sp.SparseTensor(feats, locs))
+    assert out.F.shape == (locs.shape[0], 768) and out.tensor_stride == [1, 1, 1] and torch.equal(out.C, locs)
+    g = torch.Generator().manual_seed(1)
+    dy = torch.randn(out.F.shape, generator=g)
+    out.F.backward(dy.to(DEV))
+    want = ref.minkunet_forward(model, locs.cpu(), feats.double().cpu(), params, training=True)
+    want.backward(dy.double())
+    err = (out.F.detach().double().cpu() - want.detach()).abs().max()
+    assert err <= 1e-3 * want.abs().max(), f"train forward: {err} vs max {want.abs().max()}"
+    # The bound is 1e-3 in the L2 norm, or three times the error of the same restatement computed in fp32 where that
+    # is larger.  With BatchNorm after every convolution, some gradients (BN biases, the first kernel) are sums whose
+    # terms nearly cancel, and fp32 arithmetic through the network misses 1e-3 there by itself.  On an H100, 34A:
+    # block7.0.norm1.bn.bias 2.8e-3 here vs 1.3e-3 for the fp32 restatement, conv0p1s1.kernel 1.7e-3 vs 1.5e-3.
+    params32 = {n: p.detach().float().cpu().requires_grad_(True) for n, p in params.items()}
+    ref.minkunet_forward(model, locs.cpu(), feats.cpu(), params32, training=True).backward(dy)
+    bad = []
+    for n, p in model.named_parameters():
+        ref_g = params[n].grad
+        rel = ((p.grad.double().cpu() - ref_g).norm() / ref_g.norm().clamp_min(1e-30)).item()
+        rel32 = ((params32[n].grad.double() - ref_g).norm() / ref_g.norm().clamp_min(1e-30)).item()
+        if rel > max(1e-3, 3 * rel32):
+            bad.append(f"{n}: {rel:.3g} (fp32 restatement {rel32:.3g})")
+    assert not bad, "relative L2 error of the gradient: " + "; ".join(bad)
+    model.eval()
+    with torch.no_grad():
+        out = model(sp.SparseTensor(feats, locs))
+        want = ref.minkunet_forward(model, locs.cpu(), feats.double().cpu(), _float64_params(model), training=False)
+    err = (out.F.double().cpu() - want).abs().max()
+    assert err <= 1e-3 * want.abs().max(), f"eval forward: {err} vs max {want.abs().max()}"
+
+
+def test_two_passes_are_bitwise_equal():
+    torch.manual_seed(0)
+    locs, feats, _ = _room_input(8_000)
+    model = mink_unet(56, 96, arch="MinkUNet34A").to(DEV)
+    dy = torch.randn(locs.shape[0], 96, device=DEV)
+    results = []
+    for _ in range(2):
+        model.zero_grad()
+        out = model(sp.SparseTensor(feats, locs))
+        out.F.backward(dy)
+        results.append((out.F.detach().clone(), [p.grad.clone() for p in model.parameters()]))
+    assert torch.equal(results[0][0], results[1][0])
+    for a, b in zip(results[0][1], results[1][1]):
+        assert torch.equal(a, b)
+
+
+def test_distill_loop_lowers_the_loss():
+    """distill.py's step: SparseTensor, the model, the cosine loss over the masked rows, Adam."""
+    torch.manual_seed(0)
+    locs, feats, vox_ind = _room_input(8_000)
+    P = int(vox_ind.max().item()) + 1
+    mask_full = (torch.rand(P, device=DEV) < 0.6)
+    gen = torch.Generator(device=DEV).manual_seed(2)
+    feat = torch.nn.functional.normalize(torch.randn(int(mask_full.sum()), 64, device=DEV, generator=gen), dim=-1)
+    mask, features_gt = distill_targets(vox_ind, mask_full, feat)
+    model = mink_unet(56, 64, arch="MinkUNet14A").to(DEV)
+    opt = torch.optim.Adam(model.parameters(), lr=1e-3)
+    losses = []
+    for _ in range(5):
+        locs_aug = locs.clone()
+        locs_aug[:, 1:4] += (torch.rand(3) * 100).int().to(DEV)
+        output = model(sp.SparseTensor(feats, locs_aug)).F[mask]
+        norm_mask = features_gt.norm(dim=-1) > 0
+        loss = (1 - torch.nn.CosineSimilarity()(output[norm_mask], features_gt[norm_mask])).mean()
+        opt.zero_grad()
+        loss.backward()
+        opt.step()
+        losses.append(loss.item())
+    assert losses[-1] < losses[0], losses
