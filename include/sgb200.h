@@ -373,6 +373,22 @@ int sgb_decoded_feature_loss(int32_t C, int32_t c, int64_t N, const float* rende
                              int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type,
                              float* dL_drender, float* dL_dweight, float* dL_dbias /* NULL iff bias NULL */,
                              void* workspace, double* loss /* [2] device: loss, pixels averaged over */, void* stream);
+/* The same three losses on the masked rows of a 3D network's (M, F) row-major fp32 output (MinkUNet's .F), as
+ * distill.py:111-124 takes them: x_k = output[i_k, head*C : head*C + C] for the k-th row i_k with mask[i_k] != 0, and
+ * target (K, C) row-major (one row per masked output row, in row order; SGB_FEAT_F16 or SGB_FEAT_F32, converted to
+ * fp32).  cosine averages over the Nv target rows with a non-zero element, l1 / l2 over K * C.  grad (M, F) fp32 is
+ * overwritten: d loss / d output on the head's columns of masked rows, 0 everywhere else.  loss (device, 2 doubles)
+ * receives the loss and the count averaged over (Nv for cosine, K for l1 / l2); both are 0 when nothing is averaged
+ * over, and both are NaN when the mask selects other than K rows.  workspace: device scratch of
+ * sgb_voxel_feature_loss_workspace_bytes(M) bytes, 16-byte aligned.  Every output is bitwise identical from call to
+ * call (no float atomics).  0 <= M <= 2^31 - 1, 0 <= K <= M, 1 <= C <= 1024, head >= 0, head*C + C <= F; a bad
+ * argument returns SGB_E_INVALID before anything is enqueued.  Asynchronous on `stream`, no host copy, no ctx.  The
+ * workspace-size call returns 0 for M outside those limits. */
+size_t sgb_voxel_feature_loss_workspace_bytes(int64_t M);
+int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint8_t* mask /* (M) bool */, int64_t K,
+                           int32_t C, int32_t head, const void* target,
+                           int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type, float* grad,
+                           void* workspace, double* loss /* [2] device: loss, count */, void* stream);
 int sgb_semantic_head(sgb_ctx* ctx, int32_t C, int32_t K, int64_t N, const float* render, const float* text,
                       int32_t first_class, float* sim, int64_t* label, void* stream);
 int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const float* features, const float* text,
@@ -428,6 +444,21 @@ size_t sgb_voxelize_workspace_bytes(int64_t P);
 int sgb_voxelize(int64_t P, const float* xyz, const double* transform /* [12] host */, void* workspace,
                  int64_t* first_index /* (P) */, int64_t* inverse /* (P) */, int32_t* coords /* (P,3) */,
                  int64_t* counts /* [3] */, void* stream);
+/* The same for a float64 cloud (e.g. after sgb_elastic_displace); the fp32 call's results are those of this one on the
+ * fp32 cloud promoted to fp64. */
+int sgb_voxelize_f64(int64_t P, const double* xyz, const double* transform /* [12] host */, void* workspace,
+                     int64_t* first_index /* (P) */, int64_t* inverse /* (P) */, int32_t* coords /* (P,3) */,
+                     int64_t* counts /* [3] */, void* stream);
+
+/* ---- elastic distortion: the per-point half of dataset/augmentation.py ElasticDistortion.elastic_distortion,
+ *     out = xyz + RegularGridInterpolator(axes, grid, bounds_error=0, fill_value=0)(xyz) * magnitude
+ * bitwise as scipy 1.18 evaluates it (trilinear, fp64, every product and sum rounded alone, corners in
+ * itertools.product order, 0 outside the grid, NaN for a point with a NaN coordinate).  xyz (P,3) device, fp32 or fp64
+ * (xyz_is_f64); grid (nx,ny,nz,3) fp32 device (the smoothed noise); axes device fp64, nx then ny then nz strictly
+ * ascending nodes; out (P,3) fp64 device, which may be xyz itself when xyz is fp64.  1 <= P <= 2^31 - 1, every
+ * n >= 2; a bad argument returns SGB_E_INVALID before anything is enqueued.  Asynchronous on `stream`, no host copy. */
+int sgb_elastic_displace(int64_t P, const void* xyz, int32_t xyz_is_f64, const float* grid, int32_t nx, int32_t ny,
+                         int32_t nz, const double* axes, double magnitude, double* out, void* stream);
 
 /* ---- 3-nearest-neighbour mean squared distance: `distCUDA2` of the reference's
  * simple-knn extension (submodules/simple-knn/simple_knn.cu:185-220, spatial.cu), used by

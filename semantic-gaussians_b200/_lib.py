@@ -83,7 +83,8 @@ EXPORTS = (
     "sgb_adam_step", "sgb_coord_map_bytes", "sgb_coord_map_build", "sgb_coord_stride_workspace_bytes",
     "sgb_coord_stride", "sgb_kernel_map_workspace_bytes", "sgb_kernel_map_count", "sgb_kernel_map_fill",
     "sgb_sparse_conv_forward", "sgb_sparse_conv_backward_input", "sgb_sparse_conv_backward_weight_workspace_bytes",
-    "sgb_sparse_conv_backward_weight",
+    "sgb_sparse_conv_backward_weight", "sgb_voxelize_f64", "sgb_elastic_displace", "sgb_voxel_feature_loss",
+    "sgb_voxel_feature_loss_workspace_bytes",
 )
 
 _lib = None
@@ -162,7 +163,12 @@ def load() -> C.CDLL:
         lib.sgb_decoded_feature_loss_workspace_bytes.argtypes = [i32, i32, i64]
         lib.sgb_decoded_feature_loss_workspace_bytes.restype = C.c_size_t
         lib.sgb_voxelize.argtypes = [i64, vp, C.POINTER(C.c_double), vp, vp, vp, vp, vp, vp]
+        lib.sgb_voxelize_f64.argtypes = [i64, vp, C.POINTER(C.c_double), vp, vp, vp, vp, vp, vp]
         lib.sgb_voxelize_workspace_bytes.argtypes = [i64]
+        lib.sgb_elastic_displace.argtypes = [i64, vp, i32, vp, i32, i32, i32, vp, C.c_double, vp, vp]
+        lib.sgb_voxel_feature_loss_workspace_bytes.argtypes = [i64]
+        lib.sgb_voxel_feature_loss_workspace_bytes.restype = C.c_size_t
+        lib.sgb_voxel_feature_loss.argtypes = [i64, i32, vp, vp, i64, i32, i32, vp, i32, i32, vp, vp, vp, vp]
         lib.sgb_voxelize_workspace_bytes.restype = C.c_size_t
         lib.sgb_adam_step.argtypes = [C.POINTER(AdamTensor), i32, vp]
         pi64 = C.POINTER(i64)

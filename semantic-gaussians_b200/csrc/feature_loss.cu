@@ -20,6 +20,7 @@
 #include <algorithm>
 #include <cstring>
 #include <cuda_fp16.h>
+#include <cub/cub.cuh>
 
 #include "common.cuh"
 #include "feature_loss.cuh"
@@ -294,6 +295,217 @@ int launch_feature_loss(int loss_type, int C, long long N, const float* render, 
     return launch_elementwise<T, true>(C, N, render, target, dL, loss, s);
 }
 
+// ---- Masked-row loss of a (M, F) row-major network output (MinkUNet's .F) against one (K, C) target row per masked
+// output row, on the column block [h0, h0 + C) (distill.py:111-124 after `output = model_3d(sinput).F[mask]`).
+// Passes: flags -> cub::DeviceScan (rank of each masked row among the masked rows) -> [cosine: count of non-zero target
+// rows] -> one warp per output row, which reads its slice and target row once and writes its whole gradient row
+// once -> one CTA that adds the per-CTA partial sums in a fixed order.  The only atomic is the integer row count,
+// so every output is bitwise reproducible.
+constexpr int kVlRows = 8;                   // warps (= output rows) per CTA
+constexpr int kVlThreads = 32 * kVlRows;
+constexpr int kVlPerLane = kFlMaxC / 32;
+
+struct VlWorkspace {
+    unsigned long long* nv;   // number of target rows with a non-zero element (cosine)
+    int* flags;               // [M] mask[i] != 0
+    int* rank;                // [M] exclusive scan of flags
+    double* partial;          // [ceil(M / kVlRows)] per-CTA loss sums
+    void* tmp;
+    size_t tmp_bytes;
+    size_t bytes;
+};
+
+int carve_vl_workspace(long long M, void* base, VlWorkspace& w) {
+    size_t scan_tmp = 0;
+    SGB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int*)nullptr, (int)M));
+    char* p = (char*)base;
+    size_t off = 0;
+    w.nv = (unsigned long long*)(p + off); off += align_up(sizeof(unsigned long long));
+    w.flags = (int*)(p + off); off += align_up(sizeof(int) * (size_t)M);
+    w.rank = (int*)(p + off); off += align_up(sizeof(int) * (size_t)M);
+    w.partial = (double*)(p + off); off += align_up(sizeof(double) * (size_t)((M + kVlRows - 1) / kVlRows));
+    w.tmp = p + off;
+    w.tmp_bytes = scan_tmp;
+    off += align_up(scan_tmp);
+    w.bytes = off;
+    return SGB_OK;
+}
+
+__global__ void __launch_bounds__(256) vl_flags_kernel(long long M, const uint8_t* __restrict__ mask,
+                                                       int* __restrict__ flags, unsigned long long* nv) {
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i == 0) *nv = 0;
+    if (i < M) flags[i] = mask[i] != 0;
+}
+
+// nv += number of target rows with a non-zero element (features_gt.norm(dim=-1) > 0).  Warp = one row.
+template <typename T>
+__global__ void __launch_bounds__(kVlThreads) vl_count_kernel(long long K, int C, const T* __restrict__ y,
+                                                              unsigned long long* nv) {
+    __shared__ int wn[kVlRows];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long k = (long long)blockIdx.x * kVlRows + warp;
+    int nz = 0;
+    if (k < K)
+        for (int c = lane; c < C && !nz; c += 32) nz = to_f32(y[k * C + c]) != 0.f;
+    nz = __any_sync(0xffffffffu, nz);
+    if (lane == 0) wn[warp] = nz;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int j = 0; j < kVlRows; j++) t += wn[j];
+        if (t) atomicAdd(nv, (unsigned long long)t);
+    }
+}
+
+template <typename T, int LOSS>
+__global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F, const float* __restrict__ x,
+                                                             long long K, int C, int h0, const T* __restrict__ y,
+                                                             const int* __restrict__ flags,
+                                                             const int* __restrict__ rank,
+                                                             const unsigned long long* __restrict__ nv_count,
+                                                             float* __restrict__ grad, double* __restrict__ partial) {
+    __shared__ double wsum[kVlRows];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long i = (long long)blockIdx.x * kVlRows + warp;
+    double term = 0.0;
+    if (i < M) {
+        const float* xr = x + i * F;
+        float* gr = grad + i * F;
+        for (int c = lane; c < h0; c += 32) gr[c] = 0.f;
+        for (int c = h0 + C + lane; c < F; c += 32) gr[c] = 0.f;
+        const long long r = flags[i] ? (long long)rank[i] : -1;
+        if (r < 0 || r >= K) {
+            for (int c = lane; c < C; c += 32) gr[h0 + c] = 0.f;
+        } else {
+            const T* yr = y + r * C;
+            float xv[kVlPerLane], yv[kVlPerLane];
+#pragma unroll
+            for (int j = 0; j < kVlPerLane; j++) {
+                const int c = lane + 32 * j;
+                xv[j] = c < C ? __ldg(xr + h0 + c) : 0.f;
+                yv[j] = c < C ? to_f32(yr[c]) : 0.f;
+            }
+            if (LOSS == SGB_FEATLOSS_COSINE) {
+                float dot = 0.f, xx = 0.f, yy = 0.f;
+                int nz = 0;
+#pragma unroll
+                for (int j = 0; j < kVlPerLane; j++) {
+                    dot = fmaf(xv[j], yv[j], dot);
+                    xx = fmaf(xv[j], xv[j], xx);
+                    yy = fmaf(yv[j], yv[j], yy);
+                    nz |= yv[j] != 0.f;
+                }
+                // xor butterflies: every lane ends with the same, fixed-order sums
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    dot += __shfl_xor_sync(0xffffffffu, dot, o);
+                    xx += __shfl_xor_sync(0xffffffffu, xx, o);
+                    yy += __shfl_xor_sync(0xffffffffu, yy, o);
+                }
+                const bool valid = __any_sync(0xffffffffu, nz);
+                const double nv = (double)*nv_count;
+                const float inv_nv = nv > 0.0 ? (float)(1.0 / nv) : 0.f;
+                const float nx = sqrtf(xx), a = fmaxf(nx, 1e-8f), b = fmaxf(sqrtf(yy), 1e-8f);
+                const float cosv = dot / (a * b);
+                const float u = valid ? -inv_nv / (a * b) : 0.f;
+                const float v = valid && nx > 0.f ? inv_nv * cosv / (a * nx) : 0.f;
+#pragma unroll
+                for (int j = 0; j < kVlPerLane; j++) {
+                    const int c = lane + 32 * j;
+                    if (c < C) gr[h0 + c] = fmaf(u, yv[j], v * xv[j]);
+                }
+                term = valid && lane == 0 ? 1.0 - (double)cosv : 0.0;
+            } else {
+                const float gs = (float)((LOSS == SGB_FEATLOSS_L2 ? 2.0 : 1.0) / ((double)K * (double)C));
+                double acc = 0.0;
+#pragma unroll
+                for (int j = 0; j < kVlPerLane; j++) {
+                    const int c = lane + 32 * j;
+                    if (c < C) {
+                        const float d = xv[j] - yv[j];
+                        gr[h0 + c] = LOSS == SGB_FEATLOSS_L2 ? gs * d : gs * (float)((d > 0.f) - (d < 0.f));
+                        acc += (double)(LOSS == SGB_FEATLOSS_L2 ? d * d : fabsf(d));
+                    }
+                }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+                term = lane == 0 ? acc : 0.0;
+            }
+        }
+    }
+    if (lane == 0) wsum[warp] = term;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int j = 0; j < kVlRows; j++) t += wsum[j];
+        partial[blockIdx.x] = t;
+    }
+}
+
+// loss[0] = sum of the partials / the count, loss[1] = the count (non-zero target rows for cosine, K for l1 / l2;
+// the l1 / l2 mean is over K * C).  A mask whose row count is not K makes both NaN.
+__global__ void __launch_bounds__(256) vl_finish_kernel(long long nb, const double* __restrict__ partial, long long M,
+                                                        const int* __restrict__ flags, const int* __restrict__ rank,
+                                                        long long K, int C, int loss_type,
+                                                        const unsigned long long* __restrict__ nv, double* loss) {
+    __shared__ double s[256];
+    double t = 0.0;
+    for (long long j = threadIdx.x; j < nb; j += 256) t += partial[j];
+    s[threadIdx.x] = t;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    const long long masked = (long long)rank[M - 1] + flags[M - 1];
+    if (masked != K) {
+        loss[0] = loss[1] = __longlong_as_double(0x7ff8000000000000ll);
+        return;
+    }
+    if (loss_type == SGB_FEATLOSS_COSINE) {
+        const double n = (double)*nv;
+        loss[0] = n > 0.0 ? s[0] / n : 0.0;
+        loss[1] = n;
+    } else {
+        loss[0] = K > 0 ? s[0] * (1.0 / ((double)K * (double)C)) : 0.0;
+        loss[1] = (double)K;
+    }
+}
+
+template <typename T, int LOSS>
+int launch_voxel_loss(long long M, int F, const float* x, const uint8_t* mask, long long K, int C, int h0, const T* y,
+                      float* grad, const VlWorkspace& w, double* loss, cudaStream_t s) {
+    vl_flags_kernel<<<(unsigned)((M + 255) / 256), 256, 0, s>>>(M, mask, w.flags, w.nv);
+    SGB_LAUNCH_CHECK("vl_flags_kernel", 0, s);
+    size_t tmp_bytes = w.tmp_bytes;
+    SGB_CUDA(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.flags, w.rank, (int)M, s));
+    if (LOSS == SGB_FEATLOSS_COSINE && K > 0) {
+        vl_count_kernel<T><<<(unsigned)((K + kVlRows - 1) / kVlRows), kVlThreads, 0, s>>>(K, C, y, w.nv);
+        SGB_LAUNCH_CHECK("vl_count_kernel", 0, s);
+    }
+    const long long nb = (M + kVlRows - 1) / kVlRows;
+    vl_loss_kernel<T, LOSS><<<(unsigned)nb, kVlThreads, 0, s>>>(M, F, x, K, C, h0, y, w.flags, w.rank, w.nv, grad,
+                                                                w.partial);
+    SGB_LAUNCH_CHECK("vl_loss_kernel", 0, s);
+    vl_finish_kernel<<<1, 256, 0, s>>>(nb, w.partial, M, w.flags, w.rank, K, C, LOSS, w.nv, loss);
+    SGB_LAUNCH_CHECK("vl_finish_kernel", 0, s);
+    return SGB_OK;
+}
+
+template <typename T>
+int launch_voxel_loss(int loss_type, long long M, int F, const float* x, const uint8_t* mask, long long K, int C,
+                      int h0, const T* y, float* grad, const VlWorkspace& w, double* loss, cudaStream_t s) {
+    if (loss_type == SGB_FEATLOSS_COSINE)
+        return launch_voxel_loss<T, SGB_FEATLOSS_COSINE>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
+    if (loss_type == SGB_FEATLOSS_L1)
+        return launch_voxel_loss<T, SGB_FEATLOSS_L1>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
+    return launch_voxel_loss<T, SGB_FEATLOSS_L2>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
+}
+
+bool vl_m_ok(int64_t M) { return M >= 0 && M <= INT32_MAX; }
+
 }  // namespace
 
 template <typename T>
@@ -334,6 +546,52 @@ int sgb_feature_map_loss(int32_t C, int64_t N, const float* render, const void* 
     if (target_dtype == SGB_FEAT_F16)
         return launch_feature_loss<__half>(loss_type, C, (long long)N, render, (const __half*)target, dL_drender, loss, s);
     return launch_feature_loss<float>(loss_type, C, (long long)N, render, (const float*)target, dL_drender, loss, s);
+}
+
+size_t sgb_voxel_feature_loss_workspace_bytes(int64_t M) {
+    if (!vl_m_ok(M)) return 0;
+    VlWorkspace w;
+    return carve_vl_workspace((long long)M, nullptr, w) == SGB_OK ? w.bytes : 0;
+}
+
+int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint8_t* mask, int64_t K, int32_t C,
+                           int32_t head, const void* target, int32_t target_dtype, int32_t loss_type, float* grad,
+                           void* workspace, double* loss, void* stream) {
+    static const char* fn = "sgb_voxel_feature_loss";
+    if (!vl_m_ok(M)) { set_error("%s: M = %lld outside [0, %d]", fn, (long long)M, INT32_MAX); return SGB_E_INVALID; }
+    if (C <= 0 || C > kFlMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kFlMaxC); return SGB_E_INVALID; }
+    if (head < 0 || (int64_t)head * C + C > F) {
+        set_error("%s: head %d of width %d does not fit in F = %d columns", fn, head, C, F);
+        return SGB_E_INVALID;
+    }
+    if (K < 0 || K > M) { set_error("%s: K = %lld target rows outside [0, M = %lld]", fn, (long long)K, (long long)M); return SGB_E_INVALID; }
+    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
+        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
+        return SGB_E_INVALID;
+    }
+    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
+        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
+        return SGB_E_INVALID;
+    }
+    if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
+    if (M > 0 && (!output || !mask || !grad)) { set_error("%s: null output / mask / grad", fn); return SGB_E_INVALID; }
+    if (K > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
+    if (M > 0 && !workspace) { set_error("%s: null workspace", fn); return SGB_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(workspace) % 16) { set_error("%s: workspace is not 16-byte aligned", fn); return SGB_E_INVALID; }
+    cudaStream_t s = (cudaStream_t)stream;
+    if (M == 0) {
+        SGB_CUDA(cudaMemsetAsync(loss, 0, 2 * sizeof(double), s));
+        return SGB_OK;
+    }
+    VlWorkspace w;
+    const int rc = carve_vl_workspace((long long)M, workspace, w);
+    if (rc) return rc;
+    const int h0 = head * C;
+    if (target_dtype == SGB_FEAT_F16)
+        return launch_voxel_loss<__half>(loss_type, (long long)M, F, output, mask, (long long)K, C, h0,
+                                         (const __half*)target, grad, w, loss, s);
+    return launch_voxel_loss<float>(loss_type, (long long)M, F, output, mask, (long long)K, C, h0,
+                                    (const float*)target, grad, w, loss, s);
 }
 
 }  // extern "C"

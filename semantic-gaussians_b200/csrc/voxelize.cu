@@ -48,8 +48,10 @@ struct VoxWorkspace {
     size_t bytes;
 };
 
-// Voxel floors of point p; false when any axis is not finite.
-__device__ __forceinline__ bool vox_floor(const float* __restrict__ xyz, long long p, const VoxTransform& T,
+// Voxel floors of point p; false when any axis is not finite.  Coord = float or double: either is promoted to double
+// exactly before the transform.
+template <typename Coord>
+__device__ __forceinline__ bool vox_floor(const Coord* __restrict__ xyz, long long p, const VoxTransform& T,
                                           double (&v)[3]) {
     const double x = xyz[3 * p], y = xyz[3 * p + 1], z = xyz[3 * p + 2];
     bool finite = true;
@@ -73,7 +75,8 @@ __global__ void vox_init_kernel(VoxHeader* hdr, int64_t* counts) {
     if (threadIdx.x == 0) hdr->nonfinite = hdr->huge = 0;
 }
 
-__global__ void __launch_bounds__(kVoxThreads) vox_bounds_kernel(long long P, const float* __restrict__ xyz,
+template <typename Coord>
+__global__ void __launch_bounds__(kVoxThreads) vox_bounds_kernel(long long P, const Coord* __restrict__ xyz,
                                                                  VoxTransform T, VoxHeader* hdr) {
     long long lo[3] = {LLONG_MAX, LLONG_MAX, LLONG_MAX}, hi[3] = {LLONG_MIN, LLONG_MIN, LLONG_MIN};
     unsigned nonfinite = 0, huge = 0;
@@ -116,7 +119,8 @@ __device__ __forceinline__ uint64_t vox_rel(double v, long long lo) {
     return (uint64_t)q - (uint64_t)lo;
 }
 
-__global__ void __launch_bounds__(kVoxThreads) vox_key_kernel(long long P, const float* __restrict__ xyz,
+template <typename Coord>
+__global__ void __launch_bounds__(kVoxThreads) vox_key_kernel(long long P, const Coord* __restrict__ xyz,
                                                               VoxTransform T, const VoxHeader* __restrict__ hdr,
                                                               uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
                                                               int64_t* __restrict__ counts) {
@@ -150,7 +154,8 @@ __global__ void __launch_bounds__(kVoxThreads) vox_head_kernel(long long P, cons
 }
 
 // runs[i] = number of run heads in sorted positions [0, i]: the run of position i is runs[i] - 1.
-__global__ void __launch_bounds__(kVoxThreads) vox_scatter_kernel(long long P, const float* __restrict__ xyz,
+template <typename Coord>
+__global__ void __launch_bounds__(kVoxThreads) vox_scatter_kernel(long long P, const Coord* __restrict__ xyz,
                                                                   VoxTransform T, const VoxHeader* __restrict__ hdr,
                                                                   const uint32_t* __restrict__ order,
                                                                   const int* __restrict__ heads,
@@ -195,23 +200,9 @@ int carve_workspace(long long P, void* base, VoxWorkspace& w) {
 
 bool vox_p_ok(int64_t P) { return P >= 1 && P <= INT32_MAX; }
 
-}  // namespace
-
-}  // namespace sgb
-
-using namespace sgb;
-
-extern "C" {
-
-size_t sgb_voxelize_workspace_bytes(int64_t P) {
-    if (!vox_p_ok(P)) return 0;
-    VoxWorkspace w;
-    return carve_workspace((long long)P, nullptr, w) == SGB_OK ? w.bytes : 0;
-}
-
-int sgb_voxelize(int64_t P, const float* xyz, const double* transform, void* workspace, int64_t* first_index,
-                 int64_t* inverse, int32_t* coords, int64_t* counts, void* stream) {
-    const char* fn = "sgb_voxelize";
+template <typename Coord>
+int voxelize(const char* fn, int64_t P, const Coord* xyz, const double* transform, void* workspace,
+             int64_t* first_index, int64_t* inverse, int32_t* coords, int64_t* counts, void* stream) {
     if (P <= 0) { set_error("%s: P = %lld (need at least one point)", fn, (long long)P); return SGB_E_INVALID; }
     if (P > INT32_MAX) { set_error("%s: P = %lld exceeds %d points", fn, (long long)P, INT32_MAX); return SGB_E_INVALID; }
     if (!xyz) { set_error("%s: null xyz", fn); return SGB_E_INVALID; }
@@ -257,6 +248,31 @@ int sgb_voxelize(int64_t P, const float* xyz, const double* transform, void* wor
                                                       coords, counts);
     SGB_LAUNCH_CHECK("vox_scatter_kernel", 0, s);
     return SGB_OK;
+}
+
+}  // namespace
+
+}  // namespace sgb
+
+using namespace sgb;
+
+extern "C" {
+
+size_t sgb_voxelize_workspace_bytes(int64_t P) {
+    if (!vox_p_ok(P)) return 0;
+    VoxWorkspace w;
+    return carve_workspace((long long)P, nullptr, w) == SGB_OK ? w.bytes : 0;
+}
+
+int sgb_voxelize(int64_t P, const float* xyz, const double* transform, void* workspace, int64_t* first_index,
+                 int64_t* inverse, int32_t* coords, int64_t* counts, void* stream) {
+    return voxelize<float>("sgb_voxelize", P, xyz, transform, workspace, first_index, inverse, coords, counts, stream);
+}
+
+int sgb_voxelize_f64(int64_t P, const double* xyz, const double* transform, void* workspace, int64_t* first_index,
+                     int64_t* inverse, int32_t* coords, int64_t* counts, void* stream) {
+    return voxelize<double>("sgb_voxelize_f64", P, xyz, transform, workspace, first_index, inverse, coords, counts,
+                            stream);
 }
 
 }  // extern "C"

@@ -11,7 +11,8 @@ view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:
                        not change the arg-max.
 ``distill_loss_and_grad``      training loss against per-pixel class labels and K class embeddings.
 ``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2).
-``decoded_feature_map_loss_and_grads``  the same loss for a compact field through a per-pixel linear decoder."""
+``decoded_feature_map_loss_and_grads``  the same loss for a compact field through a per-pixel linear decoder.
+``voxel_feature_loss_and_grad``  the same loss on the masked rows of a 3D network's (M, F) output (distill.py)."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -170,6 +171,67 @@ def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, los
                                                    _FEATURE_LOSSES[loss_type], grad.data_ptr(), loss2.data_ptr(),
                                                    stream), "sgb_feature_map_loss")
     return loss2[0], grad
+
+
+def voxel_feature_loss_and_grad(output: torch.Tensor, mask: torch.Tensor, features_gt: torch.Tensor,
+                                loss_type: str = "cosine", head: int = 0, channels: int = 768
+                                ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The 3D distillation loss of distill.py:109-124 and its gradient, without gathering the masked rows.  With
+    x = output[mask][:, head * channels : (head + 1) * channels] and y = features_gt.float():
+
+        "cosine"  m = y.norm(dim=-1) > 0;  (1 - torch.nn.CosineSimilarity()(x[m], y[m])).mean()
+        "l1"      torch.nn.L1Loss()(x, y)
+        "l2"      torch.nn.MSELoss()(x, y)
+
+    output: MinkUNet's (M, F) fp32 ``.F`` (read detached); mask: (M,) bool; features_gt: (mask.sum(), channels) fp16
+    or fp32, one row per masked row in row order (``FeatureDataset`` / ``distill_targets`` give exactly that).
+
+    Returns (loss, count, grad): 0-d float64 CUDA tensors and the (M, F) fp32 d loss / d output, zero outside the
+    masked rows and the head's columns.  Use as ``out.F.backward(grad)``.  ``count`` is the number of rows averaged
+    over (cosine: target rows with a non-zero element; l1 / l2: mask.sum()).  When it is 0 the loss and grad are 0;
+    the reference ``continue``s past such a cosine batch (and l1 / l2 give NaN there), so a caller that wants the
+    same skip reads ``count`` (one sync) and leaves out ``optimizer.step()``: a step with a zero gradient still
+    applies AdamW's weight decay.  If mask.sum() is not features_gt's row count, loss and count are NaN.  Nothing
+    is synchronised; every output is bitwise reproducible.  1 <= channels <= 1024, (head + 1) * channels <= F."""
+    if loss_type not in _FEATURE_LOSSES:
+        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
+    for name, t in (("output", output), ("mask", mask), ("features_gt", features_gt)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError(f"{name} must be a CUDA tensor (the voxel feature loss has no CPU path)")
+    if not (output.device == mask.device == features_gt.device):
+        raise ValueError("output, mask and features_gt must be on one device")
+    if output.dtype != torch.float32 or output.ndim != 2:
+        raise ValueError(f"output must be (M, F) float32, got {tuple(output.shape)} {output.dtype}")
+    M, F = output.shape
+    if mask.dtype != torch.bool or mask.shape != (M,):
+        raise ValueError(f"mask must be ({M},) bool, got {tuple(mask.shape)} {mask.dtype}")
+    if features_gt.requires_grad:
+        raise ValueError("features_gt must not require grad (the loss gives the gradient of the output only)")
+    if features_gt.dtype not in (torch.float16, torch.float32) or features_gt.ndim != 2 \
+            or features_gt.shape[1] != channels:
+        raise ValueError(f"features_gt must be (K, {channels}) float16 or float32, got {tuple(features_gt.shape)} "
+                         f"{features_gt.dtype}")
+    if not 1 <= channels <= 1024 or head < 0 or (head + 1) * channels > F:
+        raise ValueError(f"head {head} of {channels} channels does not fit in {F} columns (1 <= channels <= 1024)")
+    if features_gt.shape[0] > M:
+        raise ValueError(f"features_gt has {features_gt.shape[0]} rows, more than the {M} rows of output")
+    x = output.detach().contiguous()
+    y = features_gt.contiguous()
+    m = mask.contiguous()
+    grad = torch.empty_like(x)
+    loss2 = torch.empty(2, dtype=torch.float64, device=x.device)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        nbytes = lib.sgb_voxel_feature_loss_workspace_bytes(M)
+        if nbytes == 0:
+            raise _lib.SgbError("sgb_voxel_feature_loss_workspace_bytes failed")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
+        _lib.check(lib.sgb_voxel_feature_loss(M, F, x.data_ptr(), m.data_ptr(), y.shape[0], channels, head,
+                                              y.data_ptr(), dtype, _FEATURE_LOSSES[loss_type], grad.data_ptr(),
+                                              ws.data_ptr(), loss2.data_ptr(), stream), "sgb_voxel_feature_loss")
+    return loss2[0], loss2[1], grad
 
 
 def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Tensor, target: torch.Tensor,

@@ -23,7 +23,7 @@ SGB_E_CUDA, SGB_E_OVERFLOW = -2, -4
 
 
 def voxel_indices(xyz: torch.Tensor, transform):
-    """``sparse_quantize(floor(homo(xyz) @ transform.T), return_index=True)`` of a CUDA (P,3) fp32 cloud.
+    """``sparse_quantize(floor(homo(xyz) @ transform.T), return_index=True)`` of a CUDA (P,3) fp32 or fp64 cloud.
 
     ``transform``: the first three rows of a 3x4 or 4x4 fp64 matrix.  Returns ``(first_index (M,) int64,
     inverse (P,) int64, coords (M,3) int32)``: np.unique's return_index and return_inverse over the FNV-1a keys, and
@@ -32,8 +32,8 @@ def voxel_indices(xyz: torch.Tensor, transform):
     more.  Enqueued on the current stream; reads M and the status words back once."""
     if not isinstance(xyz, torch.Tensor) or not xyz.is_cuda:
         raise ValueError("xyz must be a CUDA tensor")
-    if xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] != 3:
-        raise ValueError(f"xyz must be (P, 3) float32, got {tuple(xyz.shape)} {xyz.dtype}")
+    if xyz.dtype not in (torch.float32, torch.float64) or xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise ValueError(f"xyz must be (P, 3) float32 or float64, got {tuple(xyz.shape)} {xyz.dtype}")
     T = np.ascontiguousarray(np.asarray(transform, np.float64)[:3, :4])
     if T.shape != (3, 4):
         raise ValueError(f"transform must have 3 rows and 4 columns, got {np.asarray(transform).shape}")
@@ -53,9 +53,9 @@ def voxel_indices(xyz: torch.Tensor, transform):
         coords = torch.empty((P, 3), dtype=torch.int32, device=dev)
         counts = torch.empty(3, dtype=torch.int64, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.sgb_voxelize(P, x.data_ptr(), (C.c_double * 12)(*T.ravel()), ws.data_ptr(), first.data_ptr(),
-                                    inverse.data_ptr(), coords.data_ptr(), counts.data_ptr(), stream),
-                   "sgb_voxelize")
+        name = "sgb_voxelize_f64" if x.dtype == torch.float64 else "sgb_voxelize"
+        _lib.check(getattr(lib, name)(P, x.data_ptr(), (C.c_double * 12)(*T.ravel()), ws.data_ptr(), first.data_ptr(),
+                                      inverse.data_ptr(), coords.data_ptr(), counts.data_ptr(), stream), name)
         M, nonfinite, status = counts.tolist()
     if nonfinite:
         raise ValueError(f"{nonfinite} of {P} points have a non-finite voxel coordinate")
@@ -86,8 +86,8 @@ class Voxelizer:
     """The reference's ``Voxelizer`` (same constructor and results) with the quantization on the GPU.
 
     numpy inputs give numpy outputs (coords as float64, as the reference returns them); CUDA tensors give CUDA
-    tensors and are never copied to the host.  Coordinates must be float32 (the Gaussians' xyz).  ``clip_bound`` is
-    not supported: no reference caller sets it."""
+    tensors and are never copied to the host.  Coordinates are float32 (the Gaussians' xyz) or float64 (the cloud
+    after ``feature_dataset.ElasticDistortion``).  ``clip_bound`` is not supported: no reference caller sets it."""
 
     def __init__(self, voxel_size=1, clip_bound=None, use_augmentation=False, scale_augmentation_bound=None,
                  rotation_augmentation_bound=None, translation_augmentation_ratio_bound=None, ignore_label=255):
@@ -131,8 +131,8 @@ class Voxelizer:
         if coords.ndim != 2 or coords.shape[1] != 3 or coords.shape[0] == 0 or feats.shape[0] != coords.shape[0]:
             raise ValueError(f"need coords (P, 3) with P > 0 and feats with P rows, got {tuple(coords.shape)} and "
                              f"{tuple(feats.shape)}")
-        if coords.dtype not in (np.float32, torch.float32):
-            raise ValueError(f"coords must be float32, got {coords.dtype}")
+        if coords.dtype not in (np.float32, np.float64, torch.float32, torch.float64):
+            raise ValueError(f"coords must be float32 or float64, got {coords.dtype}")
         M_v, M_r = self.get_transformation_matrix()
         transform = M_r @ M_v if self.use_augmentation else M_v
         if isinstance(coords, torch.Tensor):
