@@ -4,7 +4,7 @@
 //
 //   x_p = W r_p + b          W (C, c) row-major (nn.Linear(c, C).weight), b (C) or absent
 //
-// and the loss on x against Y is that of feature_loss.cu (cosine with its valid-pixel mask, l1, l2).  With
+// and the loss on x against Y is that of feature_loss.cuh (cosine with its valid-pixel mask, l1, l2).  With
 // g_p = dLoss / dx_p the call returns dL/dR[:, p] = W^T g_p, dL/dW = sum_p g_p r_p^T and dL/db = sum_p g_p, without
 // writing x or g anywhere but shared memory.
 //
@@ -48,12 +48,9 @@ constexpr int kDlThreads = 256;
 constexpr int kDlPB = 128;            // pixels per block
 constexpr int kDlCC = 64;             // decoded channels per chunk
 constexpr int kDlPitch = kDlPB + 4;   // shared row pitch of the R and G tiles: float4 rows 1..15 apart hit other banks
-constexpr int kDlMaxC = 1024;         // widest feature map accepted (as sgb_feature_map_loss)
 constexpr int kDlMaxc = 128;          // widest compact field accepted
 constexpr int kDlMaxCtas = kNumSMs;
 constexpr int kDlMaxSmem = 226 * 1024;  // dynamic: the 227 KB per-CTA opt-in limit less the static wsum[]
-
-enum { kDlCos = SGB_FEATLOSS_COSINE, kDlL1 = SGB_FEATLOSS_L1, kDlL2 = SGB_FEATLOSS_L2 };
 
 inline int padded_c(int c) { return c <= 16 ? 16 : c <= 32 ? 32 : c <= 64 ? 64 : 128; }
 __host__ __device__ inline int padded_C(int C) { return (C + kDlCC - 1) / kDlCC * kDlCC; }
@@ -77,9 +74,6 @@ DlWorkspace workspace_layout(int C, int c) {
     return w;
 }
 
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-
 // W (C, c) and b into the layouts the main kernel stages, zero outside (C, c): Wp [Cp][cp] row-major, Wt
 // [Cp / 64][cp][64] (each chunk's 64 rows as contiguous columns), bp [Cp].
 __global__ void __launch_bounds__(256) decoder_pack_kernel(int C, int c, int cp, const float* __restrict__ W,
@@ -95,23 +89,13 @@ __global__ void __launch_bounds__(256) decoder_pack_kernel(int C, int c, int cp,
     }
 }
 
-struct Quad { float v[4]; };
-
 // Four consecutive pixels of one target plane, `rem` of them inside the image.  VEC: p is 16- (fp32) or 8-byte
 // (fp16) aligned and rem is a multiple of 4.
 template <typename T>
 __device__ __forceinline__ Quad load_target4(const T* p, long long rem, bool vec) {
     Quad q;
     if (vec && rem >= 4) {
-        if constexpr (sizeof(T) == 4) {
-            const float4 f = __ldg(reinterpret_cast<const float4*>(p));
-            q = {{f.x, f.y, f.z, f.w}};
-        } else {
-            const uint2 r = __ldg(reinterpret_cast<const uint2*>(p));
-            const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
-            const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
-            q = {{a.x, a.y, b.x, b.y}};
-        }
+        q = load4(p);
     } else {
 #pragma unroll
         for (int j = 0; j < 4; j++) q.v[j] = j < rem ? to_f32(p[j]) : 0.f;
@@ -137,7 +121,7 @@ struct DlArgs {
 
 // Thread (tx, ty) = (tid % 16, tid / 16).  Its 8 pixel columns of a block are px(q) = 4 tx + q % 4 + 64 (q / 4), its
 // 4 decoded rows of a chunk 4 ty + i, its dL/dR channels CP/16 ty + j, its dL/dW columns tx + 16 j.
-template <typename T, int CP, int LT>
+template <typename T, int CP, int LOSS>
 __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArgs a) {
     constexpr int TC = CP / 16;
     const int C = a.C, c = a.c, Cp = padded_C(C), nch = Cp / kDlCC;
@@ -160,11 +144,11 @@ __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArg
     float* dwp = a.dw_part + (size_t)blockIdx.x * Cp * CP;
     for (int i = tid; i < Cp; i += kDlThreads) dbs[i] = 0.f;
     float inv_nv = 0.f;
-    if (LT == kDlCos) {
+    if (LOSS == SGB_FEATLOSS_COSINE) {
         const double nv = a.loss[1];
         inv_nv = nv > 0.0 ? (float)(1.0 / nv) : 0.f;
     }
-    const float gs = (float)((LT == kDlL2 ? 2.0 : 1.0) / ((double)N * C));
+    const float gs = (float)((LOSS == SGB_FEATLOSS_L2 ? 2.0 : 1.0) / ((double)N * C));
     double lsum = 0.0;
 
     auto px = [&](int q) { return 4 * tx + (q & 3) + 64 * (q >> 2); };
@@ -229,7 +213,7 @@ __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArg
             Rs[k * kDlPitch + p] = k < c && p0 + p < N ? __ldg(a.R + (size_t)k * N + p0 + p) : 0.f;
         }
         float u[8], v[8];
-        if constexpr (LT == kDlCos) {
+        if constexpr (LOSS == SGB_FEATLOSS_COSINE) {
             float dot[8], xx[8], yy[8];
             unsigned nz = 0;
 #pragma unroll
@@ -270,13 +254,9 @@ __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArg
                     b2 += red[(2 * 16 + k) * kDlPB + tid];
                     any += red[(3 * 16 + k) * kDlPB + tid];
                 }
-                const float nx = sqrtf(a2), an = fmaxf(nx, 1e-8f), bn = fmaxf(sqrtf(b2), 1e-8f);
-                const float cosv = d / (an * bn);
                 const bool valid = any > 0.f && p0 + tid < N;
-                // d cos / dx = y / (a b) - cos x / (a |x|), as feature_loss.cu
-                cu[tid] = valid ? -inv_nv / (an * bn) : 0.f;
-                cv[tid] = valid && nx > 0.f ? inv_nv * cosv / (an * nx) : 0.f;
-                if (valid) lsum += 1.0 - (double)cosv;
+                const double t = cosine_rule(d, a2, b2, valid, inv_nv, cu[tid], cv[tid]);
+                if (valid) lsum += t;
             }
             __syncthreads();
 #pragma unroll
@@ -298,20 +278,21 @@ __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArg
             {
                 float x[4][8], y[4][8];
                 decode(x);
-                load_target(ch, p0, LT == kDlCos && a.ycache, y);
+                load_target(ch, p0, LOSS == SGB_FEATLOSS_COSINE && a.ycache, y);
                 float lpart = 0.f;
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
                     float g[8], rs = 0.f;
 #pragma unroll
                     for (int q = 0; q < 8; q++) {
-                        if constexpr (LT == kDlCos) {
+                        if constexpr (LOSS == SGB_FEATLOSS_COSINE) {
                             g[q] = fmaf(u[q], y[i][q], v[q] * x[i][q]);
                         } else {
-                            const float d = x[i][q] - y[i][q];
+                            float ge;
+                            const float t = elementwise_rule<LOSS>(x[i][q] - y[i][q], gs, ge);
                             const bool in = p0 + px(q) < N;
-                            g[q] = in ? (LT == kDlL2 ? gs * d : gs * (float)((d > 0.f) - (d < 0.f))) : 0.f;
-                            lpart += in ? (LT == kDlL2 ? d * d : fabsf(d)) : 0.f;
+                            g[q] = in ? ge : 0.f;
+                            lpart += in ? t : 0.f;
                         }
                         rs += g[q];
                     }
@@ -323,7 +304,7 @@ __global__ void __launch_bounds__(kDlThreads, 1) decoder_loss_kernel(const DlArg
                     for (int o = 8; o > 0; o >>= 1) rs += __shfl_xor_sync(0xffffffffu, rs, o);
                     if (tx == 0) dbs[ch * kDlCC + 4 * ty + i] += rs;
                 }
-                if (LT != kDlCos) lsum += (double)lpart;
+                if (LOSS != SGB_FEATLOSS_COSINE) lsum += (double)lpart;
             }
             __syncthreads();
             // dL/dR += W_ch^T G
@@ -439,7 +420,7 @@ __global__ void __launch_bounds__(256) decoder_reduce_kernel(int C, int c, int c
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         double t = 0.0;
         for (int k = 0; k < ncta; k++) t += loss_part[k];
-        if (loss_type == kDlCos) {
+        if (loss_type == SGB_FEATLOSS_COSINE) {
             const double nv = loss[1];
             loss[0] = nv > 0.0 ? t / nv : 0.0;
         } else {
@@ -453,26 +434,26 @@ size_t main_smem_bytes(int CP, int Cp) {
     return sizeof(float) * ((size_t)CP * kDlPitch + kDlCC * kDlPitch + 2 * kDlCC * CP + kDlCC + 2 * kDlPB + Cp);
 }
 
-template <typename T, int CP, int LT>
+template <typename T, int CP, int LOSS>
 int launch_main(DlArgs& a, int ncta, cudaStream_t s) {
     const int Cp = padded_C(a.C);
     const size_t base = main_smem_bytes(CP, Cp), yc = (size_t)Cp * kDlPB * sizeof(T);
-    a.ycache = LT == kDlCos && base + yc <= (size_t)kDlMaxSmem;
+    a.ycache = LOSS == SGB_FEATLOSS_COSINE && base + yc <= (size_t)kDlMaxSmem;
     const size_t smem = base + (a.ycache ? yc : 0);
     static DeviceOnce attr_set;
     if (attr_set.first_use_on_device())
-        SGB_CUDA(cudaFuncSetAttribute(decoder_loss_kernel<T, CP, LT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        SGB_CUDA(cudaFuncSetAttribute(decoder_loss_kernel<T, CP, LOSS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       kDlMaxSmem));
-    decoder_loss_kernel<T, CP, LT><<<ncta, kDlThreads, smem, s>>>(a);
+    decoder_loss_kernel<T, CP, LOSS><<<ncta, kDlThreads, smem, s>>>(a);
     SGB_LAUNCH_CHECK("decoder_loss_kernel", 0, s);
     return SGB_OK;
 }
 
 template <typename T, int CP>
 int launch_loss(int loss_type, DlArgs& a, int ncta, cudaStream_t s) {
-    if (loss_type == kDlCos) return launch_main<T, CP, kDlCos>(a, ncta, s);
-    if (loss_type == kDlL1) return launch_main<T, CP, kDlL1>(a, ncta, s);
-    return launch_main<T, CP, kDlL2>(a, ncta, s);
+    if (loss_type == SGB_FEATLOSS_COSINE) return launch_main<T, CP, SGB_FEATLOSS_COSINE>(a, ncta, s);
+    if (loss_type == SGB_FEATLOSS_L1) return launch_main<T, CP, SGB_FEATLOSS_L1>(a, ncta, s);
+    return launch_main<T, CP, SGB_FEATLOSS_L2>(a, ncta, s);
 }
 
 template <typename T>
@@ -493,7 +474,7 @@ using namespace sgb;
 extern "C" {
 
 size_t sgb_decoded_feature_loss_workspace_bytes(int32_t C, int32_t c, int64_t N) {
-    if (C < 1 || C > kDlMaxC || c < 1 || c > kDlMaxc || N < 0) return 0;
+    if (C < 1 || C > kFeatMaxC || c < 1 || c > kDlMaxc || N < 0) return 0;
     return workspace_layout(C, c).total;
 }
 
@@ -502,17 +483,9 @@ int sgb_decoded_feature_loss(int32_t C, int32_t c, int64_t N, const float* rende
                              float* dL_drender, float* dL_dweight, float* dL_dbias, void* workspace, double* loss,
                              void* stream) {
     static const char* fn = "sgb_decoded_feature_loss";
-    if (C <= 0 || C > kDlMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kDlMaxC); return SGB_E_INVALID; }
+    if (check_feature_loss_args(fn, C, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
     if (c <= 0 || c > kDlMaxc) { set_error("%s: c = %d outside [1, %d]", fn, c, kDlMaxc); return SGB_E_INVALID; }
     if (N < 0) { set_error("%s: N = %lld is negative", fn, (long long)N); return SGB_E_INVALID; }
-    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
-        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
-        return SGB_E_INVALID;
-    }
-    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
-        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
-        return SGB_E_INVALID;
-    }
     if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
     if (!dL_dweight) { set_error("%s: null dL_dweight", fn); return SGB_E_INVALID; }
     if (dL_dbias && !bias) { set_error("%s: dL_dbias given without bias", fn); return SGB_E_INVALID; }

@@ -30,12 +30,8 @@ namespace sgb {
 namespace {
 
 constexpr int kFlThreads = 256;
-constexpr int kFlMaxC = 1024;              // widest feature map accepted (OpenSeg 768, LSeg 512)
 constexpr int kFlMaxBox = 256;             // TMA box limit per dimension
 constexpr size_t kFlStageTarget = 48 * 1024;  // staged bytes per CTA aimed at: four CTAs per SM
-
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
 
 // loss[1] = number of pixels whose target column has a non-zero element (features_gt.norm(dim=-1) > 0).  Thread =
 // one pixel.  Channel 0 decides almost every pixel of a real feature map; the rest of a column is read in groups of
@@ -146,14 +142,9 @@ __global__ void __launch_bounds__(kFlThreads) feature_cosine_kernel(int C, long 
         }
         const double nv = loss[1];
         const float inv_nv = nv > 0.0 ? (float)(1.0 / nv) : 0.f;
-        const float nx = sqrtf(a2), a = fmaxf(nx, 1e-8f), b = fmaxf(sqrtf(b2), 1e-8f);
-        const float cosv = d / (a * b);
         const bool valid = any && p0 + tid < N;
-        // d cos / dx = y / (a b) - cos x / (a |x|): the norm's own derivative x / |x| is unclamped (torch clamps the
-        // norms under no_grad), and is zero for x = 0
-        coef[0][tid] = valid ? -inv_nv / (a * b) : 0.f;
-        coef[1][tid] = valid && nx > 0.f ? inv_nv * cosv / (a * nx) : 0.f;
-        term = valid ? 1.0 - (double)cosv : 0.0;
+        const double t = cosine_rule(d, a2, b2, valid, inv_nv, coef[0][tid], coef[1][tid]);
+        term = valid ? t : 0.0;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) term += __shfl_xor_sync(0xffffffffu, term, o);
@@ -172,31 +163,14 @@ __global__ void __launch_bounds__(kFlThreads) feature_cosine_kernel(int C, long 
     for (int c = g; c < C; c += G) out[(size_t)c * N] = fmaf(u, to_f32(Ys[c * PB + tp]), v * Xs[c * PB + tp]);
 }
 
-struct Quad { float v[4]; };
-__device__ __forceinline__ Quad load4(const float* p) {
-    const float4 q = __ldg(reinterpret_cast<const float4*>(p));
-    return {{q.x, q.y, q.z, q.w}};
-}
-__device__ __forceinline__ Quad load4(const __half* p) {
-    const uint2 r = __ldg(reinterpret_cast<const uint2*>(p));
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&r.x));
-    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&r.y));
-    return {{a.x, a.y, b.x, b.y}};
-}
-
-// l1 / l2 over the M = N*C values: gradient sign(x - y) / M (sign(0) = 0, as abs()'s backward) or 2 (x - y) / M.
-// VEC: render, target and dL start 16-/8-byte aligned, so the first M - M % 4 values go as 4-wide loads.
-template <typename T, bool L2, bool VEC>
+// l1 / l2 over the M = N*C values.  VEC: render, target and dL start 16-/8-byte aligned, so the first M - M % 4
+// values go as 4-wide loads.
+template <typename T, int LOSS, bool VEC>
 __global__ void __launch_bounds__(256) feature_elementwise_kernel(long long M, long long N, const float* __restrict__ x,
                                                                   const T* __restrict__ y, float* __restrict__ dL,
                                                                   double* __restrict__ loss) {
     const double inv_m = 1.0 / (double)M;
-    const float gs = (float)((L2 ? 2.0 : 1.0) * inv_m);
-    auto term = [&](float xv, float yv, float& g) {
-        const float d = xv - yv;
-        g = L2 ? gs * d : gs * (float)((d > 0.f) - (d < 0.f));
-        return L2 ? d * d : fabsf(d);
-    };
+    const float gs = (float)((LOSS == SGB_FEATLOSS_L2 ? 2.0 : 1.0) * inv_m);
     const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
     double acc = 0.0;
     long long tail = 0;
@@ -206,7 +180,7 @@ __global__ void __launch_bounds__(256) feature_elementwise_kernel(long long M, l
             const Quad a = load4(x + 4 * i), b = load4(y + 4 * i);
             float g[4], s = 0.f;
 #pragma unroll
-            for (int j = 0; j < 4; j++) s += term(a.v[j], b.v[j], g[j]);
+            for (int j = 0; j < 4; j++) s += elementwise_rule<LOSS>(a.v[j] - b.v[j], gs, g[j]);
             *reinterpret_cast<float4*>(dL + 4 * i) = make_float4(g[0], g[1], g[2], g[3]);
             acc += (double)s;
         }
@@ -214,7 +188,7 @@ __global__ void __launch_bounds__(256) feature_elementwise_kernel(long long M, l
     }
     for (long long i = tail + t0; i < M; i += stride) {
         float g;
-        acc += (double)term(__ldg(x + i), to_f32(y[i]), g);
+        acc += (double)elementwise_rule<LOSS>(__ldg(x + i) - to_f32(y[i]), gs, g);
         dL[i] = g;
     }
 #pragma unroll
@@ -274,15 +248,15 @@ int launch_cosine(int C, long long N, const float* render, const T* target, floa
     return SGB_OK;
 }
 
-template <typename T, bool L2>
+template <typename T, int LOSS>
 int launch_elementwise(int C, long long N, const float* render, const T* target, float* dL, double* loss, cudaStream_t s) {
     const long long M = N * C;
     const bool vec = (reinterpret_cast<uintptr_t>(render) & 15) == 0 && (reinterpret_cast<uintptr_t>(dL) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(target) & (4 * sizeof(T) - 1)) == 0;
     const long long work = vec ? M / 4 : M;
     const unsigned blocks = (unsigned)std::max(1ll, std::min((work + 255) / 256, (long long)kNumSMs * 8));
-    if (vec) feature_elementwise_kernel<T, L2, true><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
-    else feature_elementwise_kernel<T, L2, false><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
+    if (vec) feature_elementwise_kernel<T, LOSS, true><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
+    else feature_elementwise_kernel<T, LOSS, false><<<blocks, 256, 0, s>>>(M, N, render, target, dL, loss);
     SGB_LAUNCH_CHECK("feature_elementwise_kernel", 0, s);
     return SGB_OK;
 }
@@ -291,8 +265,8 @@ template <typename T>
 int launch_feature_loss(int loss_type, int C, long long N, const float* render, const T* target, float* dL,
                         double* loss, cudaStream_t s) {
     if (loss_type == SGB_FEATLOSS_COSINE) return launch_cosine<T>(C, N, render, target, dL, loss, s);
-    if (loss_type == SGB_FEATLOSS_L1) return launch_elementwise<T, false>(C, N, render, target, dL, loss, s);
-    return launch_elementwise<T, true>(C, N, render, target, dL, loss, s);
+    if (loss_type == SGB_FEATLOSS_L1) return launch_elementwise<T, SGB_FEATLOSS_L1>(C, N, render, target, dL, loss, s);
+    return launch_elementwise<T, SGB_FEATLOSS_L2>(C, N, render, target, dL, loss, s);
 }
 
 // ---- Masked-row loss of a (M, F) row-major network output (MinkUNet's .F) against one (K, C) target row per masked
@@ -303,7 +277,7 @@ int launch_feature_loss(int loss_type, int C, long long N, const float* render, 
 // so every output is bitwise reproducible.
 constexpr int kVlRows = 8;                   // warps (= output rows) per CTA
 constexpr int kVlThreads = 32 * kVlRows;
-constexpr int kVlPerLane = kFlMaxC / 32;
+constexpr int kVlPerLane = kFeatMaxC / 32;
 
 struct VlWorkspace {
     unsigned long long* nv;   // number of target rows with a non-zero element (cosine)
@@ -406,16 +380,14 @@ __global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F,
                 const bool valid = __any_sync(0xffffffffu, nz);
                 const double nv = (double)*nv_count;
                 const float inv_nv = nv > 0.0 ? (float)(1.0 / nv) : 0.f;
-                const float nx = sqrtf(xx), a = fmaxf(nx, 1e-8f), b = fmaxf(sqrtf(yy), 1e-8f);
-                const float cosv = dot / (a * b);
-                const float u = valid ? -inv_nv / (a * b) : 0.f;
-                const float v = valid && nx > 0.f ? inv_nv * cosv / (a * nx) : 0.f;
+                float u, v;
+                const double t = cosine_rule(dot, xx, yy, valid, inv_nv, u, v);
 #pragma unroll
                 for (int j = 0; j < kVlPerLane; j++) {
                     const int c = lane + 32 * j;
                     if (c < C) gr[h0 + c] = fmaf(u, yv[j], v * xv[j]);
                 }
-                term = valid && lane == 0 ? 1.0 - (double)cosv : 0.0;
+                term = valid && lane == 0 ? t : 0.0;
             } else {
                 const float gs = (float)((LOSS == SGB_FEATLOSS_L2 ? 2.0 : 1.0) / ((double)K * (double)C));
                 double acc = 0.0;
@@ -423,9 +395,10 @@ __global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F,
                 for (int j = 0; j < kVlPerLane; j++) {
                     const int c = lane + 32 * j;
                     if (c < C) {
-                        const float d = xv[j] - yv[j];
-                        gr[h0 + c] = LOSS == SGB_FEATLOSS_L2 ? gs * d : gs * (float)((d > 0.f) - (d < 0.f));
-                        acc += (double)(LOSS == SGB_FEATLOSS_L2 ? d * d : fabsf(d));
+                        float g;
+                        const float t = elementwise_rule<LOSS>(xv[j] - yv[j], gs, g);
+                        gr[h0 + c] = g;
+                        acc += (double)t;
                     }
                 }
 #pragma unroll
@@ -517,6 +490,19 @@ int count_valid_pixels(int C, long long N, const T* target, double* valid, cudaS
 template int count_valid_pixels<float>(int, long long, const float*, double*, cudaStream_t);
 template int count_valid_pixels<__half>(int, long long, const __half*, double*, cudaStream_t);
 
+int check_feature_loss_args(const char* fn, int C, int target_dtype, int loss_type) {
+    if (C <= 0 || C > kFeatMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kFeatMaxC); return SGB_E_INVALID; }
+    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
+        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
+        return SGB_E_INVALID;
+    }
+    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
+        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
+        return SGB_E_INVALID;
+    }
+    return SGB_OK;
+}
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -526,16 +512,8 @@ extern "C" {
 int sgb_feature_map_loss(int32_t C, int64_t N, const float* render, const void* target, int32_t target_dtype,
                          int32_t loss_type, float* dL_drender, double* loss, void* stream) {
     static const char* fn = "sgb_feature_map_loss";
-    if (C <= 0 || C > kFlMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kFlMaxC); return SGB_E_INVALID; }
+    if (check_feature_loss_args(fn, C, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
     if (N < 0) { set_error("%s: N = %lld is negative", fn, (long long)N); return SGB_E_INVALID; }
-    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
-        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
-        return SGB_E_INVALID;
-    }
-    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
-        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
-        return SGB_E_INVALID;
-    }
     if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
     if (N > 0 && !render) { set_error("%s: null render", fn); return SGB_E_INVALID; }
     if (N > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
@@ -559,20 +537,12 @@ int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint
                            void* workspace, double* loss, void* stream) {
     static const char* fn = "sgb_voxel_feature_loss";
     if (!vl_m_ok(M)) { set_error("%s: M = %lld outside [0, %d]", fn, (long long)M, INT32_MAX); return SGB_E_INVALID; }
-    if (C <= 0 || C > kFlMaxC) { set_error("%s: C = %d outside [1, %d]", fn, C, kFlMaxC); return SGB_E_INVALID; }
+    if (check_feature_loss_args(fn, C, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
     if (head < 0 || (int64_t)head * C + C > F) {
         set_error("%s: head %d of width %d does not fit in F = %d columns", fn, head, C, F);
         return SGB_E_INVALID;
     }
     if (K < 0 || K > M) { set_error("%s: K = %lld target rows outside [0, M = %lld]", fn, (long long)K, (long long)M); return SGB_E_INVALID; }
-    if (target_dtype != SGB_FEAT_F16 && target_dtype != SGB_FEAT_F32) {
-        set_error("%s: unknown target_dtype %d (SGB_FEAT_F16 or SGB_FEAT_F32)", fn, target_dtype);
-        return SGB_E_INVALID;
-    }
-    if (loss_type != SGB_FEATLOSS_COSINE && loss_type != SGB_FEATLOSS_L1 && loss_type != SGB_FEATLOSS_L2) {
-        set_error("%s: unknown loss_type %d (SGB_FEATLOSS_COSINE, _L1 or _L2)", fn, loss_type);
-        return SGB_E_INVALID;
-    }
     if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
     if (M > 0 && (!output || !mask || !grad)) { set_error("%s: null output / mask / grad", fn); return SGB_E_INVALID; }
     if (K > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }

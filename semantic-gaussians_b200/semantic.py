@@ -130,6 +130,19 @@ def distill_loss_and_grad(rendering: torch.Tensor, class_emb: torch.Tensor, labe
 
 
 _FEATURE_LOSSES = {"cosine": _lib.FEATLOSS_COSINE, "l1": _lib.FEATLOSS_L1, "l2": _lib.FEATLOSS_L2}
+_FEATURE_MAX_C = 1024          # widest feature map the feature-loss kernels accept
+
+
+def _feature_loss_codes(loss_type: str, target: torch.Tensor, name: str, grads_of: str) -> Tuple[int, int]:
+    """(FEATLOSS_* code of loss_type, FEAT_* code of target's dtype) for the feature-loss entry points; ValueError
+    for an unknown loss_type, a target that requires grad or one that is not float16 / float32."""
+    if loss_type not in _FEATURE_LOSSES:
+        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
+    if target.requires_grad:
+        raise ValueError(f"{name} must not require grad (the loss gives the gradient{grads_of} only)")
+    if target.dtype not in (torch.float16, torch.float32):
+        raise ValueError(f"{name} must be float16 or float32, got {target.dtype}")
+    return _FEATURE_LOSSES[loss_type], _lib.FEAT_F16 if target.dtype == torch.float16 else _lib.FEAT_F32
 
 
 def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, loss_type: str = "cosine"
@@ -145,14 +158,9 @@ def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, los
 
     Returns (loss: 0-d float64 CUDA tensor, grad: (C,H,W) float32 = d loss / d rendering).  Use as
     ``rendering.backward(grad)``.  Nothing is synchronised and no full-size temporary is allocated besides grad."""
-    if loss_type not in _FEATURE_LOSSES:
-        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
     if not isinstance(rendering, torch.Tensor) or not isinstance(target, torch.Tensor):
         raise ValueError("rendering and target must be tensors")
-    if target.requires_grad:
-        raise ValueError("target must not require grad (the loss gives the gradient of the rendering only)")
-    if target.dtype not in (torch.float16, torch.float32):
-        raise ValueError(f"target must be float16 or float32, got {target.dtype}")
+    loss_code, dtype = _feature_loss_codes(loss_type, target, "target", " of the rendering")
     if rendering.ndim != 3 or target.shape != rendering.shape:
         raise ValueError(f"rendering and target must both be (C,H,W), got {tuple(rendering.shape)} and "
                          f"{tuple(target.shape)}")
@@ -164,12 +172,10 @@ def feature_map_loss_and_grad(rendering: torch.Tensor, target: torch.Tensor, los
     C_, H, W = r.shape
     grad = torch.empty_like(r)
     loss2 = torch.empty(2, dtype=torch.float64, device=r.device)      # [loss, pixels averaged over]; zeroed by the call
-    dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
     with torch.cuda.device(r.device):
         stream = torch.cuda.current_stream(r.device).cuda_stream
-        _lib.check(_lib.load().sgb_feature_map_loss(C_, H * W, r.data_ptr(), y.data_ptr(), dtype,
-                                                   _FEATURE_LOSSES[loss_type], grad.data_ptr(), loss2.data_ptr(),
-                                                   stream), "sgb_feature_map_loss")
+        _lib.check(_lib.load().sgb_feature_map_loss(C_, H * W, r.data_ptr(), y.data_ptr(), dtype, loss_code,
+                                                   grad.data_ptr(), loss2.data_ptr(), stream), "sgb_feature_map_loss")
     return loss2[0], grad
 
 
@@ -193,8 +199,6 @@ def voxel_feature_loss_and_grad(output: torch.Tensor, mask: torch.Tensor, featur
     same skip reads ``count`` (one sync) and leaves out ``optimizer.step()``: a step with a zero gradient still
     applies AdamW's weight decay.  If mask.sum() is not features_gt's row count, loss and count are NaN.  Nothing
     is synchronised; every output is bitwise reproducible.  1 <= channels <= 1024, (head + 1) * channels <= F."""
-    if loss_type not in _FEATURE_LOSSES:
-        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
     for name, t in (("output", output), ("mask", mask), ("features_gt", features_gt)):
         if not isinstance(t, torch.Tensor) or not t.is_cuda:
             raise ValueError(f"{name} must be a CUDA tensor (the voxel feature loss has no CPU path)")
@@ -205,14 +209,13 @@ def voxel_feature_loss_and_grad(output: torch.Tensor, mask: torch.Tensor, featur
     M, F = output.shape
     if mask.dtype != torch.bool or mask.shape != (M,):
         raise ValueError(f"mask must be ({M},) bool, got {tuple(mask.shape)} {mask.dtype}")
-    if features_gt.requires_grad:
-        raise ValueError("features_gt must not require grad (the loss gives the gradient of the output only)")
-    if features_gt.dtype not in (torch.float16, torch.float32) or features_gt.ndim != 2 \
-            or features_gt.shape[1] != channels:
+    loss_code, dtype = _feature_loss_codes(loss_type, features_gt, "features_gt", " of the output")
+    if features_gt.ndim != 2 or features_gt.shape[1] != channels:
         raise ValueError(f"features_gt must be (K, {channels}) float16 or float32, got {tuple(features_gt.shape)} "
                          f"{features_gt.dtype}")
-    if not 1 <= channels <= 1024 or head < 0 or (head + 1) * channels > F:
-        raise ValueError(f"head {head} of {channels} channels does not fit in {F} columns (1 <= channels <= 1024)")
+    if not 1 <= channels <= _FEATURE_MAX_C or head < 0 or (head + 1) * channels > F:
+        raise ValueError(f"head {head} of {channels} channels does not fit in {F} columns "
+                         f"(1 <= channels <= {_FEATURE_MAX_C})")
     if features_gt.shape[0] > M:
         raise ValueError(f"features_gt has {features_gt.shape[0]} rows, more than the {M} rows of output")
     x = output.detach().contiguous()
@@ -227,10 +230,9 @@ def voxel_feature_loss_and_grad(output: torch.Tensor, mask: torch.Tensor, featur
             raise _lib.SgbError("sgb_voxel_feature_loss_workspace_bytes failed")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
         stream = torch.cuda.current_stream(x.device).cuda_stream
-        dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
         _lib.check(lib.sgb_voxel_feature_loss(M, F, x.data_ptr(), m.data_ptr(), y.shape[0], channels, head,
-                                              y.data_ptr(), dtype, _FEATURE_LOSSES[loss_type], grad.data_ptr(),
-                                              ws.data_ptr(), loss2.data_ptr(), stream), "sgb_voxel_feature_loss")
+                                              y.data_ptr(), dtype, loss_code, grad.data_ptr(), ws.data_ptr(),
+                                              loss2.data_ptr(), stream), "sgb_voxel_feature_loss")
     return loss2[0], loss2[1], grad
 
 
@@ -247,15 +249,10 @@ def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Te
     ``decoder.bias.grad = g_bias``.  weight and bias are read detached (they may be nn.Parameters).  1 <= C <= 1024,
     1 <= c <= 128.  Nothing is synchronised; besides the outputs only a scratch buffer that depends on C and c alone
     is allocated, and every output is bitwise reproducible."""
-    if loss_type not in _FEATURE_LOSSES:
-        raise ValueError(f"loss_type must be one of {sorted(_FEATURE_LOSSES)}, got {loss_type!r}")
     for name, t in (("rendering", rendering), ("weight", weight), ("target", target), ("bias", bias)):
         if not isinstance(t, torch.Tensor) and not (name == "bias" and t is None):
             raise ValueError(f"{name} must be a tensor")
-    if target.requires_grad:
-        raise ValueError("target must not require grad (the loss gives the gradients of the rendering and decoder)")
-    if target.dtype not in (torch.float16, torch.float32):
-        raise ValueError(f"target must be float16 or float32, got {target.dtype}")
+    loss_code, dtype = _feature_loss_codes(loss_type, target, "target", "s of the rendering and decoder")
     if weight.dtype != torch.float32 or (bias is not None and bias.dtype != torch.float32):
         raise ValueError(f"weight and bias must be float32, got {weight.dtype} and "
                          f"{None if bias is None else bias.dtype}")
@@ -266,8 +263,9 @@ def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Te
                          f"{tuple(rendering.shape)}, {tuple(weight.shape)}, {tuple(target.shape)} and "
                          f"{None if bias is None else tuple(bias.shape)}")
     C_, c = weight.shape
-    if not (1 <= C_ <= 1024 and 1 <= c <= 128):
-        raise ValueError(f"the decoder must have 1 <= C <= 1024 outputs and 1 <= c <= 128 inputs, got ({C_}, {c})")
+    if not (1 <= C_ <= _FEATURE_MAX_C and 1 <= c <= 128):
+        raise ValueError(f"the decoder must have 1 <= C <= {_FEATURE_MAX_C} outputs and 1 <= c <= 128 inputs, got "
+                         f"({C_}, {c})")
     tensors = [rendering, weight, target] + ([bias] if bias is not None else [])
     if not rendering.is_cuda or any(t.device != rendering.device for t in tensors):
         raise ValueError(f"rendering, weight, target and bias must be CUDA tensors on one device (the decoded "
@@ -284,12 +282,11 @@ def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Te
     g_bias = torch.empty_like(b) if b is not None else None
     workspace = torch.empty(lib.sgb_decoded_feature_loss_workspace_bytes(C_, c, N), dtype=torch.uint8, device=r.device)
     loss2 = torch.empty(2, dtype=torch.float64, device=r.device)      # [loss, pixels averaged over]; zeroed by the call
-    dtype = _lib.FEAT_F16 if y.dtype == torch.float16 else _lib.FEAT_F32
     with torch.cuda.device(r.device):
         stream = torch.cuda.current_stream(r.device).cuda_stream
         _lib.check(lib.sgb_decoded_feature_loss(C_, c, N, r.data_ptr(), w.data_ptr(),
                                                 b.data_ptr() if b is not None else None, y.data_ptr(), dtype,
-                                                _FEATURE_LOSSES[loss_type], g_render.data_ptr(), g_weight.data_ptr(),
+                                                loss_code, g_render.data_ptr(), g_weight.data_ptr(),
                                                 g_bias.data_ptr() if g_bias is not None else None,
                                                 workspace.data_ptr(), loss2.data_ptr(), stream),
                    "sgb_decoded_feature_loss")

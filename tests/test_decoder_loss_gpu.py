@@ -5,6 +5,7 @@ branch on; the identity decoder against feature_map_loss_and_grad; edge cases; s
 memory at K4's view size; and a short fit of a compact field plus decoder through render_chn."""
 import pytest
 import torch
+from feature_loss_ref import feature_loss
 
 from semantic_gaussians_b200 import _lib
 from semantic_gaussians_b200.semantic import decoded_feature_map_loss_and_grads, feature_map_loss_and_grad
@@ -39,29 +40,19 @@ def _inputs(c, C, H, W, dtype, bias, seed):
 
 
 def _reference(r, w, b, y, loss_type):
-    """float64 torch autograd: (loss, dL/dr, dL/dW, dL/db, pixels averaged over, decoded x)."""
+    """float64: (loss, dL/dr, dL/dW, dL/db, pixels averaged over, decoded x), feature_loss_ref.feature_loss with one
+    row per pixel of x = W r + b, and its gradient taken back through the decoder by autograd."""
     C = w.shape[0]
+    _, H, W = r.shape
     rl = r.double().requires_grad_(True)
     wl = w.double().requires_grad_(True)
     bl = b.double().requires_grad_(True) if b is not None else None
     xi = torch.einsum("kc,chw->khw", wl, rl)
     if bl is not None:
         xi = xi + bl[:, None, None]
-    x = xi.permute(1, 2, 0).reshape(-1, C)
-    t = y.double().permute(1, 2, 0).reshape(-1, C)
-    m = t.norm(dim=-1) > 0
-    if loss_type == "cosine":
-        if int(m.sum()) == 0:
-            z = lambda v: None if v is None else torch.zeros_like(v, dtype=torch.float64)  # noqa: E731
-            return 0.0, z(r), z(w), z(b), 0, xi.detach()
-        loss = (1 - torch.nn.CosineSimilarity()(x[m], t[m])).mean()
-    elif loss_type == "l1":
-        loss = torch.nn.L1Loss()(x, t)
-    else:
-        loss = torch.nn.MSELoss()(x, t)
-    loss.backward()
-    n = int(m.sum()) if loss_type == "cosine" else x.shape[0]
-    return float(loss.detach()), rl.grad, wl.grad, bl.grad if bl is not None else None, n, xi.detach()
+    loss, n, g = feature_loss(xi.permute(1, 2, 0).reshape(-1, C), y.permute(1, 2, 0).reshape(-1, C), loss_type)
+    xi.backward(g.reshape(H, W, C).permute(2, 0, 1))
+    return loss, rl.grad, wl.grad, bl.grad if bl is not None else None, n, xi.detach()
 
 
 def _abi(r, w, b, y, loss_type):

@@ -8,6 +8,7 @@ import sys
 import numpy as np
 import pytest
 import torch
+from feature_loss_ref import feature_loss
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
@@ -100,23 +101,12 @@ def _loss_inputs(M, F, C, dtype, seed=0, p=0.6, zero_rows=True):
 
 
 def _reference(output, mask, gt, loss_type, head, C):
-    """distill.py:111-124 in float64 with autograd: (loss, count, grad)."""
-    x = output.detach().double().requires_grad_(True)
-    o = x[mask][:, head * C:(head + 1) * C]
-    y = gt.float().double()
-    if loss_type == "cosine":
-        m = y.norm(dim=-1) > 0
-        if m.sum() == 0:
-            return 0.0, 0, torch.zeros_like(x)
-        loss = (1 - torch.nn.CosineSimilarity()(o[m], y[m])).mean()
-        count = int(m.sum())
-    else:
-        if len(y) == 0:
-            return 0.0, 0, torch.zeros_like(x)
-        loss = (torch.nn.L1Loss() if loss_type == "l1" else torch.nn.MSELoss())(o, y)
-        count = len(y)
-    loss.backward()
-    return loss.item(), count, x.grad
+    """feature_loss_ref.feature_loss on the head's columns of the masked rows: (loss, count, d loss / d output)."""
+    cols = slice(head * C, (head + 1) * C)
+    loss, count, g = feature_loss(output[mask][:, cols], gt, loss_type)
+    grad = torch.zeros_like(output, dtype=torch.float64)
+    grad[mask, cols] = g
+    return loss, count, grad
 
 
 def _check(output, mask, gt, loss_type, head, C):

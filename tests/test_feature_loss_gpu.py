@@ -4,6 +4,7 @@ channel count, target dtype and image shape its kernels branch on; reproducibili
 short feature fit through render_chn."""
 import pytest
 import torch
+from feature_loss_ref import feature_loss
 
 from semantic_gaussians_b200 import _lib
 from semantic_gaussians_b200.semantic import feature_map_loss_and_grad
@@ -32,22 +33,10 @@ def _inputs(C, H, W, dtype, seed):
 
 
 def _reference(r, y, loss_type):
-    """float64 torch autograd of the reference's expressions, one row per pixel."""
-    C = r.shape[0]
-    xl = r.double().requires_grad_(True)
-    x = xl.permute(1, 2, 0).reshape(-1, C)
-    t = y.double().permute(1, 2, 0).reshape(-1, C)
-    m = t.norm(dim=-1) > 0
-    if loss_type == "cosine":
-        if int(m.sum()) == 0:
-            return 0.0, torch.zeros_like(r, dtype=torch.float64), 0
-        loss = (1 - torch.nn.CosineSimilarity()(x[m], t[m])).mean()
-    elif loss_type == "l1":
-        loss = torch.nn.L1Loss()(x, t)
-    else:
-        loss = torch.nn.MSELoss()(x, t)
-    loss.backward()
-    return float(loss.detach()), xl.grad, int(m.sum()) if loss_type == "cosine" else x.shape[0]
+    """feature_loss_ref.feature_loss with one row per pixel: (loss, d loss / d r (C,H,W), pixels averaged over)."""
+    C, H, W = r.shape
+    loss, n, g = feature_loss(r.permute(1, 2, 0).reshape(-1, C), y.permute(1, 2, 0).reshape(-1, C), loss_type)
+    return loss, g.reshape(H, W, C).permute(2, 0, 1), n
 
 
 def _abi_count(r, y, loss_type):
