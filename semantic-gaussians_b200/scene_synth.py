@@ -1,4 +1,5 @@
-"""Synthetic scenes and cameras for tests, golden fixtures and bench (numpy only).
+"""Synthetic scenes and cameras for tests, golden fixtures and bench (numpy only, except the torch voxel cloud of
+``surface_voxels``).
 
 The reference ships no generator; its distributions are the blob and room scenes below.  Camera matrices
 follow the reference's conventions exactly:
@@ -178,3 +179,28 @@ def make_scene(P: int, seed: int = 0, kind: str = "blob", sh: bool = False, chan
             feats[s:s + f.shape[0]] = f
     return SynthScene(xyz.astype(np.float32), scales.astype(np.float32), q.astype(np.float32),
                       opacity.astype(np.float32), shs, feats)
+
+
+def surface_voxels(P: int, dev, seed: int = 0):
+    """Voxel rows and features of P points on the floor (z = -1.5) and the four walls (x, y = +-4) of the 8 x 8 x 3 m
+    room, by area, with 1 cm jitter, at voxel size 0.02: closer to the occupancy of a scanned scene than the
+    volumetric `room` Gaussians.  Returns int32 rows (1, x, y, z) and 56 N(0, 1) features per voxel, on ``dev``."""
+    import torch
+
+    from .voxelize import voxel_indices
+    g = torch.Generator(device=dev).manual_seed(seed)
+    u = lambda n, lo, hi: torch.rand(n, device=dev, generator=g) * (hi - lo) + lo   # noqa: E731
+    areas = torch.tensor([64.0, 24.0, 24.0, 24.0, 24.0])
+    counts = (areas / areas.sum() * P).long().tolist()
+    parts = [torch.stack([u(counts[0], -4, 4), u(counts[0], -4, 4), torch.full((counts[0],), -1.5, device=dev)], 1)]
+    for i, (axis, val) in enumerate(((0, -4.0), (0, 4.0), (1, -4.0), (1, 4.0))):
+        n = counts[1 + i]
+        p = torch.stack([u(n, -4, 4), u(n, -4, 4), u(n, -1.5, 1.5)], 1)
+        p[:, axis] = val
+        parts.append(p)
+    xyz = torch.cat(parts) + torch.randn(sum(counts), 3, device=dev, generator=g) * 0.01
+    T = [[50.0, 0, 0, 0], [0, 50.0, 0, 0], [0, 0, 50.0, 0]]
+    _, _, vox = voxel_indices(xyz.float().contiguous(), T)
+    locs = torch.cat([torch.ones((vox.shape[0], 1), dtype=torch.int32, device=dev), vox], 1)
+    feats = torch.randn(vox.shape[0], 56, device=dev, generator=g)
+    return locs, feats

@@ -1,13 +1,37 @@
 """Float64 restatement of the sparse convolution (sparse.py) and MinkUNet (mink_unet.py) for the tests.
 
-Coordinate maps and kernel maps are built with Python dicts over coordinate tuples; the products are float64 torch
-expressions on the CPU (gather, matmul, index_add_), so autograd gives the reference gradients.  Orders are the ones
-sgb200.h documents: a strided map lists its rows in the order their first child appears, and an offset's pairs ascend
-in the output row."""
+Coordinate maps and kernel maps are built twice, neither way sharing logic with the device hash table: with Python
+dicts over coordinate tuples (Maps, for hand-checkable sizes), and with sorting torch expressions on any device
+(TensorMaps, for maps of a million rows).  The products are float64 torch expressions on the inputs' device (gather,
+matmul, index_add_), so autograd gives the reference gradients.  Orders are the ones sgb200.h documents: a strided map
+lists its rows in the order their first child appears, and an offset's pairs ascend in the output row.
+
+``random_rows`` draws the (b, x, y, z) test clouds of the GPU tests."""
 from __future__ import annotations
 
+import math
+
+import numpy as np
 import torch
 import torch.nn.functional as Fn
+
+
+def random_rows(kind, N, batches, seed=0):
+    """N distinct int32 rows (b, x, y, z) in random order, b < batches.  Kinds: "box", a cube at ~30 % occupancy;
+    "near_2_30", coordinates just below 2^30; "low_bits", coordinates that differ only in bit 0 and above bit 20."""
+    rng = np.random.default_rng(seed)
+    if kind == "box":
+        side = max(4, int(round((N / batches / 0.3) ** (1 / 3))))        # ~30 % occupancy
+        pts = rng.integers(0, side, (3 * N, 3))
+    elif kind == "near_2_30":
+        pts = (1 << 30) - 1024 + rng.integers(0, 64, (3 * N, 3)) * 32 + rng.integers(0, 3, (3 * N, 3))
+    else:   # low_bits: rows that differ only above bit 20
+        pts = (rng.integers(0, 64, (3 * N, 3)) << 20) + rng.integers(0, 2, (3 * N, 3))
+    b = rng.integers(0, batches, (3 * N, 1))
+    out = np.unique(np.concatenate([b, pts], 1), axis=0)
+    out = out[rng.permutation(len(out))[:N]]
+    assert len(out) == N
+    return out.astype(np.int32)
 
 
 def offsets(k, t):
@@ -38,19 +62,26 @@ def kernel_map(in_rows, out_rows, k, t):
 
 
 def conv(x, W, kmap, n_out, transposed=False):
-    """sum over offsets of gathered products: out[o] += x[i] W_d, or with the roles swapped for a transposed layer."""
-    out = torch.zeros((n_out, W.shape[-1]), dtype=x.dtype)
+    """sum over offsets of gathered products: out[o] += x[i] W_d, or with the roles swapped for a transposed layer.
+    ``kmap``: per offset, the (in row, out row) pairs as a list of tuples or an (n, 2) tensor; computed on x's device."""
+    out = torch.zeros((n_out, W.shape[-1]), dtype=x.dtype, device=x.device)
     for d, pairs in enumerate(kmap):
-        if not pairs:
+        if len(pairs) == 0:
             continue
-        p = torch.tensor(pairs, dtype=torch.int64)
+        p = torch.as_tensor(pairs, dtype=torch.int64, device=x.device)
         src, dst = (p[:, 1], p[:, 0]) if transposed else (p[:, 0], p[:, 1])
         out = out.index_add(0, dst, x[src] @ W[d])
     return out
 
 
+# (in stride, out stride, k) of every kernel map MinkUNet builds
+MINKUNET_KMAPS = [(1, 1, 5)] + [(t, t, 3) for t in (1, 2, 4, 8, 16)] + [(t, 2 * t, 2) for t in (1, 2, 4, 8)]
+
+
 class Maps:
     """The restatement of CoordinateManager: rows by stride and kernel maps by (in stride, out stride, k)."""
+    stride_map = staticmethod(stride_map)
+    kernel_map = staticmethod(kernel_map)
 
     def __init__(self, rows):
         self.rows = {1: [tuple(r) for r in rows]}
@@ -58,14 +89,79 @@ class Maps:
 
     def at(self, t):
         if t not in self.rows:
-            self.rows[t] = stride_map(self.at(t // 2), t // 2)
+            self.rows[t] = self.stride_map(self.at(t // 2), t // 2)
         return self.rows[t]
 
     def kmap(self, t_in, t_out, k):
         key = (t_in, t_out, k)
         if key not in self.kmaps:
-            self.kmaps[key] = kernel_map(self.at(t_in), self.at(t_out), k, t_in)
+            self.kmaps[key] = self.kernel_map(self.at(t_in), self.at(t_out), k, t_in)
         return self.kmaps[key]
+
+
+# ---------------------------------------------------------------- the same maps as torch expressions
+
+def stride_map_t(rows, t):
+    """stride_map on an (N, 4) integer tensor: the parents by floor, unique, in order of their first child's row."""
+    r = rows.long()
+    t2 = 2 * t
+    par = torch.cat([r[:, :1], torch.div(r[:, 1:], t2, rounding_mode="floor") * t2], 1)
+    uniq, inv = torch.unique(par, dim=0, return_inverse=True)
+    first = torch.full((len(uniq),), len(r), dtype=torch.int64, device=r.device)
+    first = first.scatter_reduce(0, inv, torch.arange(len(r), device=r.device), "amin")
+    return uniq[first.argsort()].to(rows.dtype)
+
+
+class RowIndex:
+    """Row lookup in a set of (b, x, y, z) rows by sorting.  Each component is replaced by its rank among the set's
+    values of that component (torch.unique, so any int32 values, such as the "low_bits" rows, work), and the four
+    ranks are packed mixed-radix into one int64 key; the set's keys are sorted and queries found by searchsorted."""
+
+    def __init__(self, rows):
+        r = rows.long()
+        self.values = [torch.unique(r[:, a]) for a in range(4)]
+        assert math.prod(len(v) for v in self.values) < 2 ** 62, "rows too varied to pack into one int64 key"
+        key, _ = self._key(r)
+        self.keys, self.order = key.sort()
+
+    def _key(self, r):
+        """(key, known): known is False where a component is not among the set's values (the key is then junk)."""
+        key = torch.zeros(len(r), dtype=torch.int64, device=r.device)
+        known = torch.ones(len(r), dtype=torch.bool, device=r.device)
+        for a, v in enumerate(self.values):
+            c = r[:, a].contiguous()
+            pos = torch.searchsorted(v, c).clamp_max(len(v) - 1)
+            known &= v[pos] == c
+            key = key * len(v) + pos
+        return key, known
+
+    def find(self, queries):
+        """Row of the set equal to each query row (int64, any values), or -1."""
+        key, known = self._key(queries)
+        pos = torch.searchsorted(self.keys, key).clamp_max(len(self.keys) - 1)
+        return torch.where(known & (self.keys[pos] == key), self.order[pos], -1)
+
+
+def kernel_map_t(in_rows, out_rows, k, t):
+    """kernel_map on tensors: per offset an (n, 2) int64 tensor of (in row, out row) pairs, ascending in the out row."""
+    index = RowIndex(in_rows)
+    out = out_rows.long()
+    maps = []
+    for off in offsets(k, t):
+        i = index.find(out + torch.tensor((0,) + off, device=out.device))
+        o = torch.nonzero(i >= 0).squeeze(1)
+        maps.append(torch.stack([i[o], o], 1))
+    return maps
+
+
+class TensorMaps(Maps):
+    """Maps over an (N, 4) integer tensor: rows by stride as tensors, kernel maps as per-offset pair tensors."""
+    stride_map = staticmethod(stride_map_t)
+    kernel_map = staticmethod(kernel_map_t)
+
+    def __init__(self, rows):
+        self.rows = {1: rows}
+        self.kmaps = {}
 
 
 def minkunet_forward(model, coords, feats, params, training):

@@ -1,7 +1,9 @@
-"""Sparse 3D convolution and MinkUNet without a GPU: the float64 restatement against hand-worked cases, the MinkUNet
-state_dict against the reference's layer structure, and argument validation before any CUDA call."""
+"""Sparse 3D convolution and MinkUNet without a GPU: the float64 restatement against hand-worked cases, its tensor maps
+against its dict maps, the MinkUNet state_dict against the reference's layer structure, and argument validation before
+any CUDA call."""
 import ctypes as C
 
+import numpy as np
 import pytest
 import torch
 
@@ -65,6 +67,31 @@ def test_rows_that_differ_only_in_b_never_pair():
             assert rows[i][0] == rows[o][0]
     assert sum(len(p) for p in km) == 4 + 2        # 4 centres, (1,3,2,2) <-> (1,2,2,2) both ways
     assert ref.stride_map(rows, 1) == [(0, 2, 2, 2), (1, 2, 2, 2)] + [(2, 2, 2, 2)]
+
+
+# ---------------------------------------------------------------- the tensor maps against the dict maps
+
+def _cloud(kind, N, batches):
+    if kind == "copies":      # one box cloud in every batch: rows that differ only in b
+        base = ref.random_rows("box", N // batches, 1, seed=N)
+        return np.concatenate([np.concatenate([np.full((len(base), 1), b, np.int32), base[:, 1:]], 1)
+                               for b in range(batches)])
+    return ref.random_rows(kind, N, batches, seed=N)
+
+
+@pytest.mark.parametrize("kind,N,batches", [("box", 1, 1), ("box", 2, 1), ("box", 2, 2), ("box", 300, 1),
+                                            ("box", 700, 3), ("box", 2000, 4), ("copies", 2, 2), ("copies", 800, 4),
+                                            ("low_bits", 500, 2), ("near_2_30", 500, 3)])
+def test_tensor_maps_equal_the_dict_maps(kind, N, batches):
+    rows = _cloud(kind, N, batches)
+    maps, tmaps = ref.Maps(rows.tolist()), ref.TensorMaps(torch.from_numpy(rows))
+    for t in (1, 2, 4, 8, 16):
+        got = tmaps.at(t)
+        assert got.dtype == torch.int32 and [tuple(r) for r in got.tolist()] == maps.at(t), t
+    for t_in, t_out, k in ref.MINKUNET_KMAPS:
+        got = tmaps.kmap(t_in, t_out, k)
+        assert len(got) == k ** 3
+        assert [[tuple(p) for p in pairs.tolist()] for pairs in got] == maps.kmap(t_in, t_out, k), (t_in, t_out, k)
 
 
 # ---------------------------------------------------------------- MinkUNet state_dict

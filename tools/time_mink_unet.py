@@ -26,8 +26,8 @@ import torch  # noqa: E402
 from semantic_gaussians_b200 import sparse as sp  # noqa: E402
 from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
 from semantic_gaussians_b200.mink_unet import mink_unet  # noqa: E402
-from semantic_gaussians_b200.scene_synth import make_scene  # noqa: E402
-from semantic_gaussians_b200.voxelize import voxel_indices, voxelize_gaussians  # noqa: E402
+from semantic_gaussians_b200.scene_synth import make_scene, surface_voxels  # noqa: E402
+from semantic_gaussians_b200.voxelize import voxelize_gaussians  # noqa: E402
 
 
 def card() -> str:
@@ -40,26 +40,6 @@ def room_input(P, dev):
     scene = make_scene(P, 0, kind="room", sh=True)
     m = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, shs=scene.shs, device=dev)
     locs, feats, _ = voxelize_gaussians(m, 0.02, "all")
-    return locs, feats
-
-
-def surface_input(P, dev, seed=0):
-    """Points on the floor (z = -1.5) and the four walls (x, y = +-4) of the 8 x 8 x 3 m room, by area."""
-    g = torch.Generator(device=dev).manual_seed(seed)
-    u = lambda n, lo, hi: torch.rand(n, device=dev, generator=g) * (hi - lo) + lo   # noqa: E731
-    areas = torch.tensor([64.0, 24.0, 24.0, 24.0, 24.0])
-    counts = (areas / areas.sum() * P).long().tolist()
-    parts = [torch.stack([u(counts[0], -4, 4), u(counts[0], -4, 4), torch.full((counts[0],), -1.5, device=dev)], 1)]
-    for i, (axis, val) in enumerate(((0, -4.0), (0, 4.0), (1, -4.0), (1, 4.0))):
-        n = counts[1 + i]
-        p = torch.stack([u(n, -4, 4), u(n, -4, 4), u(n, -1.5, 1.5)], 1)
-        p[:, axis] = val
-        parts.append(p)
-    xyz = torch.cat(parts) + torch.randn(sum(counts), 3, device=dev, generator=g) * 0.01
-    T = [[50.0, 0, 0, 0], [0, 50.0, 0, 0], [0, 0, 50.0, 0]]
-    _, _, vox = voxel_indices(xyz.float().contiguous(), T)
-    locs = torch.cat([torch.ones((vox.shape[0], 1), dtype=torch.int32, device=dev), vox], 1)
-    feats = torch.randn(vox.shape[0], 56, device=dev, generator=g)
     return locs, feats
 
 
@@ -168,7 +148,7 @@ def main():
     model = mink_unet(56, 768, arch="MinkUNet34A").to(dev)
     result = {"card": card(), "arch": "MinkUNet34A", "points": args.points, "sets": {}}
     for name in args.sets.split(","):
-        locs, feats = room_input(args.points, dev) if name == "room" else surface_input(args.points, dev)
+        locs, feats = room_input(args.points, dev) if name == "room" else surface_voxels(args.points, dev)
         M = int(locs.shape[0])
 
         def build_maps():
