@@ -259,6 +259,7 @@ int64_t sgb_state_field(const char* name, int32_t P, int64_t num_rendered, int32
 
 #define SGB_FEAT_F16 0
 #define SGB_FEAT_F32 1
+#define SGB_FEAT_BF16 2   /* the half-precision sparse convolution only; the feature losses reject it */
 
 typedef struct sgb_fusion_view {
     int32_t P;
@@ -594,6 +595,35 @@ size_t sgb_sparse_conv_backward_weight_workspace_bytes(int32_t K, const int64_t*
 int sgb_sparse_conv_backward_weight(int32_t K, const int64_t* offsets_host, const int32_t* pairs, int32_t transposed,
                                     int64_t n_in, int32_t C_in, const float* x, int64_t n_out, int32_t C_out,
                                     const float* dy, void* workspace, float* dkernel, void* stream);
+
+/* Half-precision products (sparse_conv_half.cu): the same three products over the same kernel maps (offsets_host,
+ * pairs) the fp32 products take, with the same argument rules, on tensor cores.  dtype is SGB_FEAT_F16 or
+ * SGB_FEAT_BF16; x, dy, out, dx and the kernel ((K, C_in, C_out) row-major) are in that type.
+ *   forward / input: the products of every offset are accumulated in fp32, in offset order, in the workspace
+ *     (sgb_sparse_conv_half_{forward,backward_input}_workspace_bytes(...) bytes, 16-byte aligned: one fp32 copy of
+ *     out / dx), and each element is rounded to the half type once, at the end.
+ *   weight: dkernel is fp32 (the kernel parameter it updates is fp32), accumulated in fp32 in the fp32 product's
+ *     chunk partials and summed in chunk order; workspace sgb_sparse_conv_half_backward_weight_workspace_bytes(...).
+ * Half x half products are exact in fp32: only the fp32 accumulation (and, for out / dx, the one final rounding)
+ * rounds.  Any C_in, C_out >= 1; rows whose width is a multiple of 8 elements take the fast path.  No float atomics:
+ * the same inputs give bitwise identical outputs.  Validation, asynchrony and the workspace-size rule are those of
+ * the fp32 products. */
+size_t sgb_sparse_conv_half_forward_workspace_bytes(int32_t dtype, int32_t K, const int64_t* offsets_host,
+                                                    int64_t n_in, int32_t C_in, int64_t n_out, int32_t C_out);
+int sgb_sparse_conv_half_forward(int32_t dtype, int32_t K, const int64_t* offsets_host, const int32_t* pairs,
+                                 int32_t transposed, int64_t n_in, int32_t C_in, const void* x, const void* kernel,
+                                 int64_t n_out, int32_t C_out, void* workspace, void* out, void* stream);
+size_t sgb_sparse_conv_half_backward_input_workspace_bytes(int32_t dtype, int32_t K, const int64_t* offsets_host,
+                                                           int64_t n_in, int32_t C_in, int64_t n_out, int32_t C_out);
+int sgb_sparse_conv_half_backward_input(int32_t dtype, int32_t K, const int64_t* offsets_host, const int32_t* pairs,
+                                        int32_t transposed, int64_t n_in, int32_t C_in, void* dx, const void* kernel,
+                                        int64_t n_out, int32_t C_out, const void* dy, void* workspace, void* stream);
+size_t sgb_sparse_conv_half_backward_weight_workspace_bytes(int32_t dtype, int32_t K, const int64_t* offsets_host,
+                                                            int32_t C_in, int32_t C_out);
+int sgb_sparse_conv_half_backward_weight(int32_t dtype, int32_t K, const int64_t* offsets_host, const int32_t* pairs,
+                                         int32_t transposed, int64_t n_in, int32_t C_in, const void* x, int64_t n_out,
+                                         int32_t C_out, const void* dy, void* workspace, float* dkernel,
+                                         void* stream);
 
 #ifdef __cplusplus
 }

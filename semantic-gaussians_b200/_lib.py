@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libsgb200.so")
 
 SGB_OK = 0
 DEPTH_NONE, DEPTH_F32, DEPTH_F64, DEPTH_SURFACE = 0, 1, 2, 3
-FEAT_F16, FEAT_F32 = 0, 1
+FEAT_F16, FEAT_F32, FEAT_BF16 = 0, 1, 2
 FEATLOSS_COSINE, FEATLOSS_L1, FEATLOSS_L2 = 0, 1, 2
 
 
@@ -84,7 +84,10 @@ EXPORTS = (
     "sgb_coord_stride", "sgb_kernel_map_workspace_bytes", "sgb_kernel_map_count", "sgb_kernel_map_fill",
     "sgb_sparse_conv_forward", "sgb_sparse_conv_backward_input", "sgb_sparse_conv_backward_weight_workspace_bytes",
     "sgb_sparse_conv_backward_weight", "sgb_voxelize_f64", "sgb_elastic_displace", "sgb_voxel_feature_loss",
-    "sgb_voxel_feature_loss_workspace_bytes",
+    "sgb_voxel_feature_loss_workspace_bytes", "sgb_sparse_conv_half_forward_workspace_bytes",
+    "sgb_sparse_conv_half_forward", "sgb_sparse_conv_half_backward_input_workspace_bytes",
+    "sgb_sparse_conv_half_backward_input", "sgb_sparse_conv_half_backward_weight_workspace_bytes",
+    "sgb_sparse_conv_half_backward_weight",
 )
 
 _lib = None
@@ -186,6 +189,17 @@ def load() -> C.CDLL:
         lib.sgb_sparse_conv_backward_weight_workspace_bytes.argtypes = [i32, pi64, i32, i32]
         lib.sgb_sparse_conv_backward_weight_workspace_bytes.restype = C.c_size_t
         lib.sgb_sparse_conv_backward_weight.argtypes = [i32, pi64, vp, i32, i64, i32, vp, i64, i32, vp, vp, vp, vp]
+        for name in ("sgb_sparse_conv_half_forward_workspace_bytes",
+                     "sgb_sparse_conv_half_backward_input_workspace_bytes"):
+            getattr(lib, name).argtypes = [i32, i32, pi64, i64, i32, i64, i32]
+            getattr(lib, name).restype = C.c_size_t
+        lib.sgb_sparse_conv_half_forward.argtypes = [i32, i32, pi64, vp, i32, i64, i32, vp, vp, i64, i32, vp, vp, vp]
+        lib.sgb_sparse_conv_half_backward_input.argtypes = [i32, i32, pi64, vp, i32, i64, i32, vp, vp, i64, i32, vp, vp,
+                                                            vp]
+        lib.sgb_sparse_conv_half_backward_weight_workspace_bytes.argtypes = [i32, i32, pi64, i32, i32]
+        lib.sgb_sparse_conv_half_backward_weight_workspace_bytes.restype = C.c_size_t
+        lib.sgb_sparse_conv_half_backward_weight.argtypes = [i32, i32, pi64, vp, i32, i64, i32, vp, i64, i32, vp, vp,
+                                                             vp, vp]
         _lib = lib
         return lib
 

@@ -18,19 +18,14 @@
 //
 // Tiles: 64 rows x 64 columns per CTA of 256 threads, each thread a 4 x 4 FFMA register tile over 16-deep shared
 // operands.
-#include "common.cuh"
+#include "sparse_conv.cuh"
 
 namespace sgb {
 
 namespace {
 
 constexpr int kBM = 64, kBN = 64, kBK = 16, kConvThreads = 256;
-constexpr long long kChunk = 2048;     // pairs per weight-gradient partial
 constexpr int kInner = 128;            // pairs per inner accumulation block of the weight gradient
-
-struct ConvOffsets {
-    long long at[SGB_SPARSE_MAX_K + 1];
-};
 
 // Y[dst(p)] += X[src(p)] B for the n pairs at `pairs`, where B(k, n) = trans ? W[n * Kd + k] : W[k * Nd + n].
 // Kd: columns of X (reduction depth), Nd: columns of Y.
@@ -89,21 +84,6 @@ __global__ void __launch_bounds__(kConvThreads) sparse_gather_gemm_kernel(const 
             if (c < Nd) y[c] += acc[i][j];
         }
     }
-}
-
-// Which (offset, first pair, end) chunk c is.  K <= SGB_SPARSE_MAX_K; one short loop per CTA.
-__device__ __forceinline__ int chunk_of(const ConvOffsets& off, int K, long long c, long long& p0, long long& p1) {
-    for (int d = 0; d < K; d++) {
-        const long long n = off.at[d + 1] - off.at[d];
-        const long long nc = (n + kChunk - 1) / kChunk;
-        if (c < nc) {
-            p0 = off.at[d] + c * kChunk;
-            p1 = min(p0 + kChunk, off.at[d + 1]);
-            return d;
-        }
-        c -= nc;
-    }
-    return -1;
 }
 
 // partial[c] (Ci x Co) = sum over chunk c's pairs of X[xs]^T DY[ys], one 64 x 64 tile per CTA (grid.y, grid.z).
@@ -180,41 +160,6 @@ __global__ void sparse_wgrad_reduce_kernel(ConvOffsets off, int K, long long CC,
     dW[(long long)d * CC + e] = s;
 }
 
-long long total_chunks(const ConvOffsets& off, int K) {
-    long long n = 0;
-    for (int d = 0; d < K; d++) n += (off.at[d + 1] - off.at[d] + kChunk - 1) / kChunk;
-    return n;
-}
-
-// Validates K, the channel counts and the offsets, and copies the offsets.
-int check_offsets(const char* fn, int32_t K, const int64_t* offsets_host, int32_t C_in, int32_t C_out,
-                  ConvOffsets& off) {
-    if (K < 1 || K > SGB_SPARSE_MAX_K) { set_error("%s: K = %d (need 1 <= K <= %d)", fn, K, SGB_SPARSE_MAX_K); return SGB_E_INVALID; }
-    if (C_in <= 0 || C_out <= 0) { set_error("%s: C_in = %d, C_out = %d (need > 0)", fn, C_in, C_out); return SGB_E_INVALID; }
-    if (!offsets_host) { set_error("%s: null offsets", fn); return SGB_E_INVALID; }
-    if (offsets_host[0] != 0) { set_error("%s: offsets[0] = %lld (need 0)", fn, (long long)offsets_host[0]); return SGB_E_INVALID; }
-    for (int d = 0; d <= K; d++) {
-        if (d > 0 && offsets_host[d] < offsets_host[d - 1]) { set_error("%s: offsets decrease at %d", fn, d); return SGB_E_INVALID; }
-        off.at[d] = offsets_host[d];
-    }
-    return SGB_OK;
-}
-
-// check_offsets, the row counts, and the pairs (which may be null only when there are none).
-int check_conv_args(const char* fn, int32_t K, const int64_t* offsets_host, const int32_t* pairs, int64_t n_in,
-                    int32_t C_in, int64_t n_out, int32_t C_out, ConvOffsets& off) {
-    if (int rc = check_offsets(fn, K, offsets_host, C_in, C_out, off)) return rc;
-    if (n_in < 0 || n_out < 0 || n_in > INT32_MAX || n_out > INT32_MAX) {
-        set_error("%s: row counts %lld, %lld out of range", fn, (long long)n_in, (long long)n_out);
-        return SGB_E_INVALID;
-    }
-    if (off.at[K] > 0 && (!pairs || reinterpret_cast<uintptr_t>(pairs) % 8)) {
-        set_error("%s: null or unaligned pairs", fn);
-        return SGB_E_INVALID;
-    }
-    return SGB_OK;
-}
-
 // Y (rows x Nd, zeroed here) = sum over offsets of the gathered products, offset by offset.
 int run_gather_gemm(const char* fn, const ConvOffsets& off, int K, const int32_t* pairs, int src_side, bool trans,
                     const float* X, int Kd, const float* W, int Nd, float* Y, long long rows, cudaStream_t s) {
@@ -235,6 +180,47 @@ int run_gather_gemm(const char* fn, const ConvOffsets& off, int K, const int32_t
 }
 
 }  // namespace
+
+long long total_chunks(const ConvOffsets& off, int K) {
+    long long n = 0;
+    for (int d = 0; d < K; d++) n += (off.at[d + 1] - off.at[d] + kChunk - 1) / kChunk;
+    return n;
+}
+
+int check_offsets(const char* fn, int32_t K, const int64_t* offsets_host, int32_t C_in, int32_t C_out,
+                  ConvOffsets& off) {
+    if (K < 1 || K > SGB_SPARSE_MAX_K) { set_error("%s: K = %d (need 1 <= K <= %d)", fn, K, SGB_SPARSE_MAX_K); return SGB_E_INVALID; }
+    if (C_in <= 0 || C_out <= 0) { set_error("%s: C_in = %d, C_out = %d (need > 0)", fn, C_in, C_out); return SGB_E_INVALID; }
+    if (!offsets_host) { set_error("%s: null offsets", fn); return SGB_E_INVALID; }
+    if (offsets_host[0] != 0) { set_error("%s: offsets[0] = %lld (need 0)", fn, (long long)offsets_host[0]); return SGB_E_INVALID; }
+    for (int d = 0; d <= K; d++) {
+        if (d > 0 && offsets_host[d] < offsets_host[d - 1]) { set_error("%s: offsets decrease at %d", fn, d); return SGB_E_INVALID; }
+        off.at[d] = offsets_host[d];
+    }
+    return SGB_OK;
+}
+
+int check_conv_args(const char* fn, int32_t K, const int64_t* offsets_host, const int32_t* pairs, int64_t n_in,
+                    int32_t C_in, int64_t n_out, int32_t C_out, ConvOffsets& off) {
+    if (int rc = check_offsets(fn, K, offsets_host, C_in, C_out, off)) return rc;
+    if (n_in < 0 || n_out < 0 || n_in > INT32_MAX || n_out > INT32_MAX) {
+        set_error("%s: row counts %lld, %lld out of range", fn, (long long)n_in, (long long)n_out);
+        return SGB_E_INVALID;
+    }
+    if (off.at[K] > 0 && (!pairs || reinterpret_cast<uintptr_t>(pairs) % 8)) {
+        set_error("%s: null or unaligned pairs", fn);
+        return SGB_E_INVALID;
+    }
+    return SGB_OK;
+}
+
+int launch_wgrad_reduce(const ConvOffsets& off, int K, long long CC, const float* partial, float* dW,
+                        cudaStream_t s) {
+    const dim3 grid((unsigned)((CC + 255) / 256), (unsigned)K);
+    sparse_wgrad_reduce_kernel<<<grid, 256, 0, s>>>(off, K, CC, partial, dW);
+    SGB_LAUNCH_CHECK("sparse_wgrad_reduce_kernel", 0, s);
+    return SGB_OK;
+}
 
 }  // namespace sgb
 
@@ -294,11 +280,7 @@ int sgb_sparse_conv_backward_weight(int32_t K, const int64_t* offsets_host, cons
                                                                   transposed ? 1 : 0, x, C_in, dy, C_out, partial);
         SGB_LAUNCH_CHECK("sparse_wgrad_partial_kernel", 0, s);
     }
-    const long long CC = (long long)C_in * C_out;
-    const dim3 grid((unsigned)((CC + 255) / 256), (unsigned)K);
-    sparse_wgrad_reduce_kernel<<<grid, 256, 0, s>>>(off, K, CC, partial, dkernel);
-    SGB_LAUNCH_CHECK("sparse_wgrad_reduce_kernel", 0, s);
-    return SGB_OK;
+    return launch_wgrad_reduce(off, K, (long long)C_in * C_out, partial, dkernel, s);
 }
 
 }  // extern "C"

@@ -12,7 +12,12 @@ one for the input map (its duplicate / negative counts), one per strided map (it
 Layers: ``Convolution`` (``kernel`` shaped ``(K, in, out)``, or ``(in, out)`` for kernel size 1, no bias),
 ``ConvolutionTranspose``, ``BatchNorm`` (``.bn`` is a ``torch.nn.BatchNorm1d``), ``ReLU`` and ``cat``.  Supported:
 kernel size 3 or 5 at stride 1, kernel size 1 at stride 1 (a dense ``torch.mm``), kernel size 2 at stride 2, forward
-and transposed; anything else, dilation != 1 and D != 3 raise ``NotImplementedError``.  CUDA fp32 only.
+and transposed; anything else, dilation != 1 and D != 3 raise ``NotImplementedError``.
+
+Features are CUDA float32, float16 or bfloat16.  Under ``torch.autocast("cuda")`` a layer runs its product in the
+autocast dtype; outside it, the features' own dtype decides.  fp16 / bf16 products run on tensor cores: each output
+element is accumulated in fp32 over every offset and rounded once, and the kernel parameter stays fp32 (it is rounded
+to the half type once per forward, and its gradient is accumulated and returned in fp32).
 
 Offsets (sgb200.h): index d = jx + k jy + k^2 jz, offset lb + j t per axis with lb = -((k-1)//2) t for odd k and 0
 for k = 2.  This is how we read ME's hyper-cube region; it has not been compared with ME itself."""
@@ -33,10 +38,21 @@ def _stream(dev):
     return torch.cuda.current_stream(dev).cuda_stream
 
 
+_HALF = {torch.float16: _lib.FEAT_F16, torch.bfloat16: _lib.FEAT_BF16}
+
+
 def _check_features(F, what="features"):
-    if not isinstance(F, torch.Tensor) or not F.is_cuda or F.dtype != torch.float32 or F.dim() != 2:
+    if not isinstance(F, torch.Tensor) or not F.is_cuda or F.dtype not in (torch.float32, *_HALF) or F.dim() != 2:
         desc = f"{tuple(F.shape)} {F.dtype} on {F.device}" if isinstance(F, torch.Tensor) else type(F).__name__
-        raise ValueError(f"{what} must be a 2-D float32 CUDA tensor, got {desc}")
+        raise ValueError(f"{what} must be a 2-D float32 CUDA tensor (or float16 / bfloat16), got {desc}")
+
+
+def _product_dtype(F):
+    """The dtype a layer computes in: the autocast dtype under torch.autocast("cuda"), else the features' own."""
+    if torch.is_autocast_enabled("cuda"):
+        dt = torch.get_autocast_dtype("cuda")
+        return dt if dt in _HALF else torch.float32
+    return F.dtype
 
 
 class CoordinateMap:
@@ -201,6 +217,59 @@ class _SparseConvFunction(torch.autograd.Function):
         return dx, dW, None, None, None
 
 
+class _HalfSparseConvFunction(torch.autograd.Function):
+    """The product on fp16 / bf16 features x with the fp32 kernel parameter: the kernel is rounded to x's dtype once
+    here, that copy is saved for the input gradient, and the kernel gradient is the fp32 one of the native call."""
+
+    @staticmethod
+    def forward(ctx, x, kernel, kmap, transposed, n_out):
+        lib = _lib.load()
+        dtype = _HALF[x.dtype]
+        x, wh = x.contiguous(), kernel.detach().to(x.dtype).contiguous()
+        K, Ci, Co = wh.shape
+        out = torch.empty((n_out, Co), dtype=x.dtype, device=x.device)
+        nbytes = lib.sgb_sparse_conv_half_forward_workspace_bytes(dtype, K, kmap.offsets_host, x.shape[0], Ci, n_out,
+                                                                  Co)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+        _lib.check(lib.sgb_sparse_conv_half_forward(dtype, K, kmap.offsets_host, kmap.pairs.data_ptr(), int(transposed),
+                                                    x.shape[0], Ci, x.data_ptr(), wh.data_ptr(), n_out, Co,
+                                                    ws.data_ptr(), out.data_ptr(), _stream(x.device)),
+                   "sgb_sparse_conv_half_forward")
+        ctx.save_for_backward(x, wh)
+        ctx.kmap, ctx.transposed = kmap, int(transposed)
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        lib = _lib.load()
+        x, wh = ctx.saved_tensors
+        km, dy = ctx.kmap, dy.to(x.dtype).contiguous()
+        dtype = _HALF[x.dtype]
+        K, Ci, Co = wh.shape
+        s = _stream(x.device)
+        dx = dW = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            nbytes = lib.sgb_sparse_conv_half_backward_input_workspace_bytes(dtype, K, km.offsets_host, x.shape[0], Ci,
+                                                                             dy.shape[0], Co)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+            _lib.check(lib.sgb_sparse_conv_half_backward_input(dtype, K, km.offsets_host, km.pairs.data_ptr(),
+                                                               ctx.transposed, x.shape[0], Ci, dx.data_ptr(),
+                                                               wh.data_ptr(), dy.shape[0], Co, dy.data_ptr(),
+                                                               ws.data_ptr(), s),
+                       "sgb_sparse_conv_half_backward_input")
+        if ctx.needs_input_grad[1]:
+            dW = torch.empty(wh.shape, dtype=torch.float32, device=x.device)
+            nbytes = lib.sgb_sparse_conv_half_backward_weight_workspace_bytes(dtype, K, km.offsets_host, Ci, Co)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+            _lib.check(lib.sgb_sparse_conv_half_backward_weight(dtype, K, km.offsets_host, km.pairs.data_ptr(),
+                                                                ctx.transposed, x.shape[0], Ci, x.data_ptr(),
+                                                                dy.shape[0], Co, dy.data_ptr(), ws.data_ptr(),
+                                                                dW.data_ptr(), s),
+                       "sgb_sparse_conv_half_backward_weight")
+        return dx, dW, None, None, None
+
+
 def _check_layer(kernel_size, stride, dilation, dimension, transposed):
     if dimension != 3:
         raise NotImplementedError(f"dimension {dimension}: only D = 3 is supported")
@@ -236,7 +305,11 @@ class _ConvBase(nn.Module):
         if x.F.shape[1] != self.in_channels:
             raise ValueError(f"input has {x.F.shape[1]} channels, the layer {self.in_channels}")
         n_out = x.coordinate_manager.map(out_stride).n
-        F = _SparseConvFunction.apply(x.F, self.kernel, kmap, transposed, n_out)
+        dt = _product_dtype(x.F)
+        if dt == torch.float32:
+            F = _SparseConvFunction.apply(x.F.float(), self.kernel, kmap, transposed, n_out)
+        else:
+            F = _HalfSparseConvFunction.apply(x.F.to(dt), self.kernel, kmap, transposed, n_out)
         return SparseTensor(F, tensor_stride=out_stride, coordinate_manager=x.coordinate_manager)
 
 
@@ -250,7 +323,8 @@ class Convolution(_ConvBase):
         t = x._stride
         if self.kernel_size == 1:
             _check_features(x.F, "input features")
-            return x._with(torch.mm(x.F, self.kernel))
+            dt = _product_dtype(x.F)
+            return x._with(torch.mm(x.F.to(dt), self.kernel.to(dt)))
         km = x.coordinate_manager.kernel_map(t, t * self.stride, self.kernel_size)
         return self._product(x, km, False, t * self.stride)
 

@@ -10,8 +10,14 @@ and forward + backward in train mode, timed with CUDA events around work that en
 The baseline replaces the native products by torch over the same pair lists (gather, mm, index_add_ per offset);
 native and baseline alternate --rounds times.  A separate torch.profiler pass gives the forward kernel time of each
 layer; mean pairs per output row and the FP32 rate (2 * pairs * C_in * C_out per product) come from the pair
-counts.  Prints the card name, power limit and max SM clock, then one JSON line."""
+counts.  Prints the card name, power limit and max SM clock, then one JSON line.
+
+--dtype fp32,bf16,fp16 times each listed dtype, alternating them within every round: fp32 runs as before, bf16 / fp16
+run the same fp32 model under torch.autocast("cuda", dtype) (the half-precision products).  Each dtype reports
+forward, forward + backward, the peak memory allocated during forward + backward, and its own per-layer profile.  The
+torch baseline runs for fp32 only (--no-baseline skips it)."""
 import argparse
+import contextlib
 import json
 import os
 import subprocess
@@ -54,6 +60,14 @@ def torch_conv(x, kernel, km, transposed, n_out):
         src, dst = (p[a:b, 1], p[a:b, 0]) if transposed else (p[a:b, 0], p[a:b, 1])
         out = out.index_add(0, dst, x[src] @ kernel[d])
     return out
+
+
+AMP = {"fp32": None, "bf16": torch.bfloat16, "fp16": torch.float16}
+
+
+def amp(dt):
+    """The autocast context of one timed dtype (none for fp32)."""
+    return torch.autocast("cuda", dtype=AMP[dt]) if AMP[dt] else contextlib.nullcontext()
 
 
 def timed(fn, reps):
@@ -135,9 +149,14 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--sets", default="room,surface")
+    ap.add_argument("--dtype", default="fp32", help="comma-separated fp32, bf16, fp16: alternated in every round")
+    ap.add_argument("--no-baseline", action="store_true", help="skip the torch baseline arm")
     ap.add_argument("--out", default=None, help="directory for the profiler traces and the JSON (default: a new "
                                                 "temporary directory)")
     args = ap.parse_args()
+    dtypes = args.dtype.split(",")
+    if not dtypes or set(dtypes) - set(AMP):
+        raise SystemExit(f"--dtype: comma-separated values of {sorted(AMP)}")
     if not torch.cuda.is_available():
         raise SystemExit("time_mink_unet.py needs a CUDA device")
     dev = torch.device("cuda:0")
@@ -146,7 +165,7 @@ def main():
     print(card(), flush=True)
     torch.manual_seed(0)
     model = mink_unet(56, 768, arch="MinkUNet34A").to(dev)
-    result = {"card": card(), "arch": "MinkUNet34A", "points": args.points, "sets": {}}
+    result = {"card": card(), "arch": "MinkUNet34A", "points": args.points, "dtypes": dtypes, "sets": {}}
     for name in args.sets.split(","):
         locs, feats = room_input(args.points, dev) if name == "room" else surface_voxels(args.points, dev)
         M = int(locs.shape[0])
@@ -176,41 +195,53 @@ def main():
             model(x).F.sum().backward()
 
         native = sp._SparseConvFunction.apply
-        arms = {"native": {}, "torch": {}}
-        fwd(), fwd_bwd()
+        arms = {f"native_{dt}": {} for dt in dtypes}
+        if "fp32" in dtypes and not args.no_baseline:
+            arms["torch_fp32"] = {}
+        for dt in dtypes:
+            with amp(dt):
+                fwd(), fwd_bwd()
         for _ in range(args.rounds):
-            for arm in ("native", "torch"):
-                sp._SparseConvFunction.apply = native if arm == "native" else torch_conv
+            for arm in arms:
+                dt = arm.split("_")[1]
+                sp._SparseConvFunction.apply = native if arm.startswith("native") else torch_conv
                 try:
-                    fwd(), fwd_bwd()
-                    arms[arm].setdefault("forward_ms", []).append(round(timed(fwd, args.reps), 3))
-                    arms[arm].setdefault("forward_backward_ms", []).append(round(timed(fwd_bwd, args.reps), 3))
+                    with amp(dt):
+                        fwd(), fwd_bwd()
+                        arms[arm].setdefault("forward_ms", []).append(round(timed(fwd, args.reps), 3))
+                        torch.cuda.reset_peak_memory_stats(dev)
+                        arms[arm].setdefault("forward_backward_ms", []).append(round(timed(fwd_bwd, args.reps), 3))
+                        arms[arm]["peak_allocated_gib"] = round(torch.cuda.max_memory_allocated(dev) / 2 ** 30, 3)
                 except torch.OutOfMemoryError:       # the baseline's autograd keeps every per-offset gather
                     arms[arm]["error"] = f"out of memory at {M} voxels"
                     model.zero_grad(set_to_none=True)
                     torch.cuda.empty_cache()
                 finally:
                     sp._SparseConvFunction.apply = native
-        t_e2e = timed(lambda: model(sp.SparseTensor(feats, locs)), args.reps)   # maps + forward, train mode
+        t_e2e = timed(lambda: model(sp.SparseTensor(feats, locs)), args.reps)   # maps + forward, train mode, fp32
         layers = layer_stats(model, x)
-        per_layer, per_kernel = profile_layers(model, x, args.out, name)
-        flops = 0
-        for r in layers:
-            f = 2 * r["pairs"] * r["cin"] * r["cout"]
-            flops += f
-            ms = per_layer.get(r["layer"])
-            r["fwd_kernel_ms"] = None if ms is None else round(ms, 4)
-            r["fwd_tflops"] = None if not ms else round(f / ms / 1e9, 2)
-        best = min(arms["native"]["forward_ms"])
+        flops = sum(2 * r["pairs"] * r["cin"] * r["cout"] for r in layers)
+        profiles = {}
+        for dt in dtypes:
+            with amp(dt):
+                per_layer, per_kernel = profile_layers(model, x, args.out, f"{name}_{dt}")
+            rows = []
+            for r in layers:
+                f = 2 * r["pairs"] * r["cin"] * r["cout"]
+                ms = per_layer.get(r["layer"])
+                rows.append(dict(r, fwd_kernel_ms=None if ms is None else round(ms, 4),
+                                 fwd_tflops=None if not ms else round(f / ms / 1e9, 2)))
+            best = min(arms[f"native_{dt}"]["forward_ms"])
+            profiles[dt] = dict(forward_tflops_best=round(flops / best / 1e9, 2), layers=rows,
+                                kernels_by_name=dict(sorted(per_kernel.items(), key=lambda kv: -kv[1])[:20]))
         result["sets"][name] = dict(
             voxels=M, map_build_ms=round(t_maps, 3), maps_plus_forward_ms=round(t_e2e, 3), arms=arms,
-            forward_flop=flops, forward_tflops_best=round(flops / best / 1e9, 2), layers=layers,
-            kernels_by_name=dict(sorted(per_kernel.items(), key=lambda kv: -kv[1])[:20]))
-        print(json.dumps({name: {k: v for k, v in result["sets"][name].items() if k not in ("layers",
-                                                                                          "kernels_by_name")}}),
-              flush=True)
-        for r in layers:
-            print(r, flush=True)
+            forward_flop=flops, profiles=profiles)
+        print(json.dumps({name: {k: v for k, v in result["sets"][name].items() if k != "profiles"}}), flush=True)
+        for dt in dtypes:
+            print(f"{name} {dt}: forward {profiles[dt]['forward_tflops_best']} TFLOP/s (best)", flush=True)
+            for r in profiles[dt]["layers"]:
+                print(r, flush=True)
     with open(os.path.join(args.out, "time_mink_unet.json"), "w") as f:
         json.dump(result, f, indent=1)
     print(json.dumps({k: v for k, v in result.items() if k != "sets"}), "->", args.out)
