@@ -259,7 +259,8 @@ int64_t sgb_state_field(const char* name, int32_t P, int64_t num_rendered, int32
 
 #define SGB_FEAT_F16 0
 #define SGB_FEAT_F32 1
-#define SGB_FEAT_BF16 2   /* the half-precision sparse convolution only; the feature losses reject it */
+#define SGB_FEAT_BF16 2   /* the half-precision sparse convolution, and the output of the split voxel feature loss;
+                             no feature loss accepts it as a target */
 
 typedef struct sgb_fusion_view {
     int32_t P;
@@ -390,6 +391,32 @@ int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint
                            int32_t C, int32_t head, const void* target,
                            int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */, int32_t loss_type, float* grad,
                            void* workspace, double* loss /* [2] device: loss, count */, void* stream);
+/* The same loss split into a forward and a gradient pass, for an output in its own dtype (output_dtype
+ * SGB_FEAT_F32, SGB_FEAT_F16 or SGB_FEAT_BF16, e.g. MinkUNet's .F under autocast); targets stay SGB_FEAT_F16 /
+ * SGB_FEAT_F32.  Half values widen to fp32 exactly, and both passes run sgb_voxel_feature_loss's per-row sums in its
+ * order on those fp32 values.
+ *   _forward writes loss[2] exactly as sgb_voxel_feature_loss does on output widened to fp32 (the NaN and 0 / 0 cases
+ *     included) and no gradient.  It leaves the mask's row flags and ranks and the cosine count in the workspace
+ *     (sgb_voxel_feature_loss_workspace_bytes(M) bytes, 16-byte aligned).
+ *   _backward reads that workspace, which must hold a _forward pass on the same M, mask and target, and overwrites grad
+ *     (M, F) in output_dtype with grad = round(float(*dloss) * g): g the fp32 gradient sgb_voxel_feature_loss writes
+ *     for that element (0 outside the masked rows and the head's columns), *dloss the upstream gradient of the loss
+ *     (device, one double, e.g. a GradScaler scale).  The scale multiplies the finished g, so for a power-of-two scale
+ *     grad is exactly g scaled and rounded once to the output type; for fp32 output and *dloss = 1 it is g bitwise.
+ *     Cosine rows recompute x.y, |x|^2 and |y|^2 from output and target; nothing per row is stored between the passes.
+ * Argument rules are sgb_voxel_feature_loss's; an unknown output_dtype, a null dloss and an output or grad not aligned
+ * to its element size also return SGB_E_INVALID before anything is enqueued.  No float atomics, no host copy, no
+ * synchronisation; M == 0 only zeroes loss (_forward) or does nothing (_backward). */
+int sgb_voxel_feature_loss_forward(int64_t M, int32_t F, const void* output,
+                                   int32_t output_dtype /* SGB_FEAT_F32 | SGB_FEAT_F16 | SGB_FEAT_BF16 */,
+                                   const uint8_t* mask /* (M) bool */, int64_t K, int32_t C, int32_t head,
+                                   const void* target, int32_t target_dtype /* SGB_FEAT_F16 | SGB_FEAT_F32 */,
+                                   int32_t loss_type, void* workspace, double* loss /* [2] device: loss, count */,
+                                   void* stream);
+int sgb_voxel_feature_loss_backward(int64_t M, int32_t F, const void* output, int32_t output_dtype, int64_t K,
+                                    int32_t C, int32_t head, const void* target, int32_t target_dtype,
+                                    int32_t loss_type, const void* workspace, const double* dloss /* device, 1 */,
+                                    void* grad /* (M, F) in output_dtype */, void* stream);
 int sgb_semantic_head(sgb_ctx* ctx, int32_t C, int32_t K, int64_t N, const float* render, const float* text,
                       int32_t first_class, float* sim, int64_t* label, void* stream);
 int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const float* features, const float* text,

@@ -87,7 +87,7 @@ EXPORTS = (
     "sgb_voxel_feature_loss_workspace_bytes", "sgb_sparse_conv_half_forward_workspace_bytes",
     "sgb_sparse_conv_half_forward", "sgb_sparse_conv_half_backward_input_workspace_bytes",
     "sgb_sparse_conv_half_backward_input", "sgb_sparse_conv_half_backward_weight_workspace_bytes",
-    "sgb_sparse_conv_half_backward_weight",
+    "sgb_sparse_conv_half_backward_weight", "sgb_voxel_feature_loss_forward", "sgb_voxel_feature_loss_backward",
 )
 
 _lib = None
@@ -172,6 +172,8 @@ def load() -> C.CDLL:
         lib.sgb_voxel_feature_loss_workspace_bytes.argtypes = [i64]
         lib.sgb_voxel_feature_loss_workspace_bytes.restype = C.c_size_t
         lib.sgb_voxel_feature_loss.argtypes = [i64, i32, vp, vp, i64, i32, i32, vp, i32, i32, vp, vp, vp, vp]
+        lib.sgb_voxel_feature_loss_forward.argtypes = [i64, i32, vp, i32, vp, i64, i32, i32, vp, i32, i32, vp, vp, vp]
+        lib.sgb_voxel_feature_loss_backward.argtypes = [i64, i32, vp, i32, i64, i32, i32, vp, i32, i32, vp, vp, vp, vp]
         lib.sgb_voxelize_workspace_bytes.restype = C.c_size_t
         lib.sgb_adam_step.argtypes = [C.POINTER(AdamTensor), i32, vp]
         pi64 = C.POINTER(i64)

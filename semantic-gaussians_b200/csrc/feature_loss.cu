@@ -332,32 +332,50 @@ __global__ void __launch_bounds__(kVlThreads) vl_count_kernel(long long K, int C
     }
 }
 
-template <typename T, int LOSS>
-__global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F, const float* __restrict__ x,
+// What one vl_loss_kernel launch writes.  kVlFused: the per-CTA loss partials and the fp32 gradient
+// (sgb_voxel_feature_loss).  kVlForward: the partials only.  kVlBackward: only the gradient, each element
+// from_f32(*dloss * g) with g the fp32 value kVlFused writes; the scale multiplies the finished g, so a power-of-two
+// scale gives exactly the rounded, scaled kVlFused gradient.
+enum VlPass { kVlFused, kVlForward, kVlBackward };
+
+// TX: the output's element type (float, __half or __nv_bfloat16), which is also the gradient's.  Half values widen
+// to fp32 exactly, so every pass sees the fp32 values of x and runs the same per-lane sums and butterflies.
+template <typename TX, typename T, int LOSS, int PASS>
+__global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F, const TX* __restrict__ x,
                                                              long long K, int C, int h0, const T* __restrict__ y,
                                                              const int* __restrict__ flags,
                                                              const int* __restrict__ rank,
                                                              const unsigned long long* __restrict__ nv_count,
-                                                             float* __restrict__ grad, double* __restrict__ partial) {
+                                                             const double* __restrict__ dloss,
+                                                             TX* __restrict__ grad, double* __restrict__ partial) {
     __shared__ double wsum[kVlRows];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long i = (long long)blockIdx.x * kVlRows + warp;
     double term = 0.0;
     if (i < M) {
-        const float* xr = x + i * F;
-        float* gr = grad + i * F;
-        for (int c = lane; c < h0; c += 32) gr[c] = 0.f;
-        for (int c = h0 + C + lane; c < F; c += 32) gr[c] = 0.f;
+        const TX* xr = x + i * F;
+        TX* gr = grad + i * F;
+        const float scale = PASS == kVlBackward ? (float)*dloss : 1.f;
+        // element c of the head's gradient slice
+        auto store = [&](int c, float g) {
+            if (PASS == kVlFused) gr[h0 + c] = g;
+            if (PASS == kVlBackward) gr[h0 + c] = from_f32<TX>(scale * g);
+        };
+        if (PASS != kVlForward) {
+            for (int c = lane; c < h0; c += 32) gr[c] = from_f32<TX>(0.f);
+            for (int c = h0 + C + lane; c < F; c += 32) gr[c] = from_f32<TX>(0.f);
+        }
         const long long r = flags[i] ? (long long)rank[i] : -1;
         if (r < 0 || r >= K) {
-            for (int c = lane; c < C; c += 32) gr[h0 + c] = 0.f;
+            if (PASS != kVlForward)
+                for (int c = lane; c < C; c += 32) gr[h0 + c] = from_f32<TX>(0.f);
         } else {
             const T* yr = y + r * C;
             float xv[kVlPerLane], yv[kVlPerLane];
 #pragma unroll
             for (int j = 0; j < kVlPerLane; j++) {
                 const int c = lane + 32 * j;
-                xv[j] = c < C ? __ldg(xr + h0 + c) : 0.f;
+                xv[j] = c < C ? load_f32(xr + h0 + c) : 0.f;
                 yv[j] = c < C ? to_f32(yr[c]) : 0.f;
             }
             if (LOSS == SGB_FEATLOSS_COSINE) {
@@ -385,7 +403,7 @@ __global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F,
 #pragma unroll
                 for (int j = 0; j < kVlPerLane; j++) {
                     const int c = lane + 32 * j;
-                    if (c < C) gr[h0 + c] = fmaf(u, yv[j], v * xv[j]);
+                    if (c < C) store(c, fmaf(u, yv[j], v * xv[j]));
                 }
                 term = valid && lane == 0 ? t : 0.0;
             } else {
@@ -397,7 +415,7 @@ __global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F,
                     if (c < C) {
                         float g;
                         const float t = elementwise_rule<LOSS>(xv[j] - yv[j], gs, g);
-                        gr[h0 + c] = g;
+                        store(c, g);
                         acc += (double)t;
                     }
                 }
@@ -407,6 +425,7 @@ __global__ void __launch_bounds__(kVlThreads) vl_loss_kernel(long long M, int F,
             }
         }
     }
+    if (PASS == kVlBackward) return;
     if (lane == 0) wsum[warp] = term;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -447,37 +466,101 @@ __global__ void __launch_bounds__(256) vl_finish_kernel(long long nb, const doub
     }
 }
 
-template <typename T, int LOSS>
-int launch_voxel_loss(long long M, int F, const float* x, const uint8_t* mask, long long K, int C, int h0, const T* y,
-                      float* grad, const VlWorkspace& w, double* loss, cudaStream_t s) {
-    vl_flags_kernel<<<(unsigned)((M + 255) / 256), 256, 0, s>>>(M, mask, w.flags, w.nv);
-    SGB_LAUNCH_CHECK("vl_flags_kernel", 0, s);
-    size_t tmp_bytes = w.tmp_bytes;
-    SGB_CUDA(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.flags, w.rank, (int)M, s));
-    if (LOSS == SGB_FEATLOSS_COSINE && K > 0) {
-        vl_count_kernel<T><<<(unsigned)((K + kVlRows - 1) / kVlRows), kVlThreads, 0, s>>>(K, C, y, w.nv);
-        SGB_LAUNCH_CHECK("vl_count_kernel", 0, s);
+// One call's operands, untyped until the dispatch below picks TX and T.  grad is null for kVlForward, dloss is
+// non-null for kVlBackward only, and loss and mask are not read by kVlBackward.
+struct VlCall {
+    long long M;
+    int F;
+    const void* x;
+    const uint8_t* mask;
+    long long K;
+    int C, h0;
+    const void* y;
+    const double* dloss;
+    void* grad;
+    VlWorkspace w;
+    double* loss;
+    cudaStream_t s;
+};
+
+// kVlFused and kVlForward: flags, rank and (cosine) Nv into the workspace, the rows, then loss[0..1].  kVlBackward:
+// the rows alone, on the flags, rank and Nv a kVlForward pass on the same mask and target left in the workspace.
+template <int PASS, typename TX, typename T, int LOSS>
+int launch_voxel_loss(const VlCall& a) {
+    const VlWorkspace& w = a.w;
+    const T* y = (const T*)a.y;
+    cudaStream_t s = a.s;
+    if (PASS != kVlBackward) {
+        vl_flags_kernel<<<(unsigned)((a.M + 255) / 256), 256, 0, s>>>(a.M, a.mask, w.flags, w.nv);
+        SGB_LAUNCH_CHECK("vl_flags_kernel", 0, s);
+        size_t tmp_bytes = w.tmp_bytes;
+        SGB_CUDA(cub::DeviceScan::ExclusiveSum(w.tmp, tmp_bytes, w.flags, w.rank, (int)a.M, s));
+        if (LOSS == SGB_FEATLOSS_COSINE && a.K > 0) {
+            vl_count_kernel<T><<<(unsigned)((a.K + kVlRows - 1) / kVlRows), kVlThreads, 0, s>>>(a.K, a.C, y, w.nv);
+            SGB_LAUNCH_CHECK("vl_count_kernel", 0, s);
+        }
     }
-    const long long nb = (M + kVlRows - 1) / kVlRows;
-    vl_loss_kernel<T, LOSS><<<(unsigned)nb, kVlThreads, 0, s>>>(M, F, x, K, C, h0, y, w.flags, w.rank, w.nv, grad,
-                                                                w.partial);
+    const long long nb = (a.M + kVlRows - 1) / kVlRows;
+    vl_loss_kernel<TX, T, LOSS, PASS><<<(unsigned)nb, kVlThreads, 0, s>>>(
+        a.M, a.F, (const TX*)a.x, a.K, a.C, a.h0, y, w.flags, w.rank, w.nv, a.dloss, (TX*)a.grad, w.partial);
     SGB_LAUNCH_CHECK("vl_loss_kernel", 0, s);
-    vl_finish_kernel<<<1, 256, 0, s>>>(nb, w.partial, M, w.flags, w.rank, K, C, LOSS, w.nv, loss);
-    SGB_LAUNCH_CHECK("vl_finish_kernel", 0, s);
+    if (PASS != kVlBackward) {
+        vl_finish_kernel<<<1, 256, 0, s>>>(nb, w.partial, a.M, w.flags, w.rank, a.K, a.C, LOSS, w.nv, a.loss);
+        SGB_LAUNCH_CHECK("vl_finish_kernel", 0, s);
+    }
     return SGB_OK;
 }
 
-template <typename T>
-int launch_voxel_loss(int loss_type, long long M, int F, const float* x, const uint8_t* mask, long long K, int C,
-                      int h0, const T* y, float* grad, const VlWorkspace& w, double* loss, cudaStream_t s) {
-    if (loss_type == SGB_FEATLOSS_COSINE)
-        return launch_voxel_loss<T, SGB_FEATLOSS_COSINE>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
-    if (loss_type == SGB_FEATLOSS_L1)
-        return launch_voxel_loss<T, SGB_FEATLOSS_L1>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
-    return launch_voxel_loss<T, SGB_FEATLOSS_L2>(M, F, x, mask, K, C, h0, y, grad, w, loss, s);
+template <int PASS, typename TX, typename T>
+int launch_voxel_loss(int loss_type, const VlCall& a) {
+    if (loss_type == SGB_FEATLOSS_COSINE) return launch_voxel_loss<PASS, TX, T, SGB_FEATLOSS_COSINE>(a);
+    if (loss_type == SGB_FEATLOSS_L1) return launch_voxel_loss<PASS, TX, T, SGB_FEATLOSS_L1>(a);
+    return launch_voxel_loss<PASS, TX, T, SGB_FEATLOSS_L2>(a);
+}
+
+template <int PASS, typename TX>
+int launch_voxel_loss(int target_dtype, int loss_type, const VlCall& a) {
+    if (target_dtype == SGB_FEAT_F16) return launch_voxel_loss<PASS, TX, __half>(loss_type, a);
+    return launch_voxel_loss<PASS, TX, float>(loss_type, a);
+}
+
+template <int PASS>
+int launch_voxel_loss(int output_dtype, int target_dtype, int loss_type, const VlCall& a) {
+    if (output_dtype == SGB_FEAT_F16) return launch_voxel_loss<PASS, __half>(target_dtype, loss_type, a);
+    if (output_dtype == SGB_FEAT_BF16) return launch_voxel_loss<PASS, __nv_bfloat16>(target_dtype, loss_type, a);
+    return launch_voxel_loss<PASS, float>(target_dtype, loss_type, a);
 }
 
 bool vl_m_ok(int64_t M) { return M >= 0 && M <= INT32_MAX; }
+
+// The argument rules every voxel-row entry point shares: M, C, target_dtype, loss_type, head and K.
+int check_voxel_loss_args(const char* fn, int64_t M, int32_t F, int64_t K, int32_t C, int32_t head,
+                          int32_t target_dtype, int32_t loss_type) {
+    if (!vl_m_ok(M)) { set_error("%s: M = %lld outside [0, %d]", fn, (long long)M, INT32_MAX); return SGB_E_INVALID; }
+    if (check_feature_loss_args(fn, C, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
+    if (head < 0 || (int64_t)head * C + C > F) {
+        set_error("%s: head %d of width %d does not fit in F = %d columns", fn, head, C, F);
+        return SGB_E_INVALID;
+    }
+    if (K < 0 || K > M) { set_error("%s: K = %lld target rows outside [0, M = %lld]", fn, (long long)K, (long long)M); return SGB_E_INVALID; }
+    return SGB_OK;
+}
+
+// The output dtype's element size, or 0 (error set) for an unknown code.
+size_t vl_output_size(const char* fn, int32_t output_dtype) {
+    if (output_dtype == SGB_FEAT_F32) return 4;
+    if (output_dtype == SGB_FEAT_F16 || output_dtype == SGB_FEAT_BF16) return 2;
+    set_error("%s: unknown output_dtype %d (SGB_FEAT_F32, SGB_FEAT_F16 or SGB_FEAT_BF16)", fn, output_dtype);
+    return 0;
+}
+
+int check_vl_alignment(const char* fn, const char* name, const void* p, size_t es) {
+    if (reinterpret_cast<uintptr_t>(p) % es) {
+        set_error("%s: %s is not %d-byte aligned for its dtype", fn, name, (int)es);
+        return SGB_E_INVALID;
+    }
+    return SGB_OK;
+}
 
 }  // namespace
 
@@ -536,13 +619,7 @@ int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint
                            int32_t head, const void* target, int32_t target_dtype, int32_t loss_type, float* grad,
                            void* workspace, double* loss, void* stream) {
     static const char* fn = "sgb_voxel_feature_loss";
-    if (!vl_m_ok(M)) { set_error("%s: M = %lld outside [0, %d]", fn, (long long)M, INT32_MAX); return SGB_E_INVALID; }
-    if (check_feature_loss_args(fn, C, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
-    if (head < 0 || (int64_t)head * C + C > F) {
-        set_error("%s: head %d of width %d does not fit in F = %d columns", fn, head, C, F);
-        return SGB_E_INVALID;
-    }
-    if (K < 0 || K > M) { set_error("%s: K = %lld target rows outside [0, M = %lld]", fn, (long long)K, (long long)M); return SGB_E_INVALID; }
+    if (check_voxel_loss_args(fn, M, F, K, C, head, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
     if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
     if (M > 0 && (!output || !mask || !grad)) { set_error("%s: null output / mask / grad", fn); return SGB_E_INVALID; }
     if (K > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
@@ -553,15 +630,59 @@ int sgb_voxel_feature_loss(int64_t M, int32_t F, const float* output, const uint
         SGB_CUDA(cudaMemsetAsync(loss, 0, 2 * sizeof(double), s));
         return SGB_OK;
     }
-    VlWorkspace w;
-    const int rc = carve_vl_workspace((long long)M, workspace, w);
+    VlCall a{(long long)M, F, output, mask, (long long)K, C, head * C, target, nullptr, grad, {}, loss, s};
+    const int rc = carve_vl_workspace((long long)M, workspace, a.w);
     if (rc) return rc;
-    const int h0 = head * C;
-    if (target_dtype == SGB_FEAT_F16)
-        return launch_voxel_loss<__half>(loss_type, (long long)M, F, output, mask, (long long)K, C, h0,
-                                         (const __half*)target, grad, w, loss, s);
-    return launch_voxel_loss<float>(loss_type, (long long)M, F, output, mask, (long long)K, C, h0,
-                                    (const float*)target, grad, w, loss, s);
+    return launch_voxel_loss<kVlFused, float>(target_dtype, loss_type, a);
+}
+
+int sgb_voxel_feature_loss_forward(int64_t M, int32_t F, const void* output, int32_t output_dtype,
+                                   const uint8_t* mask, int64_t K, int32_t C, int32_t head, const void* target,
+                                   int32_t target_dtype, int32_t loss_type, void* workspace, double* loss,
+                                   void* stream) {
+    static const char* fn = "sgb_voxel_feature_loss_forward";
+    if (check_voxel_loss_args(fn, M, F, K, C, head, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
+    const size_t es = vl_output_size(fn, output_dtype);
+    if (!es) return SGB_E_INVALID;
+    if (!loss) { set_error("%s: null loss", fn); return SGB_E_INVALID; }
+    if (M > 0 && (!output || !mask)) { set_error("%s: null output / mask", fn); return SGB_E_INVALID; }
+    if (K > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
+    if (M > 0 && !workspace) { set_error("%s: null workspace", fn); return SGB_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(workspace) % 16) { set_error("%s: workspace is not 16-byte aligned", fn); return SGB_E_INVALID; }
+    if (check_vl_alignment(fn, "output", output, es) != SGB_OK) return SGB_E_INVALID;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (M == 0) {
+        SGB_CUDA(cudaMemsetAsync(loss, 0, 2 * sizeof(double), s));
+        return SGB_OK;
+    }
+    VlCall a{(long long)M, F, output, mask, (long long)K, C, head * C, target, nullptr, nullptr, {}, loss, s};
+    const int rc = carve_vl_workspace((long long)M, workspace, a.w);
+    if (rc) return rc;
+    return launch_voxel_loss<kVlForward>(output_dtype, target_dtype, loss_type, a);
+}
+
+int sgb_voxel_feature_loss_backward(int64_t M, int32_t F, const void* output, int32_t output_dtype, int64_t K,
+                                    int32_t C, int32_t head, const void* target, int32_t target_dtype,
+                                    int32_t loss_type, const void* workspace, const double* dloss, void* grad,
+                                    void* stream) {
+    static const char* fn = "sgb_voxel_feature_loss_backward";
+    if (check_voxel_loss_args(fn, M, F, K, C, head, target_dtype, loss_type) != SGB_OK) return SGB_E_INVALID;
+    const size_t es = vl_output_size(fn, output_dtype);
+    if (!es) return SGB_E_INVALID;
+    if (!dloss) { set_error("%s: null dloss", fn); return SGB_E_INVALID; }
+    if (M > 0 && (!output || !grad)) { set_error("%s: null output / grad", fn); return SGB_E_INVALID; }
+    if (K > 0 && !target) { set_error("%s: null target", fn); return SGB_E_INVALID; }
+    if (M > 0 && !workspace) { set_error("%s: null workspace", fn); return SGB_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(workspace) % 16) { set_error("%s: workspace is not 16-byte aligned", fn); return SGB_E_INVALID; }
+    if (check_vl_alignment(fn, "output", output, es) != SGB_OK) return SGB_E_INVALID;
+    if (check_vl_alignment(fn, "grad", grad, es) != SGB_OK) return SGB_E_INVALID;
+    if (M == 0) return SGB_OK;
+    VlCall a{(long long)M, F, output, nullptr, (long long)K, C, head * C, target, dloss, grad, {}, nullptr,
+             (cudaStream_t)stream};
+    // the carve is a pure function of M: it finds what the forward pass left where that pass put it
+    const int rc = carve_vl_workspace((long long)M, const_cast<void*>(workspace), a.w);
+    if (rc) return rc;
+    return launch_voxel_loss<kVlBackward>(output_dtype, target_dtype, loss_type, a);
 }
 
 }  // extern "C"

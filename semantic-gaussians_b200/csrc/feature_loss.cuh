@@ -2,6 +2,7 @@
 // feature-map loss and the voxel-row loss (feature_loss.cu) and the decoded-feature loss (decoder_loss.cu).
 #pragma once
 
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -10,8 +11,16 @@ namespace sgb {
 
 constexpr int kFeatMaxC = 1024;  // widest feature map accepted (OpenSeg 768, LSeg 512)
 
+// Half values widen to fp32 exactly; from_f32 rounds to nearest even, as torch's .to(dtype) does.
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+// One value of T as fp32, through the read-only cache.
+template <typename T> __device__ __forceinline__ float load_f32(const T* p) { return to_f32(__ldg(p)); }
 
 // Four consecutive values as fp32; p is 16- (fp32) or 8-byte (fp16) aligned.
 struct Quad { float v[4]; };

@@ -12,12 +12,14 @@ view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:
 ``distill_loss_and_grad``      training loss against per-pixel class labels and K class embeddings.
 ``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2).
 ``decoded_feature_map_loss_and_grads``  the same loss for a compact field through a per-pixel linear decoder.
-``voxel_feature_loss_and_grad``  the same loss on the masked rows of a 3D network's (M, F) output (distill.py)."""
+``voxel_feature_loss_and_grad``  the same loss on the masked rows of a 3D network's (M, F) output (distill.py).
+``voxel_feature_loss``  that loss as an autograd function of an fp32 / fp16 / bf16 output (mixed precision)."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -234,6 +236,92 @@ def voxel_feature_loss_and_grad(output: torch.Tensor, mask: torch.Tensor, featur
                                               y.data_ptr(), dtype, loss_code, grad.data_ptr(), ws.data_ptr(),
                                               loss2.data_ptr(), stream), "sgb_voxel_feature_loss")
     return loss2[0], loss2[1], grad
+
+
+_VOXEL_OUTPUT_DTYPES = {torch.float32: _lib.FEAT_F32, torch.float16: _lib.FEAT_F16, torch.bfloat16: _lib.FEAT_BF16}
+
+
+class _VoxelFeatureLoss(torch.autograd.Function):
+    """sgb_voxel_feature_loss_forward, and sgb_voxel_feature_loss_backward with the upstream gradient as dloss."""
+
+    @staticmethod
+    def forward(ctx, output, mask, features_gt, loss_code, target_code, head, channels):
+        M, F = output.shape
+        lib = _lib.load()
+        nbytes = lib.sgb_voxel_feature_loss_workspace_bytes(M)
+        if nbytes == 0:
+            raise _lib.SgbError("sgb_voxel_feature_loss_workspace_bytes failed")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=output.device)
+        loss2 = torch.empty(2, dtype=torch.float64, device=output.device)
+        stream = torch.cuda.current_stream(output.device).cuda_stream
+        _lib.check(lib.sgb_voxel_feature_loss_forward(M, F, output.data_ptr(), _VOXEL_OUTPUT_DTYPES[output.dtype],
+                                                      mask.data_ptr(), features_gt.shape[0], channels, head,
+                                                      features_gt.data_ptr(), target_code, loss_code, ws.data_ptr(),
+                                                      loss2.data_ptr(), stream), "sgb_voxel_feature_loss_forward")
+        # the workspace keeps the mask's row flags and ranks and the cosine count for the gradient pass
+        ctx.save_for_backward(output, features_gt, ws)
+        ctx.codes = (loss_code, target_code, head, channels)
+        loss, count = loss2.unbind()
+        ctx.mark_non_differentiable(count)
+        return loss, count
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dloss, _dcount):
+        output, features_gt, ws = ctx.saved_tensors
+        loss_code, target_code, head, channels = ctx.codes
+        M, F = output.shape
+        d = dloss.to(device=output.device, dtype=torch.float64).contiguous()
+        grad = torch.empty_like(output)
+        stream = torch.cuda.current_stream(output.device).cuda_stream
+        _lib.check(_lib.load().sgb_voxel_feature_loss_backward(
+            M, F, output.data_ptr(), _VOXEL_OUTPUT_DTYPES[output.dtype], features_gt.shape[0], channels, head,
+            features_gt.data_ptr(), target_code, loss_code, ws.data_ptr(), d.data_ptr(), grad.data_ptr(), stream),
+            "sgb_voxel_feature_loss_backward")
+        return grad, None, None, None, None, None, None
+
+
+def voxel_feature_loss(output: torch.Tensor, mask: torch.Tensor, features_gt: torch.Tensor,
+                       loss_type: str = "cosine", head: int = 0, channels: int = 768
+                       ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``voxel_feature_loss_and_grad``'s loss as a differentiable function of the network output in its own dtype:
+    MinkUNet's (M, F) ``.F`` in fp32, fp16 or bf16 (inside or outside autocast, ``output``'s dtype is used as given).
+    The other arguments and their rules are ``voxel_feature_loss_and_grad``'s.
+
+    Returns (loss, count), 0-d float64 CUDA tensors.  ``loss`` has a ``grad_fn``: ``loss.backward()``, or
+    ``scaler.scale(loss).backward()`` with a ``torch.amp.GradScaler``, sends d loss / d output to ``output`` in
+    output's dtype, computed as ``round(float(upstream) * g)`` with g the fp32 gradient ``voxel_feature_loss_and_grad``
+    gives on ``output.float()``: the scale is applied before the one rounding, so a GradScaler scale keeps fp16
+    gradients out of the subnormal range.  The loss and count are bitwise those of
+    ``voxel_feature_loss_and_grad(output.float(), ...)``.  ``count`` is not differentiable.  Nothing is synchronised and
+    nothing of output's size is allocated besides the gradient; output, features_gt and a workspace of about 9 bytes
+    per row are kept for the backward pass.  Bitwise reproducible."""
+    for name, t in (("output", output), ("mask", mask), ("features_gt", features_gt)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+    if output.dtype not in _VOXEL_OUTPUT_DTYPES or output.ndim != 2:
+        raise ValueError(f"output must be (M, F) float32, float16 or bfloat16, got {tuple(output.shape)} "
+                         f"{output.dtype}")
+    M, F = output.shape
+    if mask.dtype != torch.bool or mask.shape != (M,):
+        raise ValueError(f"mask must be ({M},) bool, got {tuple(mask.shape)} {mask.dtype}")
+    loss_code, target_code = _feature_loss_codes(loss_type, features_gt, "features_gt", " of the output")
+    if features_gt.ndim != 2 or features_gt.shape[1] != channels:
+        raise ValueError(f"features_gt must be (K, {channels}) float16 or float32, got {tuple(features_gt.shape)} "
+                         f"{features_gt.dtype}")
+    if not 1 <= channels <= _FEATURE_MAX_C or head < 0 or (head + 1) * channels > F:
+        raise ValueError(f"head {head} of {channels} channels does not fit in {F} columns "
+                         f"(1 <= channels <= {_FEATURE_MAX_C})")
+    if features_gt.shape[0] > M:
+        raise ValueError(f"features_gt has {features_gt.shape[0]} rows, more than the {M} rows of output")
+    for name, t in (("output", output), ("mask", mask), ("features_gt", features_gt)):
+        if not t.is_cuda:
+            raise ValueError(f"{name} must be a CUDA tensor (the voxel feature loss has no CPU path)")
+    if not (output.device == mask.device == features_gt.device):
+        raise ValueError("output, mask and features_gt must be on one device")
+    with torch.cuda.device(output.device):
+        return _VoxelFeatureLoss.apply(output.contiguous(), mask.contiguous(), features_gt.contiguous(), loss_code,
+                                       target_code, int(head), int(channels))
 
 
 def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Tensor, target: torch.Tensor,
