@@ -19,63 +19,18 @@ is timed: at 3 M x 512 one set of moments is 13 GB."""
 import argparse
 import json
 import os
-import subprocess
 import sys
-from types import SimpleNamespace
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
+from timing import Pipe, device_views, gpu, kernel_ms, time_ms  # noqa: E402
 
 from semantic_gaussians_b200.optim import GaussianAdam, visible_rows  # noqa: E402
 
 PEAK_TBPS = 3.35
 GEOMETRY = (("xyz", (3,)), ("f_dc", (1, 3)), ("f_rest", (15, 3)), ("opacity", (1,)), ("scaling", (3,)), ("rotation", (4,)))
-
-
-class Pipe:
-    convert_shs_python = False
-    compute_cov3d_python = False
-    debug = False
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn, warmup: int, reps: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def kernel_ms(fn, n: int = 5) -> float:
-    """sgb_adam_* kernel time per call, from a profiler pass of its own."""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(n):
-            fn()
-        torch.cuda.synchronize()
-    return sum(e.device_time_total for e in prof.key_averages() if "sgb_adam_" in e.key) / 1e3 / n
-
-
-def views_on(cams, dev):
-    return [SimpleNamespace(image_width=c.image_width, image_height=c.image_height, FoVx=c.FoVx, FoVy=c.FoVy,
-                            world_view_transform=torch.as_tensor(c.world_view_transform, device=dev),
-                            full_proj_transform=torch.as_tensor(c.full_proj_transform, device=dev),
-                            camera_center=torch.as_tensor(c.camera_center, device=dev)) for c in cams]
 
 
 def room_visibility(P, W, H, dev):
@@ -87,7 +42,7 @@ def room_visibility(P, W, H, dev):
     pc = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, device=dev)
     pc.active_sh_degree = 0
     with torch.no_grad():
-        outs = render_chn_batch(views_on(room_cameras(8, W, H), dev), pc, Pipe, torch.zeros(8, device=dev),
+        outs = render_chn_batch(device_views(room_cameras(8, W, H), dev), pc, Pipe, torch.zeros(8, device=dev),
                                 num_channels=8, override_color=torch.rand((P, 8), device=dev))
         one, eight = visible_rows(outs[0]).clone(), visible_rows(outs).clone()
     del outs, pc
@@ -113,12 +68,8 @@ def main():
     ap.add_argument("--sizes", default="1000000x256x1920x1080,3000000x512x1296x968", help="PxCxWxH, comma separated")
     ap.add_argument("--no-step", action="store_true", help="skip the K3-shaped training step")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_adam.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
-    result = {"card": gpu, "tables": {}, "step": {}}
+    dev, gpu_name = gpu("time_adam.py")
+    result = {"card": gpu_name, "tables": {}, "step": {}}
     gen = torch.Generator(device=dev).manual_seed(0)
 
     for size in args.sizes.split(","):
@@ -136,9 +87,9 @@ def main():
             for arm, mask in masks.items():
                 opt = make_optimizer(arm, params)
                 fn = (lambda: opt.step()) if arm in ("torch", "fused") else (lambda: opt.step(visibility=mask))
-                times[arm].append(time_ms(fn, args.warmup, args.reps))
+                times[arm].append(time_ms(fn, args.reps, args.warmup))
                 if rnd == 0 and arm not in ("torch", "fused"):
-                    kern[arm] = kernel_ms(fn)
+                    kern[arm] = kernel_ms(fn, 5, ["sgb_adam_"], warmup=1)["sgb_adam_"]
                 del opt, fn
                 torch.cuda.empty_cache()
         rec = {}
@@ -172,7 +123,7 @@ def main():
         params = [feats, pc._xyz, pc._scaling, pc._rotation, pc._opacity]
         for p in params[1:]:
             p.requires_grad_(True)
-        views = views_on(orbit_cameras(8, W, H), dev)
+        views = device_views(orbit_cameras(8, W, H), dev)
         bg = torch.zeros(C, device=dev)
         with torch.no_grad():
             other = torch.randn(feats.shape, generator=gen, device=dev)
@@ -203,7 +154,7 @@ def main():
                     for p, s in zip(params, start):
                         p.copy_(s)
                 opt = make_optimizer("dense" if arm == "view" else arm, params)
-                times[arm].append(time_ms(lambda: step(opt, arm), 3, args.step_reps))
+                times[arm].append(time_ms(lambda: step(opt, arm), args.step_reps, 3))
                 del opt
                 torch.cuda.empty_cache()
         with torch.no_grad():

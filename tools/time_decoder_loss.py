@@ -15,7 +15,6 @@ backward, against render_chn at C = 512 + feature_map_loss_and_grad + backward (
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,30 +22,12 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
+from timing import Pipe, device_views, gpu, kernel_ms, time_ms  # noqa: E402
 
 from semantic_gaussians_b200.semantic import decoded_feature_map_loss_and_grads, feature_map_loss_and_grad  # noqa: E402
 
 KERNELS = ("decoder_pack_kernel", "count_valid_pixels_kernel", "decoder_loss_kernel", "decoder_reduce_kernel")
 LOSS_TYPES = ("cosine", "l1", "l2")
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn, warmup: int, reps: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def torch_loss(x, target, loss_type):
@@ -69,20 +50,6 @@ def arms(loss_type):
     return {"torch": torch_arm, "fused": fused_arm}
 
 
-def kernel_ms(fn, n=5):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(n):
-            fn()
-        torch.cuda.synchronize()
-    k = {}
-    for e in prof.key_averages():
-        for name in KERNELS:
-            if name in e.key:
-                k[name] = k.get(name, 0.0) + e.device_time_total / 1e3 / n
-    return k
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -93,12 +60,8 @@ def main():
     ap.add_argument("--no-torch", action="store_true", help="time the fused call only")
     ap.add_argument("--profile", action="store_true", help="also report the fused kernels' time (torch.profiler)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_decoder_loss.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
-    result = {"card": gpu, "loss": {}, "step": {}}
+    dev, gpu_name = gpu("time_decoder_loss.py")
+    result = {"card": gpu_name, "loss": {}, "step": {}}
 
     g = torch.Generator(device=dev).manual_seed(0)
     for C, c, H, W in ((512, 64, 968, 1296), (768, 128, 1080, 1920)):
@@ -117,7 +80,7 @@ def main():
             times = {n: [] for n in names}
             for _ in range(args.rounds):
                 for name in names:
-                    times[name].append(time_ms(lambda: fns[name](render, weight, bias, target), args.warmup, args.reps))
+                    times[name].append(time_ms(lambda: fns[name](render, weight, bias, target), args.reps, args.warmup))
             t_f = min(times["fused"])
             line = f"{key}: fused {', '.join(f'{t:.3f}' for t in times['fused'])} ms"
             rec = {"fused_ms": times["fused"], "flops": flops, "algorithmic_GB": nbytes / 1e9}
@@ -129,8 +92,7 @@ def main():
                 rec["torch_ms"] = times["torch"]
             print(line, flush=True)
             if args.profile:
-                # kernel time alone, in a pass of its own (tracing slows the host)
-                k = kernel_ms(lambda: fns["fused"](render, weight, bias, target))
+                k = kernel_ms(lambda: fns["fused"](render, weight, bias, target), 5, KERNELS)
                 tk = sum(k.values())
                 tm = k.get("decoder_loss_kernel", float("nan"))
                 print(f"{key}: kernels " + ", ".join(f"{n_} {v:.3f} ms" for n_, v in sorted(k.items())) +
@@ -144,16 +106,9 @@ def main():
         torch.cuda.empty_cache()
 
     if not args.no_step:
-        from types import SimpleNamespace
-
         from semantic_gaussians_b200.gaussian_model import GaussianModel
         from semantic_gaussians_b200.renderer import render_chn
         from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras
-
-        class Pipe:
-            convert_shs_python = False
-            compute_cov3d_python = False
-            debug = False
 
         C, c, W, H = 512, 64, 1296, 968
         scene = make_scene(1_000_000, seed=0, channels=c)
@@ -166,13 +121,7 @@ def main():
         geo = [pc._xyz, pc._scaling, pc._rotation, pc._opacity]
         for p in geo:
             p.requires_grad_(True)
-        views = []
-        for cam in orbit_cameras(8, W, H):
-            views.append(SimpleNamespace(image_width=cam.image_width, image_height=cam.image_height, FoVx=cam.FoVx,
-                                         FoVy=cam.FoVy,
-                                         world_view_transform=torch.as_tensor(cam.world_view_transform, device=dev),
-                                         full_proj_transform=torch.as_tensor(cam.full_proj_transform, device=dev),
-                                         camera_center=torch.as_tensor(cam.camera_center, device=dev)))
+        views = device_views(orbit_cameras(8, W, H), dev)
         with torch.no_grad():                   # targets: the same scene rendered with other 512-ch features, fp16
             other = torch.randn((P, C), generator=g, device=dev)
             fmaps = [render_chn(v, pc, Pipe, torch.zeros(C, device=dev), num_channels=C,
@@ -201,7 +150,7 @@ def main():
         times = {"wide": [], "compact": []}
         for _ in range(args.rounds):
             for name in ("wide", "compact"):
-                times[name].append(time_ms(lambda: step(name), 2, args.step_reps))
+                times[name].append(time_ms(lambda: step(name), args.step_reps, 2))
         print(f"training step (1M Gaussians, {W}x{H}, cosine): render_chn C={C} + feature_map_loss_and_grad + backward "
               f"{', '.join(f'{t:.2f}' for t in times['wide'])} ms | render_chn c={c} + decoded loss + backward "
               f"{', '.join(f'{t:.2f}' for t in times['compact'])} ms", flush=True)

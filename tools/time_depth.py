@@ -11,45 +11,19 @@ in one run.  Prints the card name, power limit and max SM clock, then one JSON l
 import argparse
 import json
 import os
-import subprocess
 import sys
-from types import SimpleNamespace
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
+from timing import Pipe, device_views, gpu, time_ms  # noqa: E402
 
 from semantic_gaussians_b200 import channel_rasterization as chn  # noqa: E402
 from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
 from semantic_gaussians_b200.loss_utils import photometric_loss  # noqa: E402
 from semantic_gaussians_b200.renderer import _prepare, render, render_with_depth  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras  # noqa: E402
-
-
-class Pipe:
-    convert_shs_python = False
-    compute_cov3d_python = False
-    debug = False
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn, warmup: int, reps: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def depth_l1(E, A, target):
@@ -66,11 +40,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_depth.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
+    dev, gpu_name = gpu("time_depth.py")
     W, H = args.width, args.height
 
     scene = make_scene(args.P, 0, sh=True)
@@ -78,11 +48,7 @@ def main():
     params = [m._xyz, m._opacity, m._scaling, m._rotation, m._features_dc, m._features_rest]
     for p in params:
         p.requires_grad_(True)
-    views = [SimpleNamespace(image_width=c.image_width, image_height=c.image_height, FoVx=c.FoVx, FoVy=c.FoVy,
-                             world_view_transform=torch.as_tensor(c.world_view_transform, device=dev),
-                             full_proj_transform=torch.as_tensor(c.full_proj_transform, device=dev),
-                             camera_center=torch.as_tensor(c.camera_center, device=dev))
-             for c in orbit_cameras(8, W, H)]
+    views = device_views(orbit_cameras(8, W, H), dev)
     bg = torch.zeros(3, device=dev)
     g = torch.Generator(device=dev).manual_seed(0)
     gt = torch.rand((3, H, W), generator=g, device=dev)
@@ -119,13 +85,13 @@ def main():
     times = {a: [] for a in arms}
     for _ in range(args.rounds):
         for a in arms:
-            times[a].append(time_ms(lambda: step(a), args.warmup, args.reps))
+            times[a].append(time_ms(lambda: step(a), args.reps, args.warmup))
     for a in arms:
         print(f"{a:12s} {', '.join(f'{t:.2f}' for t in times[a])} ms/step", flush=True)
     best = {a: min(t) for a, t in times.items()}
     print(f"depth supervision over plain (best of rounds): in-pass +{best['in_pass'] - best['plain']:.2f} ms, "
           f"two renders +{best['two_renders'] - best['plain']:.2f} ms", flush=True)
-    print(json.dumps({"card": gpu, "P": args.P, "W": W, "H": H, "ms_per_step": times}))
+    print(json.dumps({"card": gpu_name, "P": args.P, "W": W, "H": H, "ms_per_step": times}))
 
 
 if __name__ == "__main__":

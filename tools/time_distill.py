@@ -16,7 +16,6 @@ import argparse
 import json
 import os
 import random
-import subprocess
 import sys
 import tempfile
 
@@ -25,6 +24,7 @@ sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from timing import card, time_ms  # noqa: E402
 
 from oracle import augment_oracle as ao  # noqa: E402
 from oracle import voxel_oracle as vo  # noqa: E402
@@ -38,23 +38,6 @@ from semantic_gaussians_b200.semantic import voxel_feature_loss_and_grad  # noqa
 from semantic_gaussians_b200.voxelize import distill_targets  # noqa: E402
 
 DEV = "cuda"
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def timed(fn):
-    """(result, ms) of fn() between two CUDA events, after a synchronise on each side."""
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    r = fn()
-    b.record()
-    torch.cuda.synchronize()
-    return r, a.elapsed_time(b)
 
 
 def write_room(root, P):
@@ -130,8 +113,7 @@ def loss_arms(rows, rounds):
                 torch.cuda.synchronize()
                 base = torch.cuda.memory_allocated()
                 torch.cuda.reset_peak_memory_stats()
-                _, t = timed(lambda: fn(lt))
-                ms[k].append(t)
+                ms[k].append(time_ms(lambda: fn(lt)))
                 peak[k] = (torch.cuda.max_memory_allocated() - base) / 2**30
         res[lt] = {k: {"ms_min": min(v), "ms_max": max(v), "peak_gib": round(peak[k], 3)} for k, v in ms.items()}
         print(lt, json.dumps(res[lt]), flush=True)
@@ -165,7 +147,7 @@ def step_arms(sample, rounds):
         ms = {k: [] for k in arms}
         for _ in range(rounds):
             for k, fn in arms.items():
-                ms[k].append(timed(fn)[1])
+                ms[k].append(time_ms(fn))
         res[lt] = {k: {"ms_min": min(v), "ms_max": max(v)} for k, v in ms.items()}
         print("step", lt, json.dumps(res[lt]), flush=True)
     return res
@@ -195,14 +177,14 @@ def main():
                 else:
                     assert all(torch.equal(a, b) for a, b in zip(want[:4], got[:4])), "host and device samples differ"
             ms = {k: [] for k in arms}
+            s = [None]                       # the last sample, kept until the next one replaces it
             for r in range(args.rounds):
                 for k, fn in arms.items():
                     random.seed(r)
                     np.random.seed(r)
-                    s, t = timed(fn)
-                    ms[k].append(t)
+                    ms[k].append(time_ms(lambda: s.__setitem__(0, fn())))
                     if k == "device" and first_sample is None:
-                        first_sample = s
+                        first_sample = s[0]
             result["sample"][P] = {"voxels": int(want[0].shape[0]),
                                    **{k: {"ms_min": min(v), "ms_max": max(v)} for k, v in ms.items()}}
             print("sample", P, json.dumps(result["sample"][P]), flush=True)

@@ -19,11 +19,11 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
-from time_distill import card, timed, write_room  # noqa: E402
+from time_distill import write_room  # noqa: E402
+from timing import card, time_ms  # noqa: E402
 
 from semantic_gaussians_b200 import sparse as sp  # noqa: E402
 from semantic_gaussians_b200.feature_dataset import collate_fn  # noqa: E402
@@ -45,7 +45,7 @@ def alternate(arms, rounds):
             torch.cuda.synchronize()
             base = torch.cuda.memory_allocated()
             torch.cuda.reset_peak_memory_stats()
-            ms[k].append(timed(fn)[1])
+            ms[k].append(time_ms(fn))
             peak[k] = (torch.cuda.max_memory_allocated() - base) / 2**30
     return {k: {"ms_min": round(min(v), 3), "ms_max": round(max(v), 3), "peak_gib": round(peak[k], 3)}
             for k, v in ms.items()}

@@ -13,10 +13,8 @@ must give the identical matrix.  A separate torch.profiler pass reports the kern
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
-from types import SimpleNamespace
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -24,6 +22,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from timing import Pipe, device_views, gpu  # noqa: E402
 
 from metric_ref import reference_confusion  # noqa: E402
 from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
@@ -31,18 +30,6 @@ from semantic_gaussians_b200.metric import ConfusionMatrix  # noqa: E402
 from semantic_gaussians_b200.renderer import render_chn  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras  # noqa: E402
 from semantic_gaussians_b200.semantic import feature_logits, label_argmax  # noqa: E402
-
-
-class Pipe:
-    convert_shs_python = False
-    compute_cov3d_python = False
-    debug = False
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
 def main():
@@ -54,11 +41,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--channels", type=int, default=64, help="width of the per-Gaussian features")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_eval.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
+    dev, gpu_name = gpu("time_eval.py")
     K, nc, W, H = 20, 19, args.width, args.height
 
     scene = make_scene(args.gaussians, seed=0, channels=args.channels)
@@ -69,11 +52,7 @@ def main():
     text = torch.nn.functional.normalize(torch.randn(K, args.channels, generator=g, device=dev), dim=1)
     label_soft = feature_logits(features, text).softmax(dim=1)          # once per scene
     bg = torch.zeros(K, device=dev)
-    views = [SimpleNamespace(image_width=c.image_width, image_height=c.image_height, FoVx=c.FoVx, FoVy=c.FoVy,
-                             world_view_transform=torch.as_tensor(c.world_view_transform, device=dev),
-                             full_proj_transform=torch.as_tensor(c.full_proj_transform, device=dev),
-                             camera_center=torch.as_tensor(c.camera_center, device=dev))
-             for c in orbit_cameras(args.views, W, H)]
+    views = device_views(orbit_cameras(args.views, W, H), dev)
     rng = np.random.default_rng(0)
     gts = [rng.integers(0, nc + 1, (H, W)).astype(np.uint8) for _ in views]     # 0 = unlabelled
     gts_pinned = [torch.from_numpy(x).pin_memory() for x in gts]
@@ -130,7 +109,7 @@ def main():
                 k_n += e.count
         print(f"sgb_confusion_accumulate kernel: {k_ms / max(k_n, 1) * 1e3:.2f} us per view "
               f"({k_n} launches, {W * H} pixels each)", flush=True)
-    print(json.dumps({"card": gpu, "views": len(views), "ms_per_view": times,
+    print(json.dumps({"card": gpu_name, "views": len(views), "ms_per_view": times,
                       "confusion_kernel_us_per_view": k_ms / max(k_n, 1) * 1e3, "kernel_launches": k_n}))
 
 

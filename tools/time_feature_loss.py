@@ -17,7 +17,6 @@ the cosine loss reads on top of that the target up to each pixel's first non-zer
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -25,29 +24,11 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
+from timing import Pipe, device_views, gpu, kernel_ms, time_ms  # noqa: E402
 
 from semantic_gaussians_b200.semantic import feature_map_loss_and_grad  # noqa: E402
 
 KERNELS = ("count_valid_pixels_kernel", "feature_cosine_kernel", "feature_elementwise_kernel")
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn, warmup: int, reps: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def torch_loss(render, target, loss_type):
@@ -78,12 +59,8 @@ def main():
     ap.add_argument("--no-step", action="store_true", help="skip the K3-shaped training step")
     ap.add_argument("--profile", action="store_true", help="also report the fused kernels' time (torch.profiler)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_feature_loss.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
-    result = {"card": gpu, "loss": {}, "step": {}}
+    dev, gpu_name = gpu("time_feature_loss.py")
+    result = {"card": gpu_name, "loss": {}, "step": {}}
 
     g = torch.Generator(device=dev).manual_seed(0)
     for C, H, W in ((256, 1080, 1920), (512, 968, 1296)):
@@ -99,7 +76,7 @@ def main():
             times = {"torch": [], "fused": []}
             for _ in range(args.rounds):
                 for name in ("torch", "fused"):
-                    times[name].append(time_ms(lambda: fns[name](render, target), args.warmup, args.reps))
+                    times[name].append(time_ms(lambda: fns[name](render, target), args.reps, args.warmup))
             t_t, t_f = min(times["torch"]), min(times["fused"])
             print(f"{key}: torch {', '.join(f'{t:.3f}' for t in times['torch'])} ms | "
                   f"fused {', '.join(f'{t:.3f}' for t in times['fused'])} ms | best-of speed-up {t_t / t_f:.2f}x | "
@@ -108,18 +85,7 @@ def main():
             rec = {"torch_ms": times["torch"], "fused_ms": times["fused"], "algorithmic_GB": nbytes / 1e9,
                    "fused_call_GBps_best": nbytes / (t_f * 1e-3) / 1e9}
             if args.profile:
-                # kernel time alone, in a pass of its own (tracing slows the host)
-                from torch.profiler import ProfilerActivity, profile
-                n = 10
-                with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                    for _ in range(n):
-                        fns["fused"](render, target)
-                    torch.cuda.synchronize()
-                k = {}
-                for e in prof.key_averages():
-                    for name in KERNELS:
-                        if name in e.key:
-                            k[name] = k.get(name, 0.0) + e.device_time_total / 1e3 / n
+                k = kernel_ms(lambda: fns["fused"](render, target), 10, KERNELS)
                 tk = sum(k.values())
                 print(f"{key}: kernels " + ", ".join(f"{n_} {v:.3f} ms" for n_, v in sorted(k.items())) +
                       f" | {nbytes / (tk * 1e-3) / 1e9:.0f} GB/s against the algorithmic bytes", flush=True)
@@ -130,16 +96,9 @@ def main():
         torch.cuda.empty_cache()
 
     if not args.no_step:
-        from types import SimpleNamespace
-
         from semantic_gaussians_b200.gaussian_model import GaussianModel
         from semantic_gaussians_b200.renderer import render_chn
         from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras
-
-        class Pipe:
-            convert_shs_python = False
-            compute_cov3d_python = False
-            debug = False
 
         C, W, H = 256, 1920, 1080
         scene = make_scene(1_000_000, seed=0, channels=C)
@@ -149,12 +108,7 @@ def main():
         params = [feats, pc._xyz, pc._scaling, pc._rotation, pc._opacity]
         for p in params[1:]:
             p.requires_grad_(True)
-        views = []
-        for c in orbit_cameras(8, W, H):
-            views.append(SimpleNamespace(image_width=c.image_width, image_height=c.image_height, FoVx=c.FoVx,
-                                         FoVy=c.FoVy, world_view_transform=torch.as_tensor(c.world_view_transform, device=dev),
-                                         full_proj_transform=torch.as_tensor(c.full_proj_transform, device=dev),
-                                         camera_center=torch.as_tensor(c.camera_center, device=dev)))
+        views = device_views(orbit_cameras(8, W, H), dev)
         bg = torch.zeros(C, device=dev)
         with torch.no_grad():                   # targets: the same scene rendered with other features, stored fp16
             other = torch.randn(feats.shape, generator=g, device=dev)
@@ -176,7 +130,7 @@ def main():
         times = {"torch": [], "fused": []}
         for _ in range(args.rounds):
             for name in ("torch", "fused"):
-                times[name].append(time_ms(lambda: step(name), 3, args.step_reps))
+                times[name].append(time_ms(lambda: step(name), args.step_reps, 3))
         print(f"K3-shaped step (1M Gaussians, 256 ch, 1080p, render_chn + cosine loss + backward): torch loss "
               f"{', '.join(f'{t:.2f}' for t in times['torch'])} ms | fused loss "
               f"{', '.join(f'{t:.2f}' for t in times['fused'])} ms", flush=True)

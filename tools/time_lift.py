@@ -16,7 +16,6 @@ line."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -24,6 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
+from timing import Pipe, device_views, gpu, kernel_ms, time_ms  # noqa: E402
 
 from semantic_gaussians_b200 import _lib  # noqa: E402
 from semantic_gaussians_b200.fusion import fuse_scene, lift_scene  # noqa: E402
@@ -32,52 +32,6 @@ from semantic_gaussians_b200.renderer import render_chn  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene, room_cameras  # noqa: E402
 
 WCHUNK_BYTES = 16 + 16 * 8 + 16 * 256 * 4   # one 16-entry weight-pool chunk (csrc/weight_pool.cuh)
-
-
-class Pipe:
-    convert_shs_python = False
-    compute_cov3d_python = False
-    debug = False
-
-
-class View:
-    def __init__(self, c, dev):
-        self.image_width, self.image_height, self.FoVx, self.FoVy = c.image_width, c.image_height, c.FoVx, c.FoVy
-        self.world_view_transform = torch.as_tensor(c.world_view_transform, device=dev)
-        self.full_proj_transform = torch.as_tensor(c.full_proj_transform, device=dev)
-        self.camera_center = torch.as_tensor(c.camera_center, device=dev)
-        self.intrinsics = c.intrinsics()
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn) -> float:
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1)
-
-
-def kernel_times(fn) -> dict:
-    """Device time of each kernel over one call of fn (torch.profiler, CUDA activities)."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    out = {}
-    for e in prof.key_averages():
-        if e.device_type.name == "CUDA" and e.count:
-            t = getattr(e, "device_time_total", None) or e.cuda_time_total
-            out[e.key[:90]] = round(t / 1000.0, 3)
-    return dict(sorted(out.items(), key=lambda kv: -kv[1]))
 
 
 def main():
@@ -90,16 +44,15 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--quality-channels", type=int, default=16)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_lift.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
+    dev, gpu_name = gpu("time_lift.py")
     P, Cn, W, H, V = args.P, args.C, args.W, args.H, args.views
     scene = make_scene(P, 0, kind="room", sh=True)
     pc = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, shs=scene.shs,
                                       device=dev)
-    views = [View(c, dev) for c in room_cameras(V, W, H)]
+    cams = room_cameras(V, W, H)
+    views = device_views(cams, dev)
+    for v, c in zip(views, cams):
+        v.intrinsics = c.intrinsics()
     g = torch.Generator(device=dev).manual_seed(7)
     NM = 4   # device-resident maps cycled over the views (4 x 315 MB at 512 ch: more than L2 holds)
     maps16 = [torch.randn((Cn, H, W), device=dev, generator=g).half() for _ in range(NM)]
@@ -144,7 +97,7 @@ def main():
     stages = {k: v for k, v in _lib.profile_read(ctx).items() if v[1]}
     _lib.profile_enable(ctx, False)
     print(f"  lift stages (ms, intervals) over {V} views: {json.dumps(stages)}", flush=True)
-    kt = kernel_times(lift)
+    kt = {k: round(v, 3) for k, v in kernel_ms(lift).items()}
     print(f"  lift kernels (ms over {V} views): {json.dumps(kt)}", flush=True)
     bytes_ = {"map_fp16_per_view": Cn * H * W * 2, "map_fp32_per_view": Cn * H * W * 4,
               "pool_chunks_last_view": chunks, "pool_bytes_last_view": chunks * WCHUNK_BYTES,
@@ -171,7 +124,7 @@ def main():
                "mean_cosine_lift": cos(lf), "mean_cosine_centre": cos(cf),
                "mean_cosine_lift_all_it_sees": float(torch.nn.functional.cosine_similarity(lf[lm], f[lm], dim=1).mean())}
     print(f"  quality ({Cq} ch synthetic): {json.dumps(quality)}", flush=True)
-    print(json.dumps({"card": gpu, "P": P, "C": Cn, "W": W, "H": H, "views": V, "ms": t, "lift_stages": stages,
+    print(json.dumps({"card": gpu_name, "P": P, "C": Cn, "W": W, "H": H, "views": V, "ms": t, "lift_stages": stages,
                       "lift_kernels_ms": kt, "bytes": bytes_, "quality": quality}))
 
 

@@ -13,7 +13,6 @@ The achieved rate of (b) is stated against the algorithmic bytes, a floor comput
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -21,30 +20,12 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import torch  # noqa: E402
+from timing import Pipe, device_views, gpu, kernel_ms, time_ms  # noqa: E402
 
 from loss_ref import photometric_torch, window  # noqa: E402
 from semantic_gaussians_b200.loss_utils import photometric_loss  # noqa: E402
 
 BYTES_PER_PLANE_PIXEL = 44
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
-
-
-def time_ms(fn, warmup: int, reps: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def loss_fns(dev):
@@ -62,13 +43,9 @@ def main():
     ap.add_argument("--no-step", action="store_true", help="skip the K2-size training step")
     ap.add_argument("--profile", action="store_true", help="also report the two kernels' time (torch.profiler)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_loss.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
+    dev, gpu_name = gpu("time_loss.py")
     fns = loss_fns(dev)
-    result = {"card": gpu, "loss": {}, "step": {}}
+    result = {"card": gpu_name, "loss": {}, "step": {}}
 
     g = torch.Generator(device=dev).manual_seed(0)
     for (C, H, W), cut in (((3, 1080, 1920), False), ((3, 968, 1296), True)):
@@ -85,7 +62,7 @@ def main():
         times = {"torch": [], "fused": []}
         for _ in range(args.rounds):
             for name in ("torch", "fused"):
-                times[name].append(time_ms(lambda: run(name), args.warmup, args.reps))
+                times[name].append(time_ms(lambda: run(name), args.reps, args.warmup))
         t_t, t_f = min(times["torch"]), min(times["fused"])
         print(f"{key}: torch fwd+bwd {', '.join(f'{t:.3f}' for t in times['torch'])} ms | "
               f"fused {', '.join(f'{t:.3f}' for t in times['fused'])} ms | best-of speed-up {t_t / t_f:.2f}x | "
@@ -93,18 +70,7 @@ def main():
         result["loss"][key] = {"torch_ms": times["torch"], "fused_ms": times["fused"],
                                "algorithmic_GB": nbytes / 1e9, "fused_GBps_best": nbytes / (t_f * 1e-3) / 1e9}
         if args.profile:
-            # kernel time alone, in a pass of its own (tracing slows the host)
-            from torch.profiler import ProfilerActivity, profile
-            n = 20
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                for _ in range(n):
-                    run("fused")
-                torch.cuda.synchronize()
-            k = {}
-            for e in prof.key_averages():
-                for name in ("ssim_fwd_kernel", "ssim_bwd_kernel"):
-                    if name in e.key:
-                        k[name] = k.get(name, 0.0) + e.device_time_total / 1e3 / n
+            k = kernel_ms(lambda: run("fused"), 20, ("ssim_fwd_kernel", "ssim_bwd_kernel"))
             tk = sum(k.values())
             print(f"{key}: kernels " + ", ".join(f"{n_} {v:.3f} ms" for n_, v in sorted(k.items())) +
                   f" | {nbytes / (tk * 1e-3) / 1e9:.0f} GB/s against the algorithmic bytes", flush=True)
@@ -112,16 +78,9 @@ def main():
         del x, y
 
     if not args.no_step:
-        from types import SimpleNamespace
-
         from semantic_gaussians_b200.gaussian_model import GaussianModel
         from semantic_gaussians_b200.renderer import render
         from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras
-
-        class Pipe:
-            convert_shs_python = False
-            compute_cov3d_python = False
-            debug = False
 
         scene = make_scene(1_000_000, 0, sh=True)
         m = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, shs=scene.shs,
@@ -129,12 +88,7 @@ def main():
         params = [m._xyz, m._opacity, m._scaling, m._rotation, m._features_dc, m._features_rest]
         for p in params:
             p.requires_grad_(True)
-        views = []
-        for c in orbit_cameras(8, 1920, 1080):
-            views.append(SimpleNamespace(image_width=c.image_width, image_height=c.image_height, FoVx=c.FoVx,
-                                         FoVy=c.FoVy, world_view_transform=torch.as_tensor(c.world_view_transform, device=dev),
-                                         full_proj_transform=torch.as_tensor(c.full_proj_transform, device=dev),
-                                         camera_center=torch.as_tensor(c.camera_center, device=dev)))
+        views = device_views(orbit_cameras(8, 1920, 1080), dev)
         bg = torch.zeros(3, device=dev)
         gt = torch.rand((3, 1080, 1920), generator=g, device=dev)
         it = [0]
@@ -150,7 +104,7 @@ def main():
         times = {"torch": [], "fused": []}
         for _ in range(args.rounds):
             for name in ("torch", "fused"):
-                times[name].append(time_ms(lambda: step(name), 3, args.step_reps))
+                times[name].append(time_ms(lambda: step(name), args.step_reps, 3))
         print(f"K2 step (1M Gaussians, 1080p, render + loss + backward): torch loss "
               f"{', '.join(f'{t:.2f}' for t in times['torch'])} ms | fused loss "
               f"{', '.join(f'{t:.2f}' for t in times['fused'])} ms", flush=True)

@@ -20,7 +20,6 @@ import argparse
 import contextlib
 import json
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -28,18 +27,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
+from timing import card, time_ms  # noqa: E402
 
 from semantic_gaussians_b200 import sparse as sp  # noqa: E402
 from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
 from semantic_gaussians_b200.mink_unet import mink_unet  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene, surface_voxels  # noqa: E402
 from semantic_gaussians_b200.voxelize import voxelize_gaussians  # noqa: E402
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
 def room_input(P, dev):
@@ -68,17 +62,6 @@ AMP = {"fp32": None, "bf16": torch.bfloat16, "fp16": torch.float16}
 def amp(dt):
     """The autocast context of one timed dtype (none for fp32)."""
     return torch.autocast("cuda", dtype=AMP[dt]) if AMP[dt] else contextlib.nullcontext()
-
-
-def timed(fn, reps):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    s.record()
-    for _ in range(reps):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / reps
 
 
 def layer_stats(model, x):
@@ -182,7 +165,7 @@ def main():
             return mgr
 
         mgr = build_maps()
-        t_maps = timed(build_maps, args.reps)
+        t_maps = time_ms(build_maps, args.reps)
         x = sp.SparseTensor(feats, tensor_stride=1, coordinate_manager=mgr)
         model.train()
 
@@ -208,9 +191,9 @@ def main():
                 try:
                     with amp(dt):
                         fwd(), fwd_bwd()
-                        arms[arm].setdefault("forward_ms", []).append(round(timed(fwd, args.reps), 3))
+                        arms[arm].setdefault("forward_ms", []).append(round(time_ms(fwd, args.reps), 3))
                         torch.cuda.reset_peak_memory_stats(dev)
-                        arms[arm].setdefault("forward_backward_ms", []).append(round(timed(fwd_bwd, args.reps), 3))
+                        arms[arm].setdefault("forward_backward_ms", []).append(round(time_ms(fwd_bwd, args.reps), 3))
                         arms[arm]["peak_allocated_gib"] = round(torch.cuda.max_memory_allocated(dev) / 2 ** 30, 3)
                 except torch.OutOfMemoryError:       # the baseline's autograd keeps every per-offset gather
                     arms[arm]["error"] = f"out of memory at {M} voxels"
@@ -218,7 +201,7 @@ def main():
                     torch.cuda.empty_cache()
                 finally:
                     sp._SparseConvFunction.apply = native
-        t_e2e = timed(lambda: model(sp.SparseTensor(feats, locs)), args.reps)   # maps + forward, train mode, fp32
+        t_e2e = time_ms(lambda: model(sp.SparseTensor(feats, locs)), args.reps)   # maps + forward, train mode, fp32
         layers = layer_stats(model, x)
         flops = sum(2 * r["pairs"] * r["cin"] * r["cout"] for r in layers)
         profiles = {}

@@ -6,6 +6,7 @@ import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
+from timing import Pipe, device_views, time_ms
 from semantic_gaussians_b200.gaussian_model import GaussianModel
 from semantic_gaussians_b200.renderer import render_chn
 from semantic_gaussians_b200.scene_synth import make_scene, orbit_cameras
@@ -19,39 +20,13 @@ pc.active_sh_degree = 0
 feats = torch.as_tensor(scene.features, device=dev).contiguous()
 text = torch.nn.functional.normalize(torch.randn(K, C, device=dev), dim=1)
 bg = torch.zeros(C, device=dev)
+cams = device_views(orbit_cameras(8, W, H), dev)
 
 
-class Pipe:
-    convert_shs_python = False
-    compute_cov3d_python = False
-    debug = False
-
-
-class Cam:
-    pass
-
-
-cams = []
-for c in orbit_cameras(8, W, H):
-    v = Cam()
-    v.image_width, v.image_height, v.FoVx, v.FoVy = c.image_width, c.image_height, c.FoVx, c.FoVy
-    v.world_view_transform = torch.as_tensor(c.world_view_transform, device=dev)
-    v.full_proj_transform = torch.as_tensor(c.full_proj_transform, device=dev)
-    v.camera_center = torch.as_tensor(c.camera_center, device=dev)
-    cams.append(v)
-
-
-def timed(fn, reps=10, warm=3):
-    for i in range(warm):
-        fn(i)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(reps):
-        fn(i)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+def rep_ms(fn, reps=10, warm=3):
+    """time_ms of fn(i): i = 0..warm-1 in the warm-up, then 0..reps-1 in the timed window."""
+    i = iter([*range(warm), *range(reps)])
+    return time_ms(lambda: fn(next(i)), reps, warm)
 
 
 with torch.no_grad():
@@ -63,16 +38,16 @@ with torch.no_grad():
         sim = torch.einsum("cq,qhw->chw", text, rendering)
         return sim[1:].argmax(dim=0)
 
-    t_ref = timed(ref_head)
-    t_ours = timed(lambda i: semantic_head(imgs[i % 2], text))
-    t_label = timed(lambda i: semantic_head(imgs[i % 2], text, return_sim=False))
+    t_ref = rep_ms(ref_head)
+    t_ours = rep_ms(lambda i: semantic_head(imgs[i % 2], text))
+    t_label = rep_ms(lambda i: semantic_head(imgs[i % 2], text, return_sim=False))
     gb = C * W * H * 4 / 1e9
     print(f"head on (256,1080,1920): torch expressions {t_ref:.3f} ms | sgb_semantic_head sim+label {t_ours:.3f} ms "
           f"({gb / t_ours * 1e3:.0f} GB/s of image read) | label only {t_label:.3f} ms ({gb / t_label * 1e3:.0f} GB/s)", flush=True)
     a = ref_head(0); s, l = semantic_head(imgs[0], text)
     print("label agreement with torch:", float((a == l).float().mean()), flush=True)
     del imgs
-    t_logits = timed(lambda i: feature_logits(feats, text, pad_to=4))
+    t_logits = rep_ms(lambda i: feature_logits(feats, text, pad_to=4))
     print(f"feature_logits (1M x 256 -> 24): {t_logits:.3f} ms ({P * C * 4 / 1e9 / t_logits * 1e3:.0f} GB/s)", flush=True)
 
     def full(i):
@@ -93,7 +68,7 @@ with torch.no_grad():
     def fused_pre(i):
         return render_semantic_labels(cams[i % 8], pc, Pipe, bg, text, logits=g)["label"]
 
-    t_ft, t_full, t_fused, t_pre = timed(full_torch), timed(full), timed(fused), timed(fused_pre)
+    t_ft, t_full, t_fused, t_pre = rep_ms(full_torch), rep_ms(full), rep_ms(fused), rep_ms(fused_pre)
     print(f"label map per view: render_chn + torch head {t_ft:.3f} ms | render_chn + sgb head {t_full:.3f} ms | "
           f"logit-space render {t_fused:.3f} ms | with per-scene logits {t_pre:.3f} ms", flush=True)
     la, lb = full(0), fused(0)

@@ -11,7 +11,6 @@ kernel.  Prints the card name, power limit and max SM clock, then one JSON line.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -20,17 +19,12 @@ sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from timing import gpu, kernel_ms, time_ms  # noqa: E402
 
 from oracle import voxel_oracle as vo  # noqa: E402
 from semantic_gaussians_b200.gaussian_model import GaussianModel  # noqa: E402
 from semantic_gaussians_b200.scene_synth import make_scene  # noqa: E402
 from semantic_gaussians_b200.voxelize import voxelize_gaussians  # noqa: E402
-
-
-def card() -> str:
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown (nvidia-smi failed)"
 
 
 def host_round_trip(m, voxel_size, dev):
@@ -42,34 +36,6 @@ def host_round_trip(m, voxel_size, dev):
     return locs_t, torch.from_numpy(feats).float().to(dev), torch.from_numpy(first).to(dev)
 
 
-def time_ms(fn, reps: int) -> float:
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def kernel_times(fn, reps: int) -> dict:
-    """Mean device time per call of each kernel the device arm launches (torch.profiler, CUDA activities)."""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize()
-    out = {}
-    for e in prof.key_averages():
-        if e.device_type.name == "CUDA" and e.count:
-            t = getattr(e, "device_time_total", None) or e.cuda_time_total
-            out[e.key[:90]] = round(t / reps / 1000.0, 4)
-    return dict(sorted(out.items(), key=lambda kv: -kv[1]))
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--P", type=int, nargs="+", default=[1_000_000, 3_000_000])
@@ -78,12 +44,8 @@ def main():
     ap.add_argument("--host-reps", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_voxelize.py needs a GPU")
-    dev = torch.device("cuda:0")
-    gpu = card()
-    print(f"card (name, power limit, max SM clock): {gpu}", flush=True)
-    result = {"card": gpu, "voxel_size": args.voxel_size, "sizes": {}}
+    dev, gpu_name = gpu("time_voxelize.py")
+    result = {"card": gpu_name, "voxel_size": args.voxel_size, "sizes": {}}
     for P in args.P:
         scene = make_scene(P, 0, kind="room", sh=True)
         m = GaussianModel.from_activated(scene.xyz, scene.scales, scene.rotations, scene.opacity, shs=scene.shs,
@@ -106,7 +68,7 @@ def main():
         best = {k: min(v) for k, v in t.items()}
         print(f"  host / device (best of rounds): {best['host'] / best['device']:.0f}x "
               f"({time.perf_counter() - t0:.0f} s timed)", flush=True)
-        kt = kernel_times(dev_arm, args.reps)
+        kt = {k: round(v, 4) for k, v in kernel_ms(dev_arm, args.reps, warmup=1).items()}
         print(f"  kernels (ms per call): {json.dumps(kt)}", flush=True)
         result["sizes"][P] = {"M": M, "ms_per_call": t, "kernel_ms_per_call": kt}
     print(json.dumps(result))
