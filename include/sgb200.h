@@ -495,6 +495,25 @@ int sgb_elastic_displace(int64_t P, const void* xyz, int32_t xyz_is_f64, const f
  * reference).  Fewer than 4 points leave FLT_MAX terms, as in the reference. */
 int sgb_knn_mean_dist2(sgb_ctx* ctx, int32_t P, const float* points, float* mean_dist2, void* stream);
 
+/* ---- nearest reference point of every query point: label / feature transfer from Gaussians onto scan vertices.
+ *
+ * For every query q of query_xyz (M,3) fp32 device and every row j of ref_xyz (P,3) fp32 device:
+ *     d2(q, j) = (dx*dx + dy*dy) + dz*dz,   dx = q.x - r_j.x, dy = q.y - r_j.y, dz = q.z - r_j.z
+ * in fp32, every product and sum rounded alone (no FMA contraction).  Then
+ *     index[q] = the j minimising d2(q, j) over the rows with d2(q, j) <= max_dist2; on ties the smallest j
+ *     dist2[q] = d2(q, index[q])
+ * and a query with no such row gets index -1 and dist2 +inf.  max_dist2 = +inf sets no limit; a negative one matches
+ * nothing.  A reference row with a non-finite coordinate is never returned; a query with a non-finite coordinate gets
+ * -1.  P == 0 gives -1 everywhere; M == 0 launches nothing.  The result is exact (not approximate), so it does not
+ * depend on the order the library visits candidates in.
+ *
+ * index (M) int64 device, dist2 (M) fp32 device.  Bad arguments return SGB_E_INVALID before anything is enqueued: a
+ * null ctx, P or M outside [0, 2^31 - 1], a NaN max_dist2, a null ref_xyz with P > 0, or a null query_xyz / index /
+ * dist2 with M > 0.  Uses the ctx's scratch (grown on demand, about 32 (P + M) bytes).  Asynchronous on `stream`, no
+ * host synchronisation; the same inputs give bitwise identical outputs. */
+int sgb_nearest(sgb_ctx* ctx, int64_t P, const float* ref_xyz, int64_t M, const float* query_xyz, float max_dist2,
+                int64_t* index, float* dist2, void* stream);
+
 /* ---- photometric training loss: the RGB loss of the reference's training step (train.py:141-149)
  *     loss = (1 - lambda) * L1(x, y) + lambda * (1 - SSIM(x, y))
  * with SSIM as utils/loss_utils.py:38-72 computes it: an 11x11 Gaussian window (sigma 1.5, fp32 taps divided by

@@ -88,6 +88,7 @@ EXPORTS = (
     "sgb_sparse_conv_half_forward", "sgb_sparse_conv_half_backward_input_workspace_bytes",
     "sgb_sparse_conv_half_backward_input", "sgb_sparse_conv_half_backward_weight_workspace_bytes",
     "sgb_sparse_conv_half_backward_weight", "sgb_voxel_feature_loss_forward", "sgb_voxel_feature_loss_backward",
+    "sgb_nearest",
 )
 
 _lib = None
@@ -153,6 +154,7 @@ def load() -> C.CDLL:
         lib.sgb_ctx_set_feature_grad_event.argtypes = [vp, vp]
         lib.sgb_ctx_view_stat.argtypes = [vp, C.c_int]
         lib.sgb_knn_mean_dist2.argtypes = [vp, i32, vp, vp, vp]
+        lib.sgb_nearest.argtypes = [vp, i64, vp, i64, vp, C.c_float, vp, vp, vp]
         lib.sgb_distill_loss.argtypes = [i32, i32, i64, vp, vp, vp, i32, vp, vp, vp]
         lib.sgb_ctx_view_stat.restype = i64
         lib.sgb_semantic_head.argtypes = [vp, i32, i32, i64, vp, vp, i32, vp, vp, vp]

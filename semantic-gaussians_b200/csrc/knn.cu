@@ -16,32 +16,13 @@
 #include <cfloat>
 #include <cub/cub.cuh>
 #include "common.cuh"
+#include "spatial.cuh"
 
 namespace sgb {
 
 namespace {
 
 constexpr int kBox = 256;
-
-struct Aabb {
-    float lo[3], hi[3];
-};
-
-// order-preserving float <-> uint mapping for atomicMin / atomicMax
-__device__ __forceinline__ uint32_t f2key(float f) {
-    const uint32_t b = __float_as_uint(f);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__host__ __device__ __forceinline__ float key2f(uint32_t k) {
-    const uint32_t b = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
-#ifdef __CUDA_ARCH__
-    return __uint_as_float(b);
-#else
-    float f;
-    memcpy(&f, &b, 4);
-    return f;
-#endif
-}
 
 __global__ void knn_bounds_init_kernel(uint32_t* mm) {
     if (threadIdx.x < 3) mm[threadIdx.x] = 0xFFFFFFFFu;       // min keys
@@ -75,28 +56,11 @@ __global__ void knn_bounds_kernel(int P, const float* __restrict__ pts, uint32_t
     }
 }
 
-__device__ __forceinline__ uint32_t spread10(uint32_t v) {  // abcdefghij -> a00b00c00d00e00f00g00h00i00j
-    v &= 0x3FFu;
-    v = (v ^ (v << 16)) & 0xFF0000FFu;
-    v = (v ^ (v << 8)) & 0x0300F00Fu;
-    v = (v ^ (v << 4)) & 0x030C30C3u;
-    v = (v ^ (v << 2)) & 0x09249249u;
-    return v;
-}
-
 __global__ void knn_morton_kernel(int P, const float* __restrict__ pts, const uint32_t* __restrict__ mm,
                                   uint32_t* __restrict__ codes, uint32_t* __restrict__ ids) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
-    uint32_t q[3];
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-        const float lo = key2f(mm[a]), hi = key2f(mm[3 + a]);
-        const float ext = hi - lo;
-        const float t = ext > 0.f ? (pts[3 * (size_t)i + a] - lo) / ext : 0.f;
-        q[a] = (uint32_t)fminf(fmaxf(t * 1023.f, 0.f), 1023.f);
-    }
-    codes[i] = spread10(q[0]) | (spread10(q[1]) << 1) | (spread10(q[2]) << 2);
+    codes[i] = morton30(pts + 3 * (size_t)i, mm);
     ids[i] = (uint32_t)i;
 }
 

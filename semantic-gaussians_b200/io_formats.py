@@ -6,11 +6,13 @@
   SH coefficients stored channel-major (``transpose(1, 2).flatten``).
 * fused-feature ``.pt`` — ``{"feat": float16 (n, C), "mask_full": bool (P,)}`` (fusion.py:234-257), consumed at
   eval_segmentation.py:211-219, view_viser.py:61-75, dataset/feature_dataset.py:63-64.
-* dynamic ``params.npz`` (model/gaussian_model.py:346-378)."""
+* dynamic ``params.npz`` (model/gaussian_model.py:346-378).
+* labelled scan vertices — the ``vertex`` properties of a binary little-endian mesh PLY such as ScanNet's
+  ``*_vh_clean_2.labels.ply`` (``load_ply_vertices``), the ground truth of a 3D point evaluation."""
 from __future__ import annotations
 
 import os
-from typing import Dict, List, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -47,35 +49,40 @@ def write_vertex_ply(path: str, names: List[str], table: np.ndarray) -> None:
         f.write(table.tobytes())
 
 
+def _first_element_header(f, path: str):
+    """Read a PLY header up to end_header: (format, first element's name, its count, [(property, dtype code)])."""
+    if f.readline().strip() != b"ply":
+        raise ValueError(f"{path}: not a PLY file")
+    fmt, name, count, props, in_first, seen_elem = None, None, 0, [], False, 0
+    while True:
+        line = f.readline()
+        if not line:
+            raise ValueError(f"{path}: truncated PLY header")
+        tok = line.decode("ascii", "replace").split()
+        if not tok or tok[0] in ("comment", "obj_info"):
+            continue
+        if tok[0] == "format":
+            fmt = tok[1]
+        elif tok[0] == "element":
+            seen_elem += 1
+            in_first = seen_elem == 1
+            if in_first:
+                name, count = tok[1], int(tok[2])
+        elif tok[0] == "property" and in_first:
+            if tok[1] == "list":
+                raise ValueError(f"{path}: list properties are not supported")
+            if tok[1] not in _PLY_TYPES:
+                raise ValueError(f"{path}: unknown property type {tok[1]}")
+            props.append((tok[2], _PLY_TYPES[tok[1]]))
+        elif tok[0] == "end_header":
+            return fmt, name, count, props
+
+
 def read_vertex_ply(path: str) -> Dict[str, np.ndarray]:
     """First element of a PLY file as {property: 1-D array}.  binary_little_endian, binary_big_endian and
     ascii are accepted; list properties are not (the Gaussian layout has none)."""
     with open(path, "rb") as f:
-        if f.readline().strip() != b"ply":
-            raise ValueError(f"{path}: not a PLY file")
-        fmt, count, props, in_first, seen_elem = None, 0, [], False, 0
-        while True:
-            line = f.readline()
-            if not line:
-                raise ValueError(f"{path}: truncated PLY header")
-            tok = line.decode("ascii", "replace").split()
-            if not tok or tok[0] in ("comment", "obj_info"):
-                continue
-            if tok[0] == "format":
-                fmt = tok[1]
-            elif tok[0] == "element":
-                seen_elem += 1
-                in_first = seen_elem == 1
-                if in_first:
-                    count = int(tok[2])
-            elif tok[0] == "property" and in_first:
-                if tok[1] == "list":
-                    raise ValueError(f"{path}: list properties are not supported")
-                if tok[1] not in _PLY_TYPES:
-                    raise ValueError(f"{path}: unknown property type {tok[1]}")
-                props.append((tok[2], _PLY_TYPES[tok[1]]))
-            elif tok[0] == "end_header":
-                break
+        fmt, _, count, props = _first_element_header(f, path)
         if fmt == "ascii":
             rows = np.loadtxt(f, dtype=np.float64, max_rows=count, ndmin=2)
             if rows.shape != (count, len(props)):
@@ -87,6 +94,30 @@ def read_vertex_ply(path: str) -> Dict[str, np.ndarray]:
         dt = np.dtype([(n, order + t) for n, t in props])
         data = np.frombuffer(f.read(dt.itemsize * count), dtype=dt, count=count)
         return {n: np.ascontiguousarray(data[n]).astype(t) for n, t in props}
+
+
+def load_ply_vertices(path: str, names: Sequence[str]) -> Dict[str, np.ndarray]:
+    """The named properties of the ``vertex`` element of a binary little-endian PLY, {name: 1-D array} in each
+    property's own type (``float`` -> float32, ``ushort`` -> uint16, ...).  ``vertex`` must be the first element and
+    hold scalar properties only; the elements after it (faces, edges) are not read.  Enough for the ``x, y, z, label``
+    of a ScanNet ``*_vh_clean_2.labels.ply``; the raw-label -> class mapping is the caller's.  ASCII and big-endian
+    files, a missing property and a truncated body raise ``ValueError``."""
+    with open(path, "rb") as f:
+        fmt, element, count, props = _first_element_header(f, path)
+        if fmt != "binary_little_endian":
+            raise ValueError(f"{path}: PLY format {fmt} is not supported (binary_little_endian only)")
+        if element != "vertex":
+            raise ValueError(f"{path}: the first element is {element!r}, not 'vertex'")
+        have = dict(props)
+        missing = [n for n in names if n not in have]
+        if missing:
+            raise ValueError(f"{path}: vertex element has no properties {missing} (it has {list(have)})")
+        dt = np.dtype([(n, "<" + t) for n, t in props])
+        body = f.read(dt.itemsize * count)
+        if len(body) != dt.itemsize * count:
+            raise ValueError(f"{path}: truncated vertex data ({len(body)} of {dt.itemsize * count} bytes)")
+        data = np.frombuffer(body, dtype=dt, count=count)
+        return {n: np.ascontiguousarray(data[n]).astype(have[n]) for n in names}
 
 
 def save_gaussian_ply(path: str, model) -> None:

@@ -4,7 +4,11 @@ The reference's evaluation (``eval_segmentation.py``) ends every view with a dev
 and a numpy ``bincount``.  ``ConfusionMatrix.add`` enqueues the counting on the current stream instead
 (``sgb_confusion_accumulate``: one kernel, no synchronisation), and ``matrix()`` reads the summed matrix once after
 the last view.  ``get_iou`` / ``evaluate_confusion`` then compute, print and log exactly what the reference's
-functions do, except that the class names are passed in rather than chosen from a dataset string."""
+functions do, except that the class names are passed in rather than chosen from a dataset string.
+
+For a 3D evaluation against labelled points (scan vertices), ``nearest_points`` / ``transfer_labels`` carry the labels
+of the Gaussians (or of the voxels of the 3D network) onto the points by an exact nearest-neighbour query on the GPU
+(``sgb_nearest``), and ``ConfusionMatrix.add`` counts them as it counts label maps."""
 from __future__ import annotations
 
 from typing import Optional, Sequence
@@ -95,6 +99,60 @@ def confusion_matrix(pred_ids: torch.Tensor, gt_ids: torch.Tensor, num_classes: 
     cm = ConfusionMatrix(num_classes, pred_ids.device)
     cm.add(pred_ids, gt_ids)
     return cm.matrix()
+
+
+def nearest_points(query: torch.Tensor, ref: torch.Tensor, max_distance: Optional[float] = None):
+    """Exact nearest row of ``ref`` for every row of ``query``: ``(index int64 (M,), dist2 float32 (M,))``.
+
+    ``query`` (M,3) and ``ref`` (P,3) are float32 CUDA tensors on one device, in the same frame (for scan vertices
+    against Gaussians: the Gaussians' world frame).  ``dist2[q] = (dx*dx + dy*dy) + dz*dz`` in fp32 without FMA,
+    ``index[q]`` the row that minimises it, the smallest row on ties.  ``max_distance`` is in scene units; a row
+    matches only when ``dist2 <= float32(max_distance) * float32(max_distance)`` (that product rounded to fp32), and
+    ``None`` sets no limit.  A query with no match, or with a non-finite coordinate, gets index -1 and dist2 +inf; a
+    reference row with a non-finite coordinate is never returned.  Enqueued on the current stream, no synchronisation
+    (``sgb_nearest``)."""
+    for name, t in (("query", query), ("ref", ref)):
+        if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.ndim != 2
+                or t.shape[1] != 3):
+            raise ValueError(f"{name} must be a float32 (N, 3) CUDA tensor")
+    if query.device != ref.device:
+        raise ValueError(f"query is on {query.device}, ref on {ref.device}: they must be on one device")
+    max_dist2 = float("inf")
+    if max_distance is not None:
+        d = np.float32(max_distance)
+        if not d >= 0:
+            raise ValueError(f"max_distance must be a non-negative number or None, got {max_distance}")
+        with np.errstate(over="ignore"):
+            max_dist2 = float(d * d)
+    q, r = query.detach().contiguous(), ref.detach().contiguous()
+    M, P = q.shape[0], r.shape[0]
+    index = torch.empty(M, dtype=torch.int64, device=q.device)
+    dist2 = torch.empty(M, dtype=torch.float32, device=q.device)
+    if M == 0:
+        return index, dist2
+    with torch.cuda.device(q.device):
+        stream = torch.cuda.current_stream(q.device).cuda_stream
+        ctx = _lib.ctx_for(q.device.index, stream)
+        _lib.check(_lib.load().sgb_nearest(ctx, P, r.data_ptr(), M, q.data_ptr(), max_dist2, index.data_ptr(),
+                                           dist2.data_ptr(), stream), "sgb_nearest")
+    return index, dist2
+
+
+def transfer_labels(query: torch.Tensor, ref: torch.Tensor, ref_labels: torch.Tensor,
+                    max_distance: Optional[float] = None, fill: int = -1) -> torch.Tensor:
+    """Label of the nearest ``ref`` row for every ``query`` row, ``fill`` where ``nearest_points`` finds no match:
+    ``(M,)`` int64 on the device, with no synchronisation.  ``ref_labels`` is an integer CUDA tensor of P labels.
+    With ``fill=-1`` and ``ConfusionMatrix.add(pred, gt, pred_offset=1)`` an unmatched point lands in prediction row 0,
+    which ``get_iou`` counts as a false negative of its class."""
+    if (not isinstance(ref_labels, torch.Tensor) or not isinstance(ref, torch.Tensor)
+            or ref_labels.device != ref.device or tuple(ref_labels.shape) != tuple(ref.shape[:1])
+            or ref_labels.dtype.is_floating_point or ref_labels.dtype.is_complex or ref_labels.dtype == torch.bool):
+        raise ValueError("ref_labels must be an integer tensor of one label per ref row, on ref's device")
+    index, _ = nearest_points(query, ref, max_distance)
+    if ref.shape[0] == 0:
+        return torch.full_like(index, int(fill))
+    labels = ref_labels.to(torch.int64).index_select(0, index.clamp_min(0))
+    return torch.where(index >= 0, labels, torch.full_like(labels, int(fill)))
 
 
 def get_iou(label_id: int, confusion: np.ndarray):

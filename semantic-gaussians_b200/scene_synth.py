@@ -181,6 +181,19 @@ def make_scene(P: int, seed: int = 0, kind: str = "blob", sh: bool = False, chan
                       opacity.astype(np.float32), shs, feats)
 
 
+def surface_points(n: int, seed: int = 0) -> np.ndarray:
+    """(n,3) float32 points on the floor (z = -1.5) and the four walls (x, y = +-4) of the `room` scene, by area, with
+    1 cm jitter: stand-ins for the scan vertices a per-point 3D evaluation labels."""
+    rng = np.random.default_rng(seed)
+    areas = np.array([64.0, 24.0, 24.0, 24.0, 24.0])
+    which = rng.choice(5, size=n, p=areas / areas.sum())
+    p = np.stack([rng.uniform(-4, 4, n), rng.uniform(-4, 4, n), rng.uniform(-1.5, 1.5, n)], 1)
+    p[which == 0, 2] = -1.5
+    for i, (axis, val) in enumerate(((0, -4.0), (0, 4.0), (1, -4.0), (1, 4.0))):
+        p[which == i + 1, axis] = val
+    return (p + rng.normal(0.0, 0.01, (n, 3))).astype(np.float32)
+
+
 def surface_voxels(P: int, dev, seed: int = 0):
     """Voxel rows and features of P points on the floor (z = -1.5) and the four walls (x, y = +-4) of the 8 x 8 x 3 m
     room, by area, with 1 cm jitter, at voxel size 0.02: closer to the occupancy of a scanned scene than the
