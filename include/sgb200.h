@@ -422,6 +422,34 @@ int sgb_semantic_head(sgb_ctx* ctx, int32_t C, int32_t K, int64_t N, const float
 int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const float* features, const float* text,
                        float* out, void* stream);
 int sgb_label_argmax(int32_t K, int32_t first_class, int64_t N, const float* planes, int64_t* label, void* stream);
+/* The semantic head of a compact field through its linear decoder, without the decoded (C, N) image.  render (c, N)
+ * planar fp32, weight (C, c) row-major fp32 (nn.Linear(c, C).weight), bias (C) fp32 or NULL, text (K, C) row-major
+ * fp32.  With x_p = weight render[:, p] + bias:
+ *     sim[k][p] = sum_C text[k][C] x_p[C] / (||x_p||_2 + 1e-8)                 (sgb_semantic_head on x)
+ *     label[p]  = argmax_{first_class <= k < K} sum_C text[k][C] x_p[C] - first_class
+ * computed as A render[:, p] + beta with A = text weight, beta = text bias (float64 sums, rounded to fp32 once), and
+ * ||x_p||^2 as the float64 quadratic form r^T (W^T W) r + 2 (W^T b) . r + ||b||^2 (a negative rounding counts as 0).
+ * The label is the arg-max of the un-normalised numerators (first maximum wins) in both modes, so a label-only call
+ * gives the labels of a sim + label call bitwise; it never forms ||x_p|| and never writes K planes.  sim (K, N) and
+ * label (N) int64 are optional (NULL to skip).  workspace: caller-allocated device scratch of
+ * sgb_decoded_semantic_head_workspace_bytes(C, c, K) bytes, 16-byte aligned (it depends on the widths only).
+ * 1 <= C <= 1024, 1 <= c <= 128, 1 <= K <= 1024, 0 <= first_class < K; a bad argument returns SGB_E_INVALID before
+ * anything is enqueued.  Every output is bitwise identical from call to call (no float atomics).  Asynchronous on
+ * `stream`, no host copy, no ctx; N == 0 or no output does nothing.  The workspace-size call returns 0 for widths
+ * outside those limits.
+ *
+ * sgb_decoded_feature_logits: out[j][k] = text[k] . (weight features[j] + bias) for k < K, row pitch Kpad >= K,
+ * columns K..Kpad-1 zero (sgb_feature_logits on the decoded features, which are never formed: it runs
+ * feature_logits_kernel on A with beta added to each finished dot product; with bias NULL it is sgb_feature_logits
+ * on A).  features (P, c) row-major fp32; the workspace is the head's (same size call).  Same limits and rules. */
+size_t sgb_decoded_semantic_head_workspace_bytes(int32_t C, int32_t c, int32_t K);
+int sgb_decoded_semantic_head(int32_t C, int32_t c, int32_t K, int64_t N, const float* render, const float* weight,
+                              const float* bias /* NULL */, const float* text, int32_t first_class,
+                              float* sim /* (K, N) or NULL */, int64_t* label /* (N) or NULL */, void* workspace,
+                              void* stream);
+int sgb_decoded_feature_logits(int32_t P, int32_t C, int32_t c, int32_t K, int32_t Kpad, const float* features,
+                               const float* weight, const float* bias /* NULL */, const float* text,
+                               float* out /* (P, Kpad) */, void* workspace, void* stream);
 
 /* ---- segmentation confusion matrix: the counting of utils/metric.py::confusion_matrix, on the device.
  *

@@ -88,7 +88,8 @@ EXPORTS = (
     "sgb_sparse_conv_half_forward", "sgb_sparse_conv_half_backward_input_workspace_bytes",
     "sgb_sparse_conv_half_backward_input", "sgb_sparse_conv_half_backward_weight_workspace_bytes",
     "sgb_sparse_conv_half_backward_weight", "sgb_voxel_feature_loss_forward", "sgb_voxel_feature_loss_backward",
-    "sgb_nearest",
+    "sgb_nearest", "sgb_decoded_semantic_head", "sgb_decoded_semantic_head_workspace_bytes",
+    "sgb_decoded_feature_logits",
 )
 
 _lib = None
@@ -160,6 +161,10 @@ def load() -> C.CDLL:
         lib.sgb_semantic_head.argtypes = [vp, i32, i32, i64, vp, vp, i32, vp, vp, vp]
         lib.sgb_feature_logits.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
         lib.sgb_label_argmax.argtypes = [i32, i32, i64, vp, vp, vp]
+        lib.sgb_decoded_semantic_head.argtypes = [i32, i32, i32, i64, vp, vp, vp, vp, i32, vp, vp, vp, vp]
+        lib.sgb_decoded_semantic_head_workspace_bytes.argtypes = [i32, i32, i32]
+        lib.sgb_decoded_semantic_head_workspace_bytes.restype = C.c_size_t
+        lib.sgb_decoded_feature_logits.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
         lib.sgb_photometric_forward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp]
         lib.sgb_photometric_backward.argtypes = [i32, i32, i32, vp, i64, i64, vp, i64, i64, vp, vp, vp, i64, i64, vp]
         lib.sgb_confusion_accumulate.argtypes = [i64, vp, i32, vp, i32, i32, i32, vp, vp, vp]

@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsgb200.so")
-SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "weight_pool.cu", "chn_forward.cu", "chn_dfeature.cu", "chn_chain.cu", "geom_bwd.cu", "fusion.cu", "semantic.cu", "knn.cu", "nearest.cu", "loss.cu", "metric.cu", "feature_loss.cu", "decoder_loss.cu", "voxelize.cu", "elastic.cu", "adam.cu", "sparse_coords.cu", "sparse_conv.cu", "sparse_conv_half.cu"]
+SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "weight_pool.cu", "chn_forward.cu", "chn_dfeature.cu", "chn_chain.cu", "geom_bwd.cu", "fusion.cu", "semantic.cu", "decoded_head.cu", "knn.cu", "nearest.cu", "loss.cu", "metric.cu", "feature_loss.cu", "decoder_loss.cu", "voxelize.cu", "elastic.cu", "adam.cu", "sparse_coords.cu", "sparse_conv.cu", "sparse_conv_half.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -11,6 +11,7 @@
 // the channel planes with 16-byte loads and keeps K running dot products plus the squared norm in
 // registers; the class embeddings sit transposed in shared memory and are read as broadcasts.
 #include "common.cuh"
+#include "semantic.cuh"
 #include "tma.cuh"
 
 namespace sgb {
@@ -262,7 +263,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) semantic_head_tma_kernel(
 template <int NK4>
 __global__ void __launch_bounds__(256) feature_logits_kernel(int P, int C, int K, int Kpad, int k0,
                                                              const float* __restrict__ features,
-                                                             const float* __restrict__ text, float* __restrict__ out) {
+                                                             const float* __restrict__ text,
+                                                             const float* __restrict__ kbias, float* __restrict__ out) {
     constexpr int KC = NK4 * 4;
     extern __shared__ __align__(16) float Ts[];  // [Cp][KC], Cp = C rounded up to 4, zero padded
     const int Cp = (C + 3) & ~3;
@@ -315,6 +317,15 @@ __global__ void __launch_bounds__(256) feature_logits_kernel(int P, int C, int K
             }
         }
         // padding columns (k >= kc) accumulated zeros: the embedding table is zero there
+        if (kbias) {  // per-class constant added to the finished dot product (decoded logits: beta = text . bias)
+#pragma unroll
+            for (int k = 0; k < KC; k++)
+                if (k < kc) {
+                    const float bk = __ldg(kbias + k0 + k);
+                    a0[k] += bk;
+                    a1[k] += bk;
+                }
+        }
         float* o0 = out + (size_t)p0 * Kpad + k0;
         float* o1 = o0 + Kpad;
         if (vout) {
@@ -486,8 +497,8 @@ static int launch_semantic_head(sgb_ctx* ctx, int C, int K, long long N, const f
 }
 
 template <int NK4>
-static int launch_logits_t(int P, int C, int K, int Kpad, int k0, const float* features, const float* text, float* out,
-                           cudaStream_t s) {
+static int launch_logits_t(int P, int C, int K, int Kpad, int k0, const float* features, const float* text,
+                           const float* kbias, float* out, cudaStream_t s) {
     const int Cp = (C + 3) & ~3;
     const size_t smem = sizeof(float) * (size_t)NK4 * 4 * Cp;
     if (smem > 200 * 1024) {
@@ -499,20 +510,20 @@ static int launch_logits_t(int P, int C, int K, int Kpad, int k0, const float* f
         SGB_CUDA(cudaFuncSetAttribute(feature_logits_kernel<NK4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
     const int blocks = min((P + 511) / 512, kNumSMs * 8);
-    feature_logits_kernel<NK4><<<blocks, 256, smem, s>>>(P, C, K, Kpad, k0, features, text, out);
+    feature_logits_kernel<NK4><<<blocks, 256, smem, s>>>(P, C, K, Kpad, k0, features, text, kbias, out);
     SGB_LAUNCH_CHECK("feature_logits_kernel", 0, s);
     return SGB_OK;
 }
 
-static int launch_feature_logits(int P, int C, int K, int Kpad, const float* features, const float* text, float* out,
-                          cudaStream_t s) {
+int launch_feature_logits(int P, int C, int K, int Kpad, const float* features, const float* text, const float* kbias,
+                          float* out, cudaStream_t s) {
     for (int k0 = 0; k0 < Kpad; k0 += 32) {
         const int span = min(32, Kpad - k0);  // columns this pass writes (classes + zero padding)
         int rc;
-        if (span <= 8) rc = launch_logits_t<2>(P, C, K, Kpad, k0, features, text, out, s);
-        else if (span <= 16) rc = launch_logits_t<4>(P, C, K, Kpad, k0, features, text, out, s);
-        else if (span <= 24) rc = launch_logits_t<6>(P, C, K, Kpad, k0, features, text, out, s);
-        else rc = launch_logits_t<8>(P, C, K, Kpad, k0, features, text, out, s);
+        if (span <= 8) rc = launch_logits_t<2>(P, C, K, Kpad, k0, features, text, kbias, out, s);
+        else if (span <= 16) rc = launch_logits_t<4>(P, C, K, Kpad, k0, features, text, kbias, out, s);
+        else if (span <= 24) rc = launch_logits_t<6>(P, C, K, Kpad, k0, features, text, kbias, out, s);
+        else rc = launch_logits_t<8>(P, C, K, Kpad, k0, features, text, kbias, out, s);
         if (rc) return rc;
     }
     return SGB_OK;
@@ -585,7 +596,7 @@ int sgb_feature_logits(int32_t P, int32_t C, int32_t K, int32_t Kpad, const floa
     }
     if (P == 0) return SGB_OK;
     if (!features || !text || !out) { set_error("sgb_feature_logits: null argument"); return SGB_E_INVALID; }
-    return launch_feature_logits(P, C, K, Kpad, features, text, out, (cudaStream_t)stream);
+    return launch_feature_logits(P, C, K, Kpad, features, text, nullptr, out, (cudaStream_t)stream);
 }
 
 int sgb_label_argmax(int32_t K, int32_t first_class, int64_t N, const float* planes, int64_t* label, void* stream) {

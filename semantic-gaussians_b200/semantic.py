@@ -13,7 +13,9 @@ view_viser.py:312-315) and with the per-Gaussian features (eval_segmentation.py:
 ``feature_map_loss_and_grad``  training loss against a 2D model's feature map (cosine / l1 / l2).
 ``decoded_feature_map_loss_and_grads``  the same loss for a compact field through a per-pixel linear decoder.
 ``voxel_feature_loss_and_grad``  the same loss on the masked rows of a 3D network's (M, F) output (distill.py).
-``voxel_feature_loss``  that loss as an autograd function of an fp32 / fp16 / bf16 output (mixed precision)."""
+``voxel_feature_loss``  that loss as an autograd function of an fp32 / fp16 / bf16 output (mixed precision).
+``decoded_semantic_head`` / ``decoded_feature_logits``  the head and the per-Gaussian logits of a compact field through
+                       its linear decoder, without the decoded image or table."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -381,6 +383,109 @@ def decoded_feature_map_loss_and_grads(rendering: torch.Tensor, weight: torch.Te
     return loss2[0], g_render, g_weight, g_bias
 
 
+_DECODED_MAX_K = 1024         # most classes the decoded head accepts
+
+
+def _decoder_args(what: str, inputs, weight, text_features, bias, in_name: str, in_shape: str, c_dim: int,
+                  first_class: int = 0) -> Tuple[torch.Tensor, ...]:
+    """Checks shared by decoded_semantic_head and decoded_feature_logits: ``inputs`` (the c-channel rendering or
+    features, of ``in_shape`` with c at ``c_dim``), weight (C,c), text_features (K,C), bias (C,) or None, all CUDA
+    tensors on one device; weight and bias float32; 0 <= first_class < K.  Returns (inputs, weight, text, bias)
+    detached, float32 and contiguous."""
+    if not isinstance(inputs, torch.Tensor) or inputs.ndim != len(in_shape.split(",")):
+        raise ValueError(f"{in_name} must be a ({in_shape}) tensor")
+    for name, t in ((in_name, inputs), ("weight", weight), ("text_features", text_features), ("bias", bias)):
+        if not isinstance(t, torch.Tensor) and not (name == "bias" and t is None):
+            raise ValueError(f"{name} must be a tensor")
+    if weight.dtype != torch.float32 or (bias is not None and bias.dtype != torch.float32):
+        raise ValueError(f"weight and bias must be float32, got {weight.dtype} and "
+                         f"{None if bias is None else bias.dtype}")
+    for name, t in ((in_name, inputs), ("text_features", text_features)):
+        if not t.is_floating_point():
+            raise ValueError(f"{name} must be a floating-point tensor, got {t.dtype}")
+    if weight.ndim != 2 or text_features.ndim != 2 or text_features.shape[1] != weight.shape[0] or \
+            (bias is not None and tuple(bias.shape) != (weight.shape[0],)):
+        raise ValueError(f"weight must be (C,c), text_features (K,C) and bias (C,), got {tuple(weight.shape)}, "
+                         f"{tuple(text_features.shape)} and {None if bias is None else tuple(bias.shape)}")
+    C_, c = weight.shape
+    K = text_features.shape[0]
+    if not (1 <= C_ <= _FEATURE_MAX_C and 1 <= c <= 128 and 1 <= K <= _DECODED_MAX_K):
+        raise ValueError(f"the decoder must have 1 <= C <= {_FEATURE_MAX_C} outputs and 1 <= c <= 128 inputs, and "
+                         f"1 <= K <= {_DECODED_MAX_K} classes, got (C, c) = ({C_}, {c}) and K = {K}")
+    if inputs.shape[c_dim] != c:
+        raise ValueError(f"{in_name} must be ({in_shape}) with c = {c} (weight's columns), got {tuple(inputs.shape)}")
+    if not (0 <= first_class < K):
+        raise ValueError(f"first_class {first_class} out of range for K = {K}")
+    tensors = [inputs, weight, text_features] + ([bias] if bias is not None else [])
+    if not inputs.is_cuda or any(t.device != inputs.device for t in tensors):
+        raise ValueError(f"{in_name}, weight, text_features and bias must be CUDA tensors on one device (the {what} "
+                         f"has no CPU path), got {', '.join(str(t.device) for t in tensors)}")
+    return (inputs.detach().float().contiguous(), weight.detach().contiguous(),
+            text_features.detach().float().contiguous(), bias.detach().contiguous() if bias is not None else None)
+
+
+def decoded_semantic_head(rendering: torch.Tensor, weight: torch.Tensor, text_features: torch.Tensor,
+                          bias: Optional[torch.Tensor] = None, first_class: int = 1, return_sim: bool = True,
+                          return_label: bool = True) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """``semantic_head`` of a compact field's rendering through its linear decoder, without the decoded image:
+    rendering (c,H,W), weight (C,c) (``nn.Linear(c, C).weight``), bias (C,) or None, text_features (K,C) ->
+    (sim (K,H,W) float32 or None, label (H,W) int64 or None) with
+
+        x     = torch.einsum("kc,chw->khw", weight, rendering) + bias[:, None, None]
+        sim, label = semantic_head(x, text_features, first_class)
+
+    The label is the arg-max of the un-normalised similarities (the positive per-pixel norm does not move it), so
+    ``return_sim=False`` gives the same labels bitwise, reads the rendering once and never forms the norm.  ||x|| is a
+    float64 quadratic form in the rendering, accurate where the decoded pixel is much shorter than its terms.  weight
+    and bias are read detached (they may be nn.Parameters).  1 <= C <= 1024, 1 <= c <= 128, 1 <= K <= 1024.  Nothing
+    is synchronised; besides the outputs only a scratch buffer that depends on C, c and K is allocated; bitwise
+    reproducible."""
+    r, w, t, b = _decoder_args("decoded semantic head", rendering, weight, text_features, bias, "rendering", "c,H,W", 0,
+                               first_class)
+    C_, c = w.shape
+    K = t.shape[0]
+    _, H, W = r.shape
+    sim = torch.empty((K, H, W), dtype=torch.float32, device=r.device) if return_sim else None
+    label = torch.empty((H, W), dtype=torch.int64, device=r.device) if return_label else None
+    lib = _lib.load()
+    with torch.cuda.device(r.device):
+        ws = torch.empty(lib.sgb_decoded_semantic_head_workspace_bytes(C_, c, K), dtype=torch.uint8, device=r.device)
+        stream = torch.cuda.current_stream(r.device).cuda_stream
+        _lib.check(lib.sgb_decoded_semantic_head(C_, c, K, H * W, r.data_ptr(), w.data_ptr(),
+                                                 b.data_ptr() if b is not None else None, t.data_ptr(), first_class,
+                                                 sim.data_ptr() if sim is not None else None,
+                                                 label.data_ptr() if label is not None else None, ws.data_ptr(),
+                                                 stream), "sgb_decoded_semantic_head")
+    return sim, label
+
+
+def decoded_feature_logits(features: torch.Tensor, weight: torch.Tensor, text_features: torch.Tensor,
+                           bias: Optional[torch.Tensor] = None, pad_to: int = 1) -> torch.Tensor:
+    """``feature_logits`` of a compact field's (P,c) per-Gaussian features through its linear decoder: (P, Kpad) with
+    ``einsum("cq,dq->dc", text, features @ weight.T + bias)`` in columns [0,K) and zeros in the padding columns
+    (Kpad = K rounded up to a multiple of ``pad_to``), without forming the (P,C) decoded table.
+
+    ``render_semantic_labels(..., logits=decoded_feature_logits(f, W, text, b, pad_to=4), bg_color=W @ bg_c + b)``
+    renders the decoded label map straight from these: the blend weights and the final transmittance sum to one, so
+    the constant text . b blends through unchanged as long as the background is decoded the same way."""
+    if pad_to < 1:
+        raise ValueError(f"pad_to must be >= 1, got {pad_to}")
+    f, w, t, b = _decoder_args("decoded feature logits", features, weight, text_features, bias, "features", "P,c", 1)
+    C_, c = w.shape
+    P = f.shape[0]
+    K = t.shape[0]
+    Kpad = ((K + pad_to - 1) // pad_to) * pad_to
+    out = torch.empty((P, Kpad), dtype=torch.float32, device=f.device)
+    lib = _lib.load()
+    with torch.cuda.device(f.device):
+        ws = torch.empty(lib.sgb_decoded_semantic_head_workspace_bytes(C_, c, K), dtype=torch.uint8, device=f.device)
+        stream = torch.cuda.current_stream(f.device).cuda_stream
+        _lib.check(lib.sgb_decoded_feature_logits(P, C_, c, K, Kpad, f.data_ptr(), w.data_ptr(),
+                                                  b.data_ptr() if b is not None else None, t.data_ptr(),
+                                                  out.data_ptr(), ws.data_ptr(), stream), "sgb_decoded_feature_logits")
+    return out
+
+
 def render_semantic_labels(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, text_features: torch.Tensor,
                            features: Optional[torch.Tensor] = None, first_class: int = 1, scaling_modifier=1.0,
                            override_shape=None, foreground=None, world_rotate=None,
@@ -391,7 +496,10 @@ def render_semantic_labels(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, t
     ``render_chn(..., num_channels=C, override_color=features)`` -> normalise -> einsum -> ``sim[1:].argmax``:
     sum_c text[k][c] * (sum_j w_j f_j[c] + T bg[c]) = sum_j w_j (text[k].f_j) + T (text[k].bg).
     ``logits``: a precomputed ``feature_logits(features, text_features, pad_to=4)`` — it depends only on the
-    scene and the label set, so an evaluation loop computes it once and passes it for every view.
+    scene and the label set, so an evaluation loop computes it once and passes it for every view.  For a compact
+    field with a linear decoder, pass ``logits=decoded_feature_logits(f, W, text, b, pad_to=4)`` and the decoded
+    background ``bg_color=W @ bg_c + b``: the blend weights and the final transmittance sum to one, so text . b
+    blends through unchanged.
     Returns {"label": (H,W) int64, "logits": (K,H,W) un-normalised similarities, "radii", "visibility_filter"}."""
     from .renderer import render_chn
     t = _check(text_features, "text_features")
