@@ -234,6 +234,50 @@ int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, c
                            const float* const* dL_dalpha /* NULL or [V] */,
                            const sgb_view_grads* grads /* [V] */, void* stream);
 
+/* ---- colour and a feature field in one pass: what a joint RGB + feature training step renders.
+ *
+ * sgb_forward_render_joint_batch is sgb_forward_render_batch_ext of the RGB render in `in` (C = 3, shs or
+ * colors_precomp, RGB background; out_depths required, out_exp_depths / out_alphas as there, given together or not
+ * at all) that ALSO writes out_features[v] (c, H, W): the render of the second colour table `features` (P, c) over
+ * `bg_features` (c), bit for bit what sgb_forward_render_batch gives with colors_precomp = features.  Both images come
+ * from one geometry state per view (one sgb_forward_geometry_batch call with the RGB inputs) and ONE binning per view.
+ * For c > 4 one walk of the view's tile lists is both the RGB blend and the alpha pass that builds the feature image's
+ * weight pool; the forward contraction follows the one weight-pool check of the batch.  For c <= 4 the small-C blend
+ * runs once per image on the same lists.  Any c >= 1.
+ *
+ * sgb_backward_joint_batch is the backward of both images: per view dL/dfeature (c > 4, every view first, then the
+ * feature-gradient event), the feature image's chain / blend backward, the RGB blend backward (with the
+ * dL_dexp_depth / dL_dalpha terms when given) and ONE geometry backward with the RGB colour gradient.  The two
+ * blend backwards add into the same grads[v].dL_dmeans2D / dL_dconic / dL_dopacity, so those hold the sum of both
+ * images' gradients.  dL_dfeatures (P, c) is accumulated over the views (caller zero-fills); grads[v].dL_dcolors is
+ * the RGB colour gradient with sgb_backward_batch's sharing rule (with shs every view needs its own).
+ *
+ * Both calls return SGB_E_INVALID before enqueuing anything for: in->C != 3, c < 1, a null feature table, feature
+ * background, output (median depth included) or upstream array or entry, shared dL_dcolors under shs,
+ * out_exp_depths without out_alphas or the reverse, and every argument rule of the RGB entry points.  Neither
+ * synchronises beyond what
+ * sgb_forward_render_batch does (one sync for the weight-pool checks when c > 4; the backward syncs only when it must
+ * rebuild a pool its forward no longer holds). */
+int sgb_forward_render_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                   const int64_t* num_rendered /* [V] host */, void* const* geometry_states,
+                                   void* const* binning_states, void* const* image_states,
+                                   const int32_t* const* radii, float* const* out_colors,
+                                   float* const* out_depths /* [V] */,
+                                   float* const* out_exp_depths /* NULL or [V] */,
+                                   float* const* out_alphas /* NULL or [V] */, const float* features /* (P, c) */,
+                                   int32_t c, const float* bg_features /* (c) */,
+                                   float* const* out_features /* [V] (c, H, W) */, void* stream);
+int sgb_backward_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                             const int64_t* num_rendered, const int32_t* const* radii,
+                             const void* const* geometry_states, const void* const* binning_states,
+                             const void* const* image_states, const float* const* dL_dpix /* [V] (3, H, W) */,
+                             const float* const* dL_dexp_depth /* NULL or [V] */,
+                             const float* const* dL_dalpha /* NULL or [V] */,
+                             const sgb_view_grads* grads /* [V] */, const float* features /* (P, c) */, int32_t c,
+                             const float* bg_features /* (c) */,
+                             const float* const* dL_dfeature_pix /* [V] (c, H, W) */,
+                             float* dL_dfeatures /* (P, c) */, void* stream);
+
 /* Identity of the build: "<version> src:<sha256 prefix of csrc/ + include/>" (set by build.py; bench.py prints
  * it so that a stale prebuilt library cannot be mistaken for the sources next to it). */
 const char* sgb_build_id(void);

@@ -89,7 +89,7 @@ EXPORTS = (
     "sgb_sparse_conv_half_backward_input", "sgb_sparse_conv_half_backward_weight_workspace_bytes",
     "sgb_sparse_conv_half_backward_weight", "sgb_voxel_feature_loss_forward", "sgb_voxel_feature_loss_backward",
     "sgb_nearest", "sgb_decoded_semantic_head", "sgb_decoded_semantic_head_workspace_bytes",
-    "sgb_decoded_feature_logits",
+    "sgb_decoded_feature_logits", "sgb_forward_render_joint_batch", "sgb_backward_joint_batch",
 )
 
 _lib = None
@@ -138,6 +138,12 @@ def load() -> C.CDLL:
                                                      C.POINTER(i64), pvp, pvp, pvp, pvp, pvp, pvp, pvp, pvp, vp]
         lib.sgb_backward_batch_ext.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), C.POINTER(i64),
                                                pvp, pvp, pvp, pvp, pvp, pvp, pvp, C.POINTER(ViewGrads), vp]
+        lib.sgb_forward_render_joint_batch.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera),
+                                                       C.POINTER(i64), pvp, pvp, pvp, pvp, pvp, pvp, pvp, pvp, vp,
+                                                       i32, vp, pvp, vp]
+        lib.sgb_backward_joint_batch.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), C.POINTER(i64),
+                                                 pvp, pvp, pvp, pvp, pvp, pvp, pvp, C.POINTER(ViewGrads), vp, i32, vp,
+                                                 pvp, vp, vp]
         lib.sgb_build_id.restype = C.c_char_p
         lib.sgb_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
         lib.sgb_state_field.argtypes = [C.c_char_p, i32, i64, i32, i32, vp, vp, vp, vp, vp]

@@ -437,6 +437,151 @@ int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, c
                          dL_dexp_depth, dL_dalpha, grads, (cudaStream_t)stream);
 }
 
+// ---- colour and a feature table through one geometry pass and one binning per view ---------------------------
+// The RGB inputs with the feature table in place of the colours: the view the feature stages see.  Geometry, binning
+// and image state are the RGB render's (neither depends on the colours), so the feature blend reads the same lists.
+static sgb_view_inputs feature_inputs(const sgb_view_inputs& rgb, const float* features, int32_t c,
+                                      const float* bg_features) {
+    sgb_view_inputs f = rgb;
+    f.C = c;
+    f.shs = nullptr;
+    f.M = 0;
+    f.colors_precomp = features;
+    f.background = bg_features;
+    return f;
+}
+
+static int check_joint(const char* what, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                       const float* features, int32_t c, const float* bg_features) {
+    int rc = check_batch(in, V, cams);
+    if (rc) return rc;
+    if (in->C != 3) { set_error("%s: the colour image has C = 3, got C = %d", what, in->C); return SGB_E_INVALID; }
+    if (c < 1) { set_error("%s: need a feature table with c >= 1 channels, got c = %d", what, c); return SGB_E_INVALID; }
+    if (!features || !bg_features) { set_error("%s: null feature table or feature background", what); return SGB_E_INVALID; }
+    return SGB_OK;
+}
+
+// Per view: binning once, then both images on the same lists.  c > 4: ONE walk, the alpha pass that also blends the
+// RGB image, median depth and expected depth / alpha (alpha_pass_rgb_kernel), then after the one pool check of the
+// batch the forward contraction.  c <= 4: the small-C blend of each image.  Every walk writes final_T / n_contrib /
+// tile_last with the RGB blend's statement sequence, so the image state is what the RGB render leaves.
+static int forward_joint_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sgb_view_inputs& fin, int V,
+                              const sgb_camera* cams, const int64_t* num_rendered, void* const* geometry_states,
+                              void* const* binning_states, void* const* image_states, const int32_t* const* radii,
+                              float* const* out_colors, float* const* out_depths, float* const* out_exp_depths,
+                              float* const* out_alphas, float* const* out_features, cudaStream_t s) {
+    int64_t maxR = 0;
+    for (int v = 0; v < V; v++) maxR = num_rendered[v] > maxR ? num_rendered[v] : maxR;
+    int rc = reserve_binning(ctx, in, in.P > 0 ? maxR : 0, s);
+    if (rc) return rc;
+    ViewState vf[SGB_MAX_BATCH];
+    const bool wide = fin.C > 4;
+    for (int v = 0; v < V; v++) {
+        const ViewState w = ViewState::carve(in, cams[v], num_rendered[v], geometry_states[v], binning_states[v],
+                                             image_states[v]);
+        vf[v] = ViewState::carve(fin, cams[v], num_rendered[v], geometry_states[v], binning_states[v],
+                                 image_states[v]);
+        rc = run_binning(ctx, w.in, w.R, w.g, w.b, w.im, radii[v], s);
+        if (rc) return rc;
+        if (wide) {  // one walk: the alpha pass of the feature image is also the RGB blend
+            const AlphaRgb rgb{w.colors, w.in.background, out_colors[v], out_depths[v],
+                               out_exp_depths ? out_exp_depths[v] : nullptr, out_alphas ? out_alphas[v] : nullptr};
+            rc = weight_pool_build(ctx, vf[v], s, &rgb);
+            if (rc) return rc;
+            continue;
+        }
+        StageTimer t(ctx, ST_BLEND_FWD, s);
+        ctx->launches += 2;
+        rc = launch_blend_forward(w.in, w.g, w.b, w.im, w.colors, out_colors[v], out_depths[v],
+                                  out_exp_depths ? out_exp_depths[v] : nullptr, out_alphas ? out_alphas[v] : nullptr, s);
+        if (!rc)
+            rc = launch_blend_forward(vf[v].in, vf[v].g, vf[v].b, vf[v].im, vf[v].colors, out_features[v], nullptr,
+                                      nullptr, nullptr, s);
+        if (rc) return rc;
+    }
+    if (!wide) return SGB_OK;
+    PoolView pv[SGB_MAX_BATCH];
+    rc = weight_pool_settle(ctx, V, vf, pv, s);
+    if (rc) return rc;
+    for (int v = 0; v < V; v++) {
+        rc = chn_forward(ctx, vf[v], pv[v], out_features[v], s);
+        if (rc) return rc;
+    }
+    return SGB_OK;
+}
+
+// Per view, after every view's dL/dfeature (c > 4) and the feature-gradient event: the feature image's chain (or
+// small-C blend) backward, the RGB blend backward with the depth terms, and ONE geometry backward with the RGB colour
+// gradient.  Both blend backwards add into the same dL_dmeans2D / dL_dconic / dL_dopacity.
+static int backward_joint_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sgb_view_inputs& fin, int V,
+                               const sgb_camera* cams, const int64_t* num_rendered, const int32_t* const* radii,
+                               const void* const* geometry_states, const void* const* binning_states,
+                               const void* const* image_states, const float* const* dL_dpix,
+                               const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                               const sgb_view_grads* grads, const float* const* dL_dfeature_pix, float* dL_dfeatures,
+                               cudaStream_t s) {
+    if (in.P == 0) {
+        if (ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
+        return SGB_OK;
+    }
+    ViewState vw[SGB_MAX_BATCH], vf[SGB_MAX_BATCH];
+    for (int v = 0; v < V; v++) {
+        vw[v] = ViewState::carve(in, cams[v], num_rendered[v], geometry_states[v], binning_states[v], image_states[v]);
+        vf[v] = ViewState::carve(fin, cams[v], num_rendered[v], geometry_states[v], binning_states[v], image_states[v]);
+    }
+    const bool wide = fin.C > 4;
+    int rc;
+    float* dL_ddepth = nullptr;
+    if (dL_dexp_depth || dL_dalpha) {
+        rc = ctx->depth_grad.ensure(sizeof(float) * (size_t)in.P);
+        if (rc) return rc;
+        dL_ddepth = (float*)ctx->depth_grad.p;
+    }
+    PoolView pv[SGB_MAX_BATCH];
+    if (wide) {
+        rc = weight_rows_for_backward(ctx, V, vf, pv, s);
+        if (rc) return rc;
+        for (int v = 0; v < V; v++) {
+            if (vf[v].R <= 0) continue;
+            rc = chn_dfeature(ctx, vf[v], pv[v], dL_dfeature_pix[v], dL_dfeatures, s);
+            if (rc) return rc;
+        }
+        if (ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
+    }
+    for (int v = 0; v < V; v++) {
+        const sgb_view_grads& gr = grads[v];
+        if (vf[v].R > 0 && wide) {
+            rc = chn_chain(ctx, vf[v], pv[v], dL_dfeature_pix[v], gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dopacity, s);
+            if (rc) return rc;
+        } else if (vf[v].R > 0) {
+            StageTimer t(ctx, ST_BLEND_BWD, s);
+            ctx->launches += 1;
+            rc = launch_blend_backward(vf[v].in, vf[v].g, vf[v].b, vf[v].im, vf[v].colors, dL_dfeature_pix[v],
+                                       gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dopacity, dL_dfeatures, nullptr, nullptr,
+                                       nullptr, s);
+            if (rc) return rc;
+        }
+        if (!wide && v == V - 1 && ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
+        if (vw[v].R > 0) {
+            if (dL_ddepth) SGB_CUDA(cudaMemsetAsync(dL_ddepth, 0, sizeof(float) * (size_t)in.P, s));
+            StageTimer t(ctx, ST_BLEND_BWD, s);
+            ctx->launches += 1;
+            rc = launch_blend_backward(vw[v].in, vw[v].g, vw[v].b, vw[v].im, vw[v].colors, dL_dpix[v], gr.dL_dmeans2D,
+                                       gr.dL_dconic, gr.dL_dopacity, gr.dL_dcolors,
+                                       dL_dexp_depth ? dL_dexp_depth[v] : nullptr, dL_dalpha ? dL_dalpha[v] : nullptr,
+                                       dL_ddepth, s);
+            if (rc) return rc;
+        }
+        const float* cov3D = in.cov3D_precomp ? in.cov3D_precomp : vw[v].g.cov3D;
+        StageTimer t(ctx, ST_GEOM_BWD, s);
+        ctx->launches += 1;
+        rc = launch_geom_backward(vw[v].in, vw[v].g, radii[v], cov3D, gr.dL_dcolors, gr,
+                                  vw[v].R > 0 ? dL_ddepth : nullptr, s);
+        if (rc) return rc;
+    }
+    return SGB_OK;
+}
+
 // ---- lifting feature maps onto the Gaussians by their blend weights ------------------------------------------
 // Per view: geometry, binning and the alpha pass (the weight pool) into ctx scratch, then the dL/dfeature contraction
 // with the map as dL/dout and the per-Gaussian weight-row sums.  No colour blend, no chain or geometry backward.
@@ -527,6 +672,78 @@ int sgb_lift_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb
     if (rc) return rc;
     if (in->P == 0) return SGB_OK;
     return lift_impl(ctx, g, V, cams, maps, map_dtype, feat_sum, weight_sum, (cudaStream_t)stream);
+}
+
+int sgb_forward_render_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                   const int64_t* num_rendered, void* const* geometry_states,
+                                   void* const* binning_states, void* const* image_states,
+                                   const int32_t* const* radii, float* const* out_colors, float* const* out_depths,
+                                   float* const* out_exp_depths, float* const* out_alphas, const float* features,
+                                   int32_t c, const float* bg_features, float* const* out_features, void* stream) {
+    const char* what = "sgb_forward_render_joint_batch";
+    int rc = check_joint(what, in, V, cams, features, c, bg_features);
+    if (rc) return rc;
+    if (!ctx || !num_rendered || !geometry_states || !binning_states || !image_states || !radii || !out_colors ||
+        !out_depths || !out_features) {
+        set_error("%s: null argument", what);
+        return SGB_E_INVALID;
+    }
+    if ((out_exp_depths == nullptr) != (out_alphas == nullptr)) {
+        set_error("out_exp_depths and out_alphas are given together or not at all");
+        return SGB_E_INVALID;
+    }
+    for (int v = 0; v < V; v++)
+        if (!image_states[v] || !out_colors[v] || !out_features[v] || !out_depths[v] ||
+            (in->P > 0 && (!geometry_states[v] || !radii[v])) || (num_rendered[v] > 0 && !binning_states[v]) ||
+            (out_exp_depths && (!out_exp_depths[v] || !out_alphas[v]))) {
+            set_error("%s: null state/output of view %d", what, v);
+            return SGB_E_INVALID;
+        }
+    return forward_joint_impl(ctx, *in, feature_inputs(*in, features, c, bg_features), V, cams, num_rendered,
+                              geometry_states, binning_states, image_states, radii, out_colors, out_depths,
+                              out_exp_depths, out_alphas, out_features, (cudaStream_t)stream);
+}
+
+int sgb_backward_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                             const int64_t* num_rendered, const int32_t* const* radii,
+                             const void* const* geometry_states, const void* const* binning_states,
+                             const void* const* image_states, const float* const* dL_dpix,
+                             const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                             const sgb_view_grads* grads, const float* features, int32_t c, const float* bg_features,
+                             const float* const* dL_dfeature_pix, float* dL_dfeatures, void* stream) {
+    const char* what = "sgb_backward_joint_batch";
+    int rc = check_joint(what, in, V, cams, features, c, bg_features);
+    if (rc) return rc;
+    if (!ctx || !num_rendered || !radii || !geometry_states || !binning_states || !image_states || !dL_dpix || !grads ||
+        !dL_dfeature_pix || !dL_dfeatures) {
+        set_error("%s: null argument", what);
+        return SGB_E_INVALID;
+    }
+    for (int v = 0; v < V; v++) {
+        if ((dL_dexp_depth && !dL_dexp_depth[v]) || (dL_dalpha && !dL_dalpha[v])) {
+            set_error("%s: null dL_dexp_depth / dL_dalpha of view %d", what, v);
+            return SGB_E_INVALID;
+        }
+        if (in->P == 0) continue;
+        const sgb_view_grads& gr = grads[v];
+        if (!geometry_states[v] || !radii[v] || !image_states[v] || !dL_dpix[v] || !dL_dfeature_pix[v] ||
+            !gr.dL_dmeans2D || !gr.dL_dconic || !gr.dL_dopacity || !gr.dL_dcolors || !gr.dL_dmeans3D ||
+            !gr.dL_dcov3D || (in->shs && !gr.dL_dsh) || (in->scales && (!gr.dL_dscales || !gr.dL_drotations))) {
+            set_error("%s: null state or gradient buffer of view %d", what, v);
+            return SGB_E_INVALID;
+        }
+    }
+    if (in->shs)  // as sgb_backward_batch: view v's geometry kernel reads dL_dcolors as view v's RGB gradient
+        for (int v = 1; v < V; v++)
+            for (int u = 0; u < v; u++)
+                if (grads[v].dL_dcolors == grads[u].dL_dcolors) {
+                    set_error("%s: views %d and %d share one dL_dcolors buffer; with shs every view needs its own "
+                              "dL_dcolors", what, u, v);
+                    return SGB_E_INVALID;
+                }
+    return backward_joint_impl(ctx, *in, feature_inputs(*in, features, c, bg_features), V, cams, num_rendered, radii,
+                               geometry_states, binning_states, image_states, dL_dpix, dL_dexp_depth, dL_dalpha, grads,
+                               dL_dfeature_pix, dL_dfeatures, (cudaStream_t)stream);
 }
 
 int64_t sgb_ctx_view_stat(const sgb_ctx* ctx, int which) {

@@ -19,6 +19,9 @@ struct __align__(16) AlphaSmem {
     uint32_t cur_chunk;
     uint32_t s_last;
 };
+struct __align__(16) AlphaSmemRgb : AlphaSmem {  // the RGB walk's staging: AlphaSmem's layout, then the colours
+    float rgb[kAB][3];
+};
 
 __global__ void __launch_bounds__(kTileThreads) alpha_pass_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
@@ -166,6 +169,203 @@ __global__ void __launch_bounds__(kTileThreads) alpha_pass_kernel(
     }
 }
 
+// The alpha pass that is also the view's RGB blend (sgb_forward_render_joint_batch): alpha_pass_kernel's walk,
+// statement for statement, plus blend_fwd.cu's per-pixel colour accumulation C[k] += f * alpha * T, median depth
+// and (EXP_ALPHA) expected depth / alpha in blend_forward_kernel's order, so the RGB outputs are bit for bit that
+// kernel's.  One walk of the tile lists gives the weight pool of the feature image and the whole RGB render.  It is a
+// kernel of its own so that alpha_pass_kernel keeps its code.
+template <bool EXP_ALPHA>
+__global__ void __launch_bounds__(kTileThreads) alpha_pass_rgb_kernel(
+    const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
+    const SplatRec* __restrict__ rec, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
+    uint32_t* __restrict__ tile_last, PoolView pool, AlphaRgb rgb) {
+    constexpr bool RGB = true;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    AlphaSmem& sm = *reinterpret_cast<AlphaSmem*>(smem_raw);
+    float (*s_rgb)[3] = reinterpret_cast<AlphaSmemRgb*>(smem_raw)->rgb;
+
+    const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
+    const int tile = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t tx = tid & (SGB_TILE - 1), ty = tid >> 4;
+    const uint2 pix = {(uint32_t)(tile % tiles_x) * SGB_TILE + tx, (uint32_t)(tile / tiles_x) * SGB_TILE + ty};
+    const uint32_t pix_id = W * pix.y + pix.x;
+    const float2 pixf = {(float)pix.x, (float)pix.y};
+    const bool inside = pix.x < (uint32_t)W && pix.y < (uint32_t)H;
+    bool done = !inside;
+
+    const uint2 range = ranges[tile];
+    const int total = (int)(range.y - range.x);
+    const int nbatches = (total + kAB - 1) / kAB;
+    const uint32_t dbase = range.x / kChunkEntries + (uint32_t)tile;
+    if (tid == 0) { sm.cur_chunk = kNone; sm.s_last = 0; }
+
+    float T = 1.0f;
+    uint32_t last_contributor = 0;
+    uint32_t n_tile = 0;  // entries appended so far (uniform)
+    uint32_t n_blend = 0; // Gaussians blended into this pixel
+
+    // Staging of the (id, splat record) batches is software-pipelined in warp 0's registers: the ids run two
+    // batches ahead, the records (a dependent gather through the id) one batch ahead, so neither round trip
+    // sits between two batches of the chain (it used to: two dependent L2/DRAM latencies per 32 entries).
+    auto load_id = [&](int bb) -> uint32_t {
+        const int i = bb * kAB + tid;
+        return (tid < kAB && bb < nbatches && i < total) ? __ldg(point_list + range.x + i) : 0u;
+    };
+    uint32_t id_cur = load_id(0), id_nxt = load_id(1);
+    float4 rA = make_float4(0.f, 0.f, 0.f, 0.f), rB = rA;
+    float c0 = 0.f, c1 = 0.f, c2 = 0.f;  // RGB: the colour of the record in rA / rB
+    if (tid < kAB && tid < total) {
+        const float4* rp = reinterpret_cast<const float4*>(rec + id_cur);
+        rA = __ldg(rp);
+        rB = __ldg(rp + 1);
+        if (RGB) {
+            c0 = __ldg(rgb.colors + (size_t)id_cur * 3);
+            c1 = __ldg(rgb.colors + (size_t)id_cur * 3 + 1);
+            c2 = __ldg(rgb.colors + (size_t)id_cur * 3 + 2);
+        }
+    }
+    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;  // RGB
+    float D = 15.0f;                           // RGB: rgbd forward.cu:308, default median depth
+    float acc_z = 0.f, acc_w = 0.f;            // EXP_ALPHA: E and A
+    for (int b = 0; b < nbatches; b++) {
+        const int num_done = __syncthreads_count(done);  // forward.cu:310-312
+        if (num_done == kTileThreads) break;
+        const int base = b * kAB;
+        const int cnt = min(kAB, total - base);
+        if (tid < cnt) {
+            sm.ids[tid] = id_cur;
+            sm.recA[tid] = rA;
+            sm.recB[tid] = rB;
+            if (RGB) {
+                s_rgb[tid][0] = c0;
+                s_rgb[tid][1] = c1;
+                s_rgb[tid][2] = c2;
+            }
+        }
+        __syncthreads();
+        if (tid < kAB) {  // records of batch b+1 (its ids are already here), ids of batch b+2
+            id_cur = id_nxt;
+            if (base + kAB + tid < total) {
+                const float4* rp = reinterpret_cast<const float4*>(rec + id_cur);
+                rA = __ldg(rp);
+                rB = __ldg(rp + 1);
+                if (RGB) {
+                    c0 = __ldg(rgb.colors + (size_t)id_cur * 3);
+                    c1 = __ldg(rgb.colors + (size_t)id_cur * 3 + 1);
+                    c2 = __ldg(rgb.colors + (size_t)id_cur * 3 + 2);
+                }
+            }
+            id_nxt = load_id(b + 2);
+        }
+        uint32_t my_mask = 0;
+        for (int j = 0; j < cnt; j++) {
+            float w = 0.f;
+            if (!done) {
+                // forward.cu:333-362 verbatim
+                const float4 a = sm.recA[j];
+                const float2 xy = {a.x, a.y};
+                const float2 d = {xy.x - pixf.x, xy.y - pixf.y};
+                const float4 con_o = sm.recB[j];
+                const float power = -0.5f * (con_o.x * d.x * d.x + con_o.z * d.y * d.y) - con_o.y * d.x * d.y;
+                if (!(power > 0.0f)) {
+                    const float alpha = min(0.99f, con_o.w * exp(power));
+                    if (!(alpha < 1.0f / 255.0f)) {
+                        const float test_T = T * (1 - alpha);
+                        if (test_T < 0.0001f) {
+                            done = true;
+                        } else {
+                            if (RGB) {  // blend_fwd.cu: forward.cu:355-356, median and expected depth, in its order
+                                acc0 += s_rgb[j][0] * alpha * T;
+                                acc1 += s_rgb[j][1] * alpha * T;
+                                acc2 += s_rgb[j][2] * alpha * T;
+                                if (T > 0.5f && test_T < 0.5) D = a.z;
+                                if (EXP_ALPHA) {
+                                    acc_z += a.z * alpha * T;
+                                    // blend_fwd.cu's `acc_w += 1.0f * alpha * T` compiles to one FFMA; here the
+                                    // product alpha * T is also the weight, and would be reused rounded
+                                    acc_w = __fmaf_rn(alpha, T, acc_w);
+                                }
+                            }
+                            w = alpha * T;
+                            T = test_T;
+                            last_contributor = (uint32_t)(base + j + 1);
+                        }
+                    }
+                }
+            }
+            sm.wbuf[j][tid] = w;
+            n_blend += (w != 0.f);
+            if (__ballot_sync(0xffffffffu, w != 0.f)) my_mask |= 1u << j;
+        }
+        if (lane == 0) sm.wmask[warp] = my_mask;
+        __syncthreads();
+        uint32_t tm = 0;
+#pragma unroll
+        for (int q = 0; q < 8; q++) tm |= sm.wmask[q];
+        const int n_act = __popc(tm);
+        if (n_act) {
+            if (tid == 0) {
+                uint32_t e = n_tile, cur = sm.cur_chunk;
+                for (int k = 0; k < n_act; k++, e++) {
+                    if ((e & (kChunkEntries - 1)) == 0) {
+                        uint32_t nw = atomicAdd(&pool.hdr->counter, 1u);
+                        if (nw >= pool.capacity) {
+                            pool.hdr->overflow = 1;
+                            nw = pool.capacity - 1;
+                        }
+                        pool.dir[dbase + e / kChunkEntries] = nw;
+                        cur = nw;
+                    }
+                    sm.slot_chunk[k] = cur;
+                }
+                sm.cur_chunk = cur;
+            }
+            __syncthreads();
+            int k = 0;
+            for (uint32_t m = tm; m; m &= m - 1, k++) {
+                const int j = __ffs(m) - 1;
+                const uint32_t e = n_tile + k;
+                WChunk& ck = pool.chunks[sm.slot_chunk[k]];
+                const int s = e & (kChunkEntries - 1);
+                ck.w[s][tid] = sm.wbuf[j][tid];
+                if (tid == 0) {
+                    uint32_t strips = 0;
+#pragma unroll
+                    for (int q = 0; q < 8; q++) strips |= ((sm.wmask[q] >> j) & 1u) << q;
+                    ck.meta[s] = make_uint2(sm.ids[j], strips);
+                }
+            }
+            n_tile += n_act;
+        }
+    }
+    if (inside) {
+        final_T[pix_id] = T;
+        n_contrib[pix_id] = last_contributor;
+        atomicMax(&sm.s_last, last_contributor);
+        if (RGB) {
+            const size_t plane = (size_t)H * W;
+            rgb.out_color[pix_id] = acc0 + T * rgb.bg[0];
+            rgb.out_color[plane + pix_id] = acc1 + T * rgb.bg[1];
+            rgb.out_color[2 * plane + pix_id] = acc2 + T * rgb.bg[2];
+            rgb.out_depth[pix_id] = D;
+            if (EXP_ALPHA) {
+                rgb.out_exp_depth[pix_id] = acc_z;
+                rgb.out_alpha[pix_id] = acc_w;
+            }
+        }
+    }
+    n_blend = __reduce_add_sync(0xffffffffu, n_blend);
+    if (lane == 0 && n_blend) atomicAdd(&pool.hdr->blended, (unsigned long long)n_blend);
+    __syncthreads();
+    if (tid == 0) {
+        tile_last[tile] = sm.s_last;
+        pool.count[tile] = n_tile;
+        pool.dirbase[tile] = dbase;
+    }
+}
+
+
 // weight_sum[g] += sum over the tile's pixels of w[entry][px], for every entry of every tile of a view's pool: the
 // denominator of a lift (sgb_lift_batch).  CTA = tile, warp = one 16-entry chunk at a time; every row is read once,
 // by all 32 lanes (two coalesced float4 per lane), and reduced across the warp.
@@ -242,7 +442,7 @@ static uint64_t pool_first_guess(sgb_ctx* ctx, int tiles, int64_t R) {
 // Slot of a view that is about to be (re)built: the one already keyed by its binning state (a new forward through
 // the same pointer replaces it), else an empty one, else the least recently used.  It is carved for the first guess,
 // or keeps a larger existing carve that its memory still holds.
-int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s) {
+int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s, const AlphaRgb* rgb) {
     PoolSlot* sl = slot_of(ctx, w);
     if (!sl)
         for (PoolSlot& c : ctx->pools->slots)
@@ -263,15 +463,27 @@ int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s) {
     if (rc) return rc;
     sl->chunks = chunks;
     const PoolView pv = slot_view(w, *sl);
-    const size_t smem = sizeof(AlphaSmem);
     static DeviceOnce attr_set;
-    if (attr_set.first_use_on_device())
-        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (attr_set.first_use_on_device()) {
+        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sizeof(AlphaSmem)));
+        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_rgb_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sizeof(AlphaSmemRgb)));
+        SGB_CUDA(cudaFuncSetAttribute(alpha_pass_rgb_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sizeof(AlphaSmemRgb)));
+    }
     SGB_CUDA(cudaMemsetAsync(pv.hdr, 0, sizeof(PoolHdr), s));
     {
         StageTimer t(ctx, ST_ALPHA, s);
-        alpha_pass_kernel<<<tiles, kTileThreads, smem, s>>>(w.im.ranges, w.b.point_list, w.in.W, w.in.H, w.g.rec,
-                                                        w.im.final_T, w.im.n_contrib, w.im.tile_last, pv);
+        if (!rgb) {
+            alpha_pass_kernel<<<tiles, kTileThreads, sizeof(AlphaSmem), s>>>(
+                w.im.ranges, w.b.point_list, w.in.W, w.in.H, w.g.rec, w.im.final_T, w.im.n_contrib, w.im.tile_last, pv);
+        } else {
+            auto kern = rgb->out_exp_depth ? alpha_pass_rgb_kernel<true> : alpha_pass_rgb_kernel<false>;
+            kern<<<tiles, kTileThreads, sizeof(AlphaSmemRgb), s>>>(w.im.ranges, w.b.point_list, w.in.W, w.in.H,
+                                                                 w.g.rec, w.im.final_T, w.im.n_contrib,
+                                                                 w.im.tile_last, pv, *rgb);
+        }
         SGB_LAUNCH_CHECK("alpha_pass_kernel", w.in.debug, s);
         ctx->launches += 1;
     }

@@ -87,6 +87,18 @@ struct Readback {
     PoolHdr pool_hdr[SGB_MAX_BATCH];                 // pool header of every slot
 };
 
+// The RGB image a view's alpha pass may produce on the same walk (the joint colour + feature render): the blend of
+// `colors` (P, 3) over `bg` (3) into out_color (3, H, W) and the median depth into out_depth (1, H, W), bit for bit
+// what launch_blend_forward writes; out_exp_depth / out_alpha (both or neither) the expected depth and alpha.
+struct AlphaRgb {
+    const float* colors;
+    const float* bg;
+    float* out_color;
+    float* out_depth;
+    float* out_exp_depth;
+    float* out_alpha;
+};
+
 // ------------------------------------------------------------------ host entry points
 //   weight_pool_build         enqueue the alpha pass of one view into its slot (no sync), so that a batch enqueues
 //                             the alpha passes of all its views before the one sync that checks their pools
@@ -96,7 +108,9 @@ struct Readback {
 //                             under one sync)
 //   weight_pool_release       empties the slots of views [0, V): a lift keeps nothing for a backward
 // The blend kernels take the PoolView and look up nothing.
-int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s);
+//                             (with `rgb`, the walk is also the view's RGB blend; a rebuild after an overflow runs
+//                             the plain pass, since the walk and so the RGB outputs do not depend on the pool)
+int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s, const AlphaRgb* rgb = nullptr);
 int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s,
                        const bool* only = nullptr);
 int weight_rows_for_backward(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s);

@@ -17,6 +17,11 @@ from torch import nn
 # optimiser group name -> attribute of the model (model/gaussian_model.py:202-232)
 GROUPS = (("xyz", "_xyz"), ("f_dc", "_features_dc"), ("f_rest", "_features_rest"), ("opacity", "_opacity"),
           ("scaling", "_scaling"), ("rotation", "_rotation"))
+# Per-Gaussian tables outside the geometry: the semantic feature field (an optimiser group "semantic" when training
+# arguments carry semantic_feature_lr) and the fusion view counts.  Whenever one has a row per Gaussian, densification
+# keeps it row-aligned: clones and split children copy the parent's feature row and start with _times 0, pruned rows
+# go.  A table without a row per Gaussian (empty, as a fresh model has them) is left as it is.
+ROW_TABLES = (("semantic", "_features_semantic"), ("times", "_times"))
 
 
 def expon_lr(lr_init: float, lr_final: float, max_steps: int, delay_steps: int = 0, delay_mult: float = 1.0
@@ -35,8 +40,10 @@ def expon_lr(lr_init: float, lr_final: float, max_steps: int, delay_steps: int =
 
 
 class DensifyMixin:
-    """Mixed into GaussianModel.  State: ``optimizer`` (Adam, one group per row of GROUPS), ``xyz_gradient_accum``
-    (P,1), ``denom`` (P,1), ``max_radii2D`` (P,), ``percent_dense``, ``spatial_lr_scale``."""
+    """Mixed into GaussianModel.  State: ``optimizer`` (Adam, one group per row of GROUPS, plus "semantic" when the
+    feature field is trained), ``xyz_gradient_accum`` (P,1), ``denom`` (P,1), ``max_radii2D`` (P,),
+    ``percent_dense``, ``spatial_lr_scale``.  Groups of other names (a decoder's weights) may share the optimiser:
+    densification leaves them alone."""
 
     # ---- set-up -----------------------------------------------------------------------------------------
     def training_setup(self, training_args) -> None:
@@ -56,6 +63,11 @@ class DensifyMixin:
             p = nn.Parameter(getattr(self, attr).detach().clone().requires_grad_(True))
             setattr(self, attr, p)
             groups.append({"params": [p], "lr": lrs[name], "name": name})
+        semantic_lr = getattr(training_args, "semantic_feature_lr", None)
+        if semantic_lr is not None and self._row_table("_features_semantic") is not None:
+            p = nn.Parameter(self._features_semantic.detach().clone().requires_grad_(True))
+            self._features_semantic = p
+            groups.append({"params": [p], "lr": semantic_lr, "name": "semantic"})
         optimizer_type = getattr(training_args, "optimizer_type", "default")
         if optimizer_type == "default":
             self.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
@@ -79,21 +91,42 @@ class DensifyMixin:
             self.active_sh_degree += 1
 
     # ---- the one primitive: rewrite every parameter (and its Adam moments) row-wise ---------------------------
+    def _row_table(self, attr: str) -> Optional[torch.Tensor]:
+        """The ROW_TABLES entry ``attr`` if it has one row per Gaussian, else None."""
+        t = getattr(self, attr, None)
+        if isinstance(t, torch.Tensor) and t.ndim >= 1 and t.numel() > 0 and t.shape[0] == self._xyz.shape[0]:
+            return t
+        return None
+
     def _rewrite(self, rows: Callable[[str, torch.Tensor], torch.Tensor],
                  moments: Callable[[str, torch.Tensor], torch.Tensor]) -> None:
-        """Replace each group's parameter by ``rows(name, old)`` and, where Adam already holds moments for it,
-        those by ``moments(name, m)``; re-bind the model attributes to the new Parameters."""
-        attr_of = dict(GROUPS)
+        """Replace each per-Gaussian group's parameter by ``rows(name, old)`` and, where Adam already holds moments
+        for it, those by ``moments(name, m)``; re-bind the model attributes to the new Parameters.  The ROW_TABLES
+        entries with a row per Gaussian that no group holds get ``rows(name, old)`` too; other groups are untouched."""
+        attr_of = dict(GROUPS + ROW_TABLES)
+        tables = [(n, a) for n, a in ROW_TABLES if self._row_table(a) is not None]  # before _xyz changes length
         for g in self.optimizer.param_groups:
+            name = g.get("name")
+            if name not in attr_of:
+                continue
             old = g["params"][0]
             state = self.optimizer.state.pop(old, None)
-            new = nn.Parameter(rows(g["name"], old.detach()).requires_grad_(True))
+            new = nn.Parameter(rows(name, old.detach()).requires_grad_(True))
             if state is not None:
-                state["exp_avg"] = moments(g["name"], state["exp_avg"])
-                state["exp_avg_sq"] = moments(g["name"], state["exp_avg_sq"])
+                state["exp_avg"] = moments(name, state["exp_avg"])
+                state["exp_avg_sq"] = moments(name, state["exp_avg_sq"])
                 self.optimizer.state[new] = state
             g["params"][0] = new
-            setattr(self, attr_of[g["name"]], new)
+            setattr(self, attr_of[name], new)
+            tables = [(n, a) for n, a in tables if n != name]
+        for name, attr in tables:
+            old = getattr(self, attr)
+            new = rows(name, old.detach())
+            if isinstance(old, nn.Parameter):
+                new = nn.Parameter(new, requires_grad=old.requires_grad)
+            elif old.requires_grad:
+                new.requires_grad_(True)
+            setattr(self, attr, new)
 
     def prune_points(self, mask: torch.Tensor) -> None:
         """Remove the Gaussians where ``mask`` is True (gaussian_model.py:452-468)."""
@@ -104,7 +137,8 @@ class DensifyMixin:
         self.max_radii2D = self.max_radii2D[keep]
 
     def _append(self, new: Dict[str, torch.Tensor]) -> None:
-        """Concatenate new Gaussians (zero Adam moments) and reset the statistics (gaussian_model.py:470-527)."""
+        """Concatenate new Gaussians (zero Adam moments) and reset the statistics (gaussian_model.py:470-527).
+        ``new`` holds the GROUPS rows and, for the ROW_TABLES the model has, their rows."""
         self._rewrite(lambda n, t: torch.cat((t, new[n]), dim=0),
                       lambda n, m: torch.cat((m, torch.zeros_like(new[n])), dim=0))
         P, dev = self._xyz.shape[0], self._xyz.device
@@ -113,11 +147,12 @@ class DensifyMixin:
         self.max_radii2D = torch.zeros((P,), device=dev)
 
     def replace_tensor_to_optimizer(self, tensor: torch.Tensor, name: str) -> Dict[str, torch.Tensor]:
-        """Swap one parameter for ``tensor`` with zeroed moments (gaussian_model.py:420-433)."""
-        attr_of = dict(GROUPS)
+        """Swap one per-Gaussian parameter for ``tensor`` with zeroed moments (gaussian_model.py:420-433).  A name
+        that is not a per-Gaussian group changes nothing and returns {}."""
+        attr_of = dict(GROUPS + ROW_TABLES)
         out = {}
         for g in self.optimizer.param_groups:
-            if g["name"] != name:
+            if g.get("name") != name or name not in attr_of:
                 continue
             old = g["params"][0]
             state = self.optimizer.state.pop(old, None)
@@ -136,6 +171,17 @@ class DensifyMixin:
         op = torch.minimum(self.get_opacity, torch.full_like(self.get_opacity, 0.01))
         self.replace_tensor_to_optimizer(torch.log(op / (1 - op)), "opacity")
 
+    def _new_table_rows(self, parent_rows: Callable[[torch.Tensor], torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """Rows of the ROW_TABLES the model has for Gaussians made from ``parent_rows(table)``: the feature field
+        copies the parents' rows, the view counts start at zero."""
+        out = {}
+        for name, attr in ROW_TABLES:
+            t = self._row_table(attr)
+            if t is not None:
+                rows = parent_rows(t.detach())
+                out[name] = torch.zeros_like(rows) if name == "times" else rows
+        return out
+
     # ---- statistics + densification --------------------------------------------------------------------------
     def add_densification_stats(self, viewspace_point_tensor: torch.Tensor, update_filter: torch.Tensor) -> None:
         """Accumulate the screen-space positional gradient norm of the visible Gaussians (gaussian_model.py:608-612).
@@ -148,7 +194,8 @@ class DensifyMixin:
         """Duplicate small Gaussians with a large positional gradient (gaussian_model.py:563-586)."""
         small = self.get_scaling.max(dim=1).values <= self.percent_dense * scene_extent
         sel = (torch.norm(grads, dim=-1) >= grad_threshold) & small
-        self._append({name: getattr(self, attr).detach()[sel] for name, attr in GROUPS})
+        new = {name: getattr(self, attr).detach()[sel] for name, attr in GROUPS}
+        self._append(dict(new, **self._new_table_rows(lambda t: t[sel])))
         return int(sel.sum())
 
     def densify_and_split(self, grads: torch.Tensor, grad_threshold: float, scene_extent: float, N: int = 2) -> int:
@@ -168,7 +215,7 @@ class DensifyMixin:
             "xyz": torch.bmm(rots, samples.unsqueeze(-1)).squeeze(-1) + rep(self._xyz),
             "f_dc": rep(self._features_dc), "f_rest": rep(self._features_rest), "opacity": rep(self._opacity),
             "scaling": torch.log(self.get_scaling[sel].detach().repeat(N, 1) / (0.8 * N)),
-            "rotation": rep(self._rotation)})
+            "rotation": rep(self._rotation), **self._new_table_rows(rep)})
         self.prune_points(torch.cat((sel, torch.zeros(N * k, dtype=torch.bool, device=dev))))
         return k
 

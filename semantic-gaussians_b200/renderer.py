@@ -16,12 +16,19 @@ render_batch(..., differentiable_depth=True) also return, from the same pass,
 with gradients (to means3D through z and through the blend weights, to opacity, scales / rotations or cov3D, and
 the screen-space points).  No background term: the normalised depth is E / A.clamp_min(eps).  "depth" stays the
 reference's non-differentiable median depth.
+
+Addition: render_with_features() / render_with_features_batch() train colour and a per-Gaussian feature field
+together: one geometry pass and one binning per view produce render()'s dict (plus "expected_depth" / "alpha" under
+``differentiable_depth``) and "features" (c, H, W), the image of a (P, c) table over its background, bitwise what
+render() and render_chn() give.  One backward carries both losses.  ``viewspace_points.grad`` holds the sum of both
+images' screen-space gradients, so the densification statistic (add_densification_stats) sees the feature loss too.
 """
 import math
 
 import torch
 
 from . import channel_rasterization as chn_rasterize
+from .rasterizer import rasterize_joint_batch
 from .rgbd_rasterization import GaussianRasterizationSettings, GaussianRasterizer
 from .sh_utils import eval_sh
 
@@ -191,3 +198,59 @@ def render_chn_batch(cameras, pc, pipe, bg_color: torch.Tensor, scaling_modifier
     views inside the kernels — one (P, C) feature-gradient buffer for the whole batch."""
     return _render_batch("chn", cameras, pc, pipe, bg_color, scaling_modifier, num_channels, override_color,
                          override_shape, foreground, world_rotate)
+
+
+def render_with_features(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, features: torch.Tensor,
+                         bg_features: torch.Tensor, scaling_modifier=1.0, override_color=None, override_shape=None,
+                         foreground=None, world_rotate=None, *, differentiable_depth=False):
+    """render()'s dict (render_with_depth()'s under ``differentiable_depth``) plus "features" (c, H, W): the image of
+    ``features`` (P, c) over ``bg_features`` (c), from the same geometry pass and binning as the RGB image.  Gradients
+    reach ``features``, the Gaussian parameters and ``viewspace_points`` from both images (module docstring)."""
+    return render_with_features_batch([viewpoint_camera], pc, pipe, bg_color, features, bg_features,
+                                      scaling_modifier=scaling_modifier, override_color=override_color,
+                                      override_shape=override_shape, foreground=foreground, world_rotate=world_rotate,
+                                      differentiable_depth=differentiable_depth)[0]
+
+
+def render_with_features_batch(cameras, pc, pipe, bg_color: torch.Tensor, features: torch.Tensor,
+                               bg_features: torch.Tensor, scaling_modifier=1.0, override_color=None,
+                               override_shape=None, foreground=None, world_rotate=None, *, differentiable_depth=False):
+    """``[render_with_features(cam, ...) for cam in cameras]`` through the batched native calls, split at the native
+    batch limit as render_batch is."""
+    cameras = list(cameras)
+    if not cameras:
+        return []
+    if override_color is None and pipe.convert_shs_python:  # python SH -> colours depend on the camera
+        groups = [[cam] for cam in cameras]
+    else:
+        groups = [cameras]
+    res = []
+    for group in groups:
+        pts0, common0, call = _prepare(group[0], pc, pipe, scaling_modifier, override_color, override_shape,
+                                       foreground, world_rotate)
+        settings, points = [], []
+        for i, cam in enumerate(group):
+            common = dict(common0, tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5),
+                          viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform,
+                          campos=cam.camera_center)
+            if override_shape is None and (int(cam.image_height), int(cam.image_width)) != (
+                    common0["image_height"], common0["image_width"]):
+                raise ValueError("the views of a batch must share the image size")
+            settings.append(GaussianRasterizationSettings(bg=bg_color, debug=pipe.debug, **common))
+            if i == 0:
+                points.append(pts0)
+            else:
+                p = torch.zeros_like(pts0, requires_grad=True) + 0
+                p.retain_grad()
+                points.append(p)
+        outs = rasterize_joint_batch(call["means3D"], points, call["opacities"], settings, features, bg_features,
+                                     shs=call["shs"], colors_precomp=call["colors_precomp"], scales=call["scales"],
+                                     rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
+                                     expected_depth=differentiable_depth)
+        for pts, o in zip(points, outs):
+            d = {"render": o[0], "viewspace_points": pts, "visibility_filter": o[1] > 0, "radii": o[1],
+                 "depth": o[2], "features": o[3]}
+            if differentiable_depth:
+                d.update(expected_depth=o[4], alpha=o[5])
+            res.append(d)
+    return res
