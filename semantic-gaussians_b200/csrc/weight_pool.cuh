@@ -101,15 +101,15 @@ struct AlphaRgb {
 
 // ------------------------------------------------------------------ host entry points
 //   weight_pool_build         enqueue the alpha pass of one view into its slot (no sync), so that a batch enqueues
-//                             the alpha passes of all its views before the one sync that checks their pools
+//                             the alpha passes of all its views before the one sync that checks their pools (with
+//                             `rgb`, the same walk is also the view's RGB blend; a rebuild after an overflow runs
+//                             without it, since the walk and so the RGB outputs do not depend on the pool)
 //   weight_pool_settle        one stream sync, then the pool check of views [0, V) (of those with only[v], when
 //                             given); a view whose pool overflowed is grown and built again; fills pv[v]
 //   weight_rows_for_backward  pv[v] of every view with R > 0: the slot its forward filled, else rebuilt (all misses
 //                             under one sync)
 //   weight_pool_release       empties the slots of views [0, V): a lift keeps nothing for a backward
 // The blend kernels take the PoolView and look up nothing.
-//                             (with `rgb`, the walk is also the view's RGB blend; a rebuild after an overflow runs
-//                             the plain pass, since the walk and so the RGB outputs do not depend on the pool)
 int weight_pool_build(sgb_ctx* ctx, const ViewState& w, cudaStream_t s, const AlphaRgb* rgb = nullptr);
 int weight_pool_settle(sgb_ctx* ctx, int V, const ViewState* vw, PoolView* pv, cudaStream_t s,
                        const bool* only = nullptr);

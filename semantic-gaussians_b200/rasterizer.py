@@ -98,34 +98,49 @@ def _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, 
 
 def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opacity, scales, rotations,
              scale_modifier, cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, num_channels,
-             want_exp_alpha=False):
+             want_exp_alpha=False, features=None, bg_features=None):
     """V = len(cams) views of the same Gaussians through sgb_forward_geometry_batch / sgb_forward_render_batch_ext:
-    one stream sync for all instance counts, one for all weight-pool checks.  Returns the marshalled inputs (None for
-    an empty scene), which _backward takes, and the per-view lists (R, color, radii, geometry state, binning state,
-    image state, depth or None, expected depth or None, alpha or None)."""
+    one stream sync for all instance counts, one for all weight-pool checks.  With ``features`` (P, c) over
+    ``bg_features`` (c), the render call is sgb_forward_render_joint_batch, which also renders that table from the same
+    geometry and binning (the RGB render: ``want_depth`` and num_channels = 3).  Returns the marshalled inputs (None
+    for an empty scene), which _backward takes, and the per-view lists (R, color, radii, geometry state, binning
+    state, image state, depth or None, expected depth or None, alpha or None), followed with ``features`` by the
+    per-view list of feature images."""
     lib = _lib.load()
     V = len(cams)
+    if features is not None and (features.ndim != 2 or features.size(0) != means3D.size(0) or features.size(1) < 1):
+        raise ValueError(f"features must be (P, c) with P = {means3D.size(0)} and c >= 1, got {tuple(features.shape)}")
     if means3D.ndimension() == 2 and means3D.size(0) == 0 and means3D.is_cuda:
         # Empty scene: the reference never enters the native forward (rasterize_points.cu:84) and
         # returns its zero-initialised outputs — zeros, not the background.
         dev = means3D.device
         z = lambda *shape, dtype=torch.float32: [torch.zeros(shape, dtype=dtype, device=dev) for _ in range(V)]
+        feat = () if features is None else (z(features.size(1), image_height, image_width),)
         return None, ([0] * V, z(num_channels, image_height, image_width), z(0, dtype=torch.int32),
                       z(0, dtype=torch.uint8), z(0, dtype=torch.uint8),
                       z(lib.sgb_image_bytes(image_width, image_height), dtype=torch.uint8),
                       z(1, image_height, image_width) if want_depth else None,
                       z(1, image_height, image_width) if want_exp_alpha else None,
-                      z(1, image_height, image_width) if want_exp_alpha else None)
+                      z(1, image_height, image_width) if want_exp_alpha else None, *feat)
     native = _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                           image_height, image_width, sh, degree, prefiltered, debug, num_channels)
-    inp, cameras, _, dev = native
+    inp, cameras, keep, dev = native
     P, H, W, Cn = inp.P, inp.H, inp.W, inp.C
+    if features is not None:
+        c = features.size(1)
+        feats = _f32(features, dev, "features")
+        bg_feats = _f32(bg_features, dev, "bg_features").reshape(-1)
+        if bg_feats.numel() != c:
+            raise ValueError(f"bg_features has {bg_feats.numel()} entries, the feature table {c} channels")
+        keep["features"], keep["bg_features"] = feats, bg_feats
     u8 = dict(dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         stream, ctx = _stream_ctx(dev)
         # every pixel / every radius is written by the kernels: no zero fill (the reference's
         # torch::full of out_color is pure waste, rasterize_points.cu:73)
         out_color = [torch.empty((Cn, H, W), dtype=torch.float32, device=dev) for _ in range(V)]
+        out_feat = None if features is None else [torch.empty((c, H, W), dtype=torch.float32, device=dev)
+                                                  for _ in range(V)]
         plane = lambda want: [torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(V)] if want else None
         out_depth, out_exp_depth, out_alpha = plane(want_depth), plane(want_exp_alpha), plane(want_exp_alpha)
         radii = [torch.empty((P,), dtype=torch.int32, device=dev) for _ in range(V)]
@@ -139,10 +154,27 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
         _lib.check(lib.sgb_forward_geometry_batch(ctx, C.byref(inp), V, cameras, geom_p, radii_p, R, stream),
                    f"{what} (geometry)")
         binning = [torch.empty((lib.sgb_binning_bytes(R[v]),), **u8) for v in range(V)]
-        _lib.check(lib.sgb_forward_render_batch_ext(ctx, C.byref(inp), V, cameras, R, geom_p, _ptrs(binning), img_p,
-                                                    radii_p, color_p, depth_p, exp_p, alpha_p, stream),
-                   f"{what} (render)")
-    return native, (list(R), out_color, radii, geom, binning, img, out_depth, out_exp_depth, out_alpha)
+        common = (ctx, C.byref(inp), V, cameras, R, geom_p, _ptrs(binning), img_p, radii_p, color_p, depth_p, exp_p,
+                  alpha_p)
+        if features is None:
+            rc = lib.sgb_forward_render_batch_ext(*common, stream)
+        else:
+            rc = lib.sgb_forward_render_joint_batch(*common, feats.data_ptr(), c, bg_feats.data_ptr(), _ptrs(out_feat),
+                                                    stream)
+        _lib.check(rc, f"{what} (render)")
+    feat = () if features is None else (out_feat,)
+    return native, (list(R), out_color, radii, geom, binning, img, out_depth, out_exp_depth, out_alpha, *feat)
+
+
+def _forward_joint(what: str, cams, background, means3D, colors, opacity, scales, rotations, scale_modifier,
+                   cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, features, bg_features,
+                   want_exp_alpha=False):
+    """_forward of the RGB render (median depth always) with ``features``: (native, per-view lists as _forward's
+    without features, per-view feature images, the marshalled (features, bg_features) or None for an empty scene)."""
+    native, (*lists, feat) = _forward(True, what, cams, background, means3D, colors, opacity, scales, rotations,
+                                      scale_modifier, cov3D_precomp, image_height, image_width, sh, degree,
+                                      prefiltered, debug, 3, want_exp_alpha, features, bg_features)
+    return native, tuple(lists), feat, None if native is None else (native[2]["features"], native[2]["bg_features"])
 
 
 def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_depth=None, dL_dalpha=None,
@@ -154,7 +186,7 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_
     features accumulate over the views in ONE (P, C) buffer inside the kernels; on the SH path the per-view RGB
     gradient is an input of that view's SH backward (backward.cu:385-386), so every view gets its own (P, 3).
     ``joint`` = (features, bg_features, per-view dL/d feature image) runs sgb_backward_joint_batch instead (the forward
-    was _forward_joint) and appends the (P, c) feature gradient to the result."""
+    was _forward with ``features``) and appends the (P, c) feature gradient to the result."""
     lib = _lib.load()
     inp, cameras, _, dev = native
     V, P, M, Cn = len(dL_dout), inp.P, inp.M, inp.C
@@ -198,58 +230,6 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_
         return ([g_means2D], *summed, *tail)
     # the shared colour buffer already holds the sum over the views
     return (list(g_means2D.unbind(0)), *[t if t is g_colors and shared else t.sum(0) for t in summed], *tail)
-
-
-def _forward_joint(what: str, cams, background, means3D, colors, opacity, scales, rotations, scale_modifier,
-                   cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, features, bg_features,
-                   want_exp_alpha=False):
-    """_forward of the RGB render (median depth always, expected depth / alpha with ``want_exp_alpha``) that also
-    renders the (P, c) table ``features`` over ``bg_features`` through sgb_forward_render_joint_batch: one geometry
-    call and one binning per view for both images.  Returns (native, per-view lists as _forward's) plus the per-view
-    list of (c, H, W) feature images, and the marshalled (features, bg_features) the backward takes."""
-    lib = _lib.load()
-    V = len(cams)
-    if features.ndim != 2 or features.size(0) != means3D.size(0) or features.size(1) < 1:
-        raise ValueError(f"features must be (P, c) with P = {means3D.size(0)} and c >= 1, got {tuple(features.shape)}")
-    c = features.size(1)
-    if means3D.ndimension() == 2 and means3D.size(0) == 0 and means3D.is_cuda:
-        native, res = _forward(True, what, cams, background, means3D, colors, opacity, scales, rotations,
-                               scale_modifier, cov3D_precomp, image_height, image_width, sh, degree, prefiltered,
-                               debug, 3, want_exp_alpha)
-        dev = means3D.device
-        return native, res, [torch.zeros((c, image_height, image_width), device=dev) for _ in range(V)], None
-    native = _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                          image_height, image_width, sh, degree, prefiltered, debug, 3)
-    inp, cameras, keep, dev = native
-    feats = _f32(features, dev, "features")
-    bg_feats = _f32(bg_features, dev, "bg_features").reshape(-1)
-    if bg_feats.numel() != c:
-        raise ValueError(f"bg_features has {bg_feats.numel()} entries, the feature table {c} channels")
-    keep["features"], keep["bg_features"] = feats, bg_feats
-    P, H, W = inp.P, inp.H, inp.W
-    u8 = dict(dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        stream, ctx = _stream_ctx(dev)
-        out_color = [torch.empty((3, H, W), dtype=torch.float32, device=dev) for _ in range(V)]
-        out_feat = [torch.empty((c, H, W), dtype=torch.float32, device=dev) for _ in range(V)]
-        plane = lambda want: [torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(V)] if want else None
-        out_depth, out_exp_depth, out_alpha = plane(True), plane(want_exp_alpha), plane(want_exp_alpha)
-        radii = [torch.empty((P,), dtype=torch.int32, device=dev) for _ in range(V)]
-        geom = [torch.empty((lib.sgb_geometry_bytes(P),), **u8) for _ in range(V)]
-        img = [torch.empty((lib.sgb_image_bytes(W, H),), **u8) for _ in range(V)]
-        R = (C.c_int64 * V)()
-        geom_p, radii_p, img_p = _ptrs(geom), _ptrs(radii), _ptrs(img)
-        exp_p, alpha_p = (_ptrs(out_exp_depth), _ptrs(out_alpha)) if want_exp_alpha else (None, None)
-        _lib.check(lib.sgb_forward_geometry_batch(ctx, C.byref(inp), V, cameras, geom_p, radii_p, R, stream),
-                   f"{what} (geometry)")
-        binning = [torch.empty((lib.sgb_binning_bytes(R[v]),), **u8) for v in range(V)]
-        _lib.check(lib.sgb_forward_render_joint_batch(ctx, C.byref(inp), V, cameras, R, geom_p, _ptrs(binning), img_p,
-                                                      radii_p, _ptrs(out_color), _ptrs(out_depth), exp_p, alpha_p,
-                                                      feats.data_ptr(), c, bg_feats.data_ptr(), _ptrs(out_feat),
-                                                      stream),
-                   f"{what} (render)")
-    return (native, (list(R), out_color, radii, geom, binning, img, out_depth, out_exp_depth, out_alpha), out_feat,
-            (feats, bg_feats))
 
 
 def _mark_visible(means3D, viewmatrix, projmatrix):
@@ -362,6 +342,85 @@ def _dump(args, path):
         pass
 
 
+def _native_args(is_chn, joint, settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
+                 cov3Ds_precomp):
+    """The _make_inputs arguments of the views in ``settings_list`` (settings of the chn variant when ``is_chn``, of
+    the rgbd variant otherwise; ``joint``: of a render that also draws a feature table)."""
+    rs = settings_list[0]
+    # the rgbd extension's _C takes no debug flag (rgbd_rasterization/__init__.py:57-80); the joint render honours it
+    return (_cameras(settings_list), rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
+            cov3Ds_precomp, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.prefiltered,
+            (is_chn or joint) and rs.debug, rs.num_channels if is_chn else 3)
+
+
+def _views_forward(ctx, is_chn, what, settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
+                   cov3Ds_precomp, expected_depth, features=None, bg_features=None):
+    """Forward of _RasterizeGaussians (one view), _RasterizeGaussiansBatch and, with ``features``, _RasterizeJointBatch:
+    (*colors, *radii[, *depths][, *feature images][, *expected depths, *alphas]), the depths for the rgbd variant (not
+    ``is_chn``), the feature images with ``features``, the last two when ``expected_depth``."""
+    joint = features is not None
+    native, (R, color, radii, geom, binning, img, depth, exp_depth, alpha, *feat) = _forward(
+        not is_chn, what, *_native_args(is_chn, joint, settings_list, means3D, sh, colors_precomp, opacities, scales,
+                                        rotations, cov3Ds_precomp),
+        want_exp_alpha=expected_depth, features=features, bg_features=bg_features)
+    # the backward reuses the marshalled inputs; they also hold any contiguous copies their pointers refer to
+    ctx.settings_list, ctx.R, ctx.native, ctx.expected_depth = settings_list, R, native, expected_depth
+    ctx.is_chn = is_chn
+    ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features, *radii,
+                          *geom, *binning, *img)
+    ctx.mark_non_differentiable(*radii)
+    outs = (*color, *radii)
+    if not is_chn:
+        ctx.mark_non_differentiable(*depth)  # no median-depth gradient in the reference (backward ignores it)
+        outs += (*depth,)
+    if joint:
+        outs += (*feat[0],)
+    if not (expected_depth or joint):
+        return outs
+    # gradients arrive as None for outputs the loss does not use: a loss on E / A alone runs no colour gradient
+    # through the blend, one on the colours alone runs the plain backward, and a loss on one image of a joint render
+    # leaves the other's gradient None
+    ctx.set_materialize_grads(False)
+    return outs + (*exp_depth, *alpha) if expected_depth else outs
+
+
+def _views_backward(ctx, what, saved, grad_outputs):
+    """(per-view list of dL_dmeans2D, then the gradients of means3D, sh, colors_precomp, opacities, scales,
+    rotations, cov3Ds_precomp[, features] summed over the views; None for an absent optional input).  ``saved`` is
+    ctx.saved_tensors, ``grad_outputs`` the gradients of _views_forward's outputs."""
+    V = len(ctx.settings_list)
+    colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features, *states = saved
+    radii, geom, binning, img = states[:V], states[V:2 * V], states[2 * V:3 * V], states[3 * V:]
+    rs = ctx.settings_list[0]
+    H, W = rs.image_height, rs.image_width
+    # without materialised gradients, an output the loss does not use has a None gradient: zeros
+    fill = lambda gs, ch: [torch.zeros((ch, H, W), device=means3D.device) if g is None else g for g in gs]
+    grad_colors = fill(grad_outputs[:V], rs.num_channels if ctx.is_chn else 3)
+    k = (2 if ctx.is_chn else 3) * V  # past the colours, radii and depths
+    g_feat = g_exp = g_alpha = None
+    if features is not None:
+        g_feat, k = fill(grad_outputs[k:k + V], features.size(1)), k + V
+    if ctx.expected_depth:
+        g_exp, g_alpha = grad_outputs[k:k + V], grad_outputs[k + V:k + 2 * V]
+        g_exp = None if all(g is None for g in g_exp) else fill(g_exp, 1)
+        g_alpha = None if all(g is None for g in g_alpha) else fill(g_alpha, 1)
+    native = ctx.native
+    if native is None:  # empty scene: the forward marshalled nothing
+        native = _make_inputs(*_native_args(ctx.is_chn, features is not None, ctx.settings_list, means3D, sh,
+                                            colors_precomp, means3D, scales, rotations, cov3Ds_precomp))
+    joint = None
+    if features is not None:  # the table and background as the forward marshalled them (as given: empty scene)
+        keep = native[2]
+        joint = (keep.get("features", features), keep.get("bg_features", bg_features), g_feat)
+    g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot, *g_features = _backward(
+        what, native, radii, grad_colors, geom, ctx.R, binning, img, g_exp, g_alpha, joint)
+
+    def present(t, g):  # absent optional inputs were empty tensors; they get no gradient
+        return g if t.numel() != 0 else None
+    return (g_means2D, g_means3D, present(sh, g_sh), present(colors_precomp, g_colors), g_opac,
+            present(scales, g_scales), present(rotations, g_rot), present(cov3Ds_precomp, g_cov3D), *g_features)
+
+
 def make_module(variant: str):
     """Build (GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians,
     _RasterizeGaussians, _C) for variant 'chn' or 'rgbd'."""
@@ -399,74 +458,14 @@ def make_module(variant: str):
             prefiltered: bool
             debug: bool
 
-    def native_args(settings_list, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
-        """The _make_inputs arguments of the views in ``settings_list``."""
-        rs = settings_list[0]
-        # the rgbd extension's _C takes no debug flag (rgbd_rasterization/__init__.py:57-80)
-        return (_cameras(settings_list), rs.bg, means3D, colors_precomp, opacities, scales, rotations,
-                rs.scale_modifier, cov3Ds_precomp, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.prefiltered,
-                is_chn and rs.debug, rs.num_channels if is_chn else 3)
-
-    def views_forward(ctx, what, settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
-                      cov3Ds_precomp, expected_depth):
-        """Forward of _RasterizeGaussians (one view) and _RasterizeGaussiansBatch:
-        (*colors, *radii[, *depths][, *expected depths, *alphas]), the last two when ``expected_depth``."""
-        native, (R, color, radii, geom, binning, img, depth, exp_depth, alpha) = _forward(
-            not is_chn, what, *native_args(settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
-                                           cov3Ds_precomp), want_exp_alpha=expected_depth)
-        # the backward reuses the marshalled inputs; they also hold any contiguous copies their pointers refer to
-        ctx.settings_list, ctx.R, ctx.native, ctx.expected_depth = settings_list, R, native, expected_depth
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, *radii, *geom, *binning,
-                              *img)
-        ctx.mark_non_differentiable(*radii)
-        outs = (*color, *radii)
-        if not is_chn:
-            ctx.mark_non_differentiable(*depth)  # no median-depth gradient in the reference (backward ignores it)
-            outs += (*depth,)
-        if not expected_depth:
-            return outs
-        # gradients arrive as None for outputs the loss does not use: a loss on E / A alone runs no colour gradient
-        # through the blend, and one on the colours alone runs the plain backward
-        ctx.set_materialize_grads(False)
-        return outs + (*exp_depth, *alpha)
-
-    def views_backward(ctx, what, saved, grad_outputs):
-        """(per-view list of dL_dmeans2D, then the gradients of means3D, sh, colors_precomp, opacities, scales,
-        rotations, cov3Ds_precomp summed over the views; None for an absent optional input).  ``saved`` is
-        ctx.saved_tensors, ``grad_outputs`` the gradients of views_forward's outputs."""
-        V = len(ctx.settings_list)
-        grad_colors, g_exp, g_alpha = grad_outputs[:V], None, None
-        if ctx.expected_depth:
-            k = (2 if is_chn else 3) * V
-            g_exp, g_alpha = grad_outputs[k:k + V], grad_outputs[k + V:k + 2 * V]
-            rs = ctx.settings_list[0]
-            H, W = rs.image_height, rs.image_width
-            fill = lambda gs, *shape: [torch.zeros(shape, device=saved[1].device) if g is None else g for g in gs]
-            grad_colors = fill(grad_colors, rs.num_channels if is_chn else 3, H, W)
-            g_exp = None if all(g is None for g in g_exp) else fill(g_exp, 1, H, W)
-            g_alpha = None if all(g is None for g in g_alpha) else fill(g_alpha, 1, H, W)
-        colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, *states = saved
-        radii, geom, binning, img = states[:V], states[V:2 * V], states[2 * V:3 * V], states[3 * V:]
-        native = ctx.native
-        if native is None:  # empty scene: the forward marshalled nothing
-            native = _make_inputs(*native_args(ctx.settings_list, means3D, sh, colors_precomp, means3D, scales,
-                                               rotations, cov3Ds_precomp))
-        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = _backward(
-            what, native, radii, grad_colors, geom, ctx.R, binning, img, g_exp, g_alpha)
-
-        def present(t, g):  # absent optional inputs were empty tensors; they get no gradient
-            return g if t.numel() != 0 else None
-        return (g_means2D, g_means3D, present(sh, g_sh), present(colors_precomp, g_colors), g_opac,
-                present(scales, g_scales), present(rotations, g_rot), present(cov3Ds_precomp, g_cov3D))
-
     class _RasterizeGaussians(torch.autograd.Function):
         @staticmethod
         def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                     raster_settings, expected_depth=False):
             rs = raster_settings
             try:
-                return views_forward(ctx, "rasterize_gaussians", [rs], means3D, sh, colors_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp, expected_depth)
+                return _views_forward(ctx, is_chn, "rasterize_gaussians", [rs], means3D, sh, colors_precomp, opacities,
+                                      scales, rotations, cov3Ds_precomp, expected_depth)
             except Exception:
                 if rs.debug:
                     args = [rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
@@ -480,12 +479,13 @@ def make_module(variant: str):
         def backward(ctx, *grad_outputs):
             saved = ctx.saved_tensors
             try:
-                g_means2D, g_means3D, *grads = views_backward(ctx, "rasterize_gaussians_backward", saved,
-                                                              grad_outputs)
+                g_means2D, g_means3D, *grads = _views_backward(ctx, "rasterize_gaussians_backward", saved,
+                                                               grad_outputs)
             except Exception:
                 rs = ctx.settings_list[0]
                 if rs.debug:
-                    colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, radii, geom, binning, img = saved
+                    colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, _, _, radii, geom, binning, img = \
+                        saved
                     args = [rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier,
                             cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_outputs[0], sh,
                             rs.sh_degree, rs.campos, geom, ctx.R[0], binning, img]
@@ -511,13 +511,13 @@ def make_module(variant: str):
         def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings_list,
                     expected_depth, *means2D):
             _check_batch_settings(settings_list)
-            return views_forward(ctx, "rasterize_gaussians_batch", settings_list, means3D, sh, colors_precomp,
-                                 opacities, scales, rotations, cov3Ds_precomp, expected_depth)
+            return _views_forward(ctx, is_chn, "rasterize_gaussians_batch", settings_list, means3D, sh, colors_precomp,
+                                  opacities, scales, rotations, cov3Ds_precomp, expected_depth)
 
         @staticmethod
         def backward(ctx, *grad_outputs):
-            g_means2D, *grads = views_backward(ctx, "rasterize_gaussians_backward_batch", ctx.saved_tensors,
-                                               grad_outputs)
+            g_means2D, *grads = _views_backward(ctx, "rasterize_gaussians_backward_batch", ctx.saved_tensors,
+                                                grad_outputs)
             return (*grads, None, None, *g_means2D)
 
     def rasterize_gaussians_batch(means3D, means2D_list, opacities, settings_list, shs=None, colors_precomp=None,
@@ -584,51 +584,13 @@ class _RasterizeJointBatch(torch.autograd.Function):
     def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, features, bg_features,
                 settings_list, expected_depth, *means2D):
         _check_batch_settings(settings_list)
-        rs = settings_list[0]
-        native, (R, color, radii, geom, binning, img, depth, exp_depth, alpha), feat, marshalled = _forward_joint(
-            "rasterize_joint_batch", _cameras(settings_list), rs.bg, means3D, colors_precomp, opacities, scales,
-            rotations, rs.scale_modifier, cov3Ds_precomp, rs.image_height, rs.image_width, sh, rs.sh_degree,
-            rs.prefiltered, rs.debug, features, bg_features, want_exp_alpha=expected_depth)
-        ctx.settings_list, ctx.R, ctx.native, ctx.expected_depth = settings_list, R, native, expected_depth
-        ctx.marshalled, ctx.c = marshalled, features.size(1)
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features,
-                              *radii, *geom, *binning, *img)
-        ctx.mark_non_differentiable(*radii, *depth)
-        # a loss on one of the images leaves the other's gradient None: it is zero-filled in the backward
-        ctx.set_materialize_grads(False)
-        outs = (*color, *radii, *depth, *feat)
-        return outs + (*exp_depth, *alpha) if expected_depth else outs
+        return _views_forward(ctx, False, "rasterize_joint_batch", settings_list, means3D, sh, colors_precomp,
+                              opacities, scales, rotations, cov3Ds_precomp, expected_depth, features, bg_features)
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        V = len(ctx.settings_list)
-        colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features, *states = \
-            ctx.saved_tensors
-        radii, geom, binning, img = states[:V], states[V:2 * V], states[2 * V:3 * V], states[3 * V:]
-        rs = ctx.settings_list[0]
-        H, W, dev = rs.image_height, rs.image_width, means3D.device
-        fill = lambda gs, ch: [torch.zeros((ch, H, W), device=dev) if g is None else g for g in gs]
-        g_rgb, g_feat = fill(grad_outputs[:V], 3), fill(grad_outputs[3 * V:4 * V], ctx.c)
-        g_exp = g_alpha = None
-        if ctx.expected_depth:
-            g_exp, g_alpha = grad_outputs[4 * V:5 * V], grad_outputs[5 * V:6 * V]
-            g_exp = None if all(g is None for g in g_exp) else fill(g_exp, 1)
-            g_alpha = None if all(g is None for g in g_alpha) else fill(g_alpha, 1)
-        native, marshalled = ctx.native, ctx.marshalled
-        if native is None:  # empty scene: the forward marshalled nothing
-            native = _make_inputs(_cameras(ctx.settings_list), rs.bg, means3D, colors_precomp, means3D, scales,
-                                  rotations, rs.scale_modifier, cov3Ds_precomp, H, W, sh, rs.sh_degree, rs.prefiltered,
-                                  rs.debug, 3)
-            marshalled = (features, bg_features)
-        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot, g_features = _backward(
-            "rasterize_joint_backward_batch", native, radii, g_rgb, geom, ctx.R, binning, img, g_exp, g_alpha,
-            joint=(*marshalled, g_feat))
-
-        def present(t, g):  # absent optional inputs were empty tensors; they get no gradient
-            return g if t.numel() != 0 else None
-        return (g_means3D, present(sh, g_sh), present(colors_precomp, g_colors), g_opac, present(scales, g_scales),
-                present(rotations, g_rot), present(cov3Ds_precomp, g_cov3D), g_features, None, None, None,
-                *g_means2D)
+        g_means2D, *grads = _views_backward(ctx, "rasterize_joint_backward_batch", ctx.saved_tensors, grad_outputs)
+        return (*grads, None, None, None, *g_means2D)
 
 
 def rasterize_joint_batch(means3D, means2D_list, opacities, settings_list, features, bg_features, shs=None,

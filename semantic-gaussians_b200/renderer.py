@@ -24,6 +24,7 @@ render() and render_chn() give.  One backward carries both losses.  ``viewspace_
 images' screen-space gradients, so the densification statistic (add_densification_stats) sees the feature loss too.
 """
 import math
+from functools import partial
 
 import torch
 
@@ -85,6 +86,34 @@ def _prepare(viewpoint_camera, pc, pipe, scaling_modifier, override_color, overr
     return screenspace_points, common, call
 
 
+def _prepare_views(cameras, pc, pipe, scaling_modifier, override_color, override_shape, foreground, world_rotate,
+                   make_settings):
+    """_prepare for a batch of cameras: the Gaussian-side tensors are prepared ONCE (the reference's per-view loop,
+    eval_segmentation.py:146-157 / fusion.py:106-120, re-evaluates the activations for every view).  Returns the
+    rasterizer settings of every camera (``make_settings(**common)`` with the camera's fields), its screen-space
+    points (camera 0's from _prepare, the others new zero tensors like them) and the call arguments."""
+    pts0, common0, call = _prepare(cameras[0], pc, pipe, scaling_modifier, override_color, override_shape, foreground,
+                                   world_rotate)
+    settings, points = [], []
+    for i, cam in enumerate(cameras):
+        common = dict(common0, tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5),
+                      viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform, campos=cam.camera_center)
+        if override_shape is None and (int(cam.image_height), int(cam.image_width)) != (common0["image_height"],
+                                                                                        common0["image_width"]):
+            raise ValueError("the views of a batch must share the image size")
+        settings.append(make_settings(**common))
+        if i == 0:
+            points.append(pts0)
+        else:
+            p = torch.zeros_like(pts0, requires_grad=True) + 0
+            try:
+                p.retain_grad()
+            except Exception:
+                pass
+            points.append(p)
+    return settings, points, call
+
+
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            override_shape=None, foreground=None, world_rotate=None):
     """RGB + median depth (rgbd rasterizer).  Background tensor (bg_color) must be on the GPU."""
@@ -131,9 +160,8 @@ def render_chn(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modif
 
 def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_channels, override_color, override_shape,
                   foreground, world_rotate, differentiable_depth=False):
-    """Shared body of render_batch / render_chn_batch: the Gaussian-side tensors are prepared ONCE (the reference's
-    per-view loop, eval_segmentation.py:146-157 / fusion.py:106-120, re-evaluates the activations for every view),
-    the views go through the batched native calls (rasterizer.rasterize_gaussians_batch)."""
+    """Shared body of render_batch / render_chn_batch: the views go through _prepare_views and the batched native
+    calls (rasterizer.rasterize_gaussians_batch)."""
     cameras = list(cameras)
     if not cameras:
         return []
@@ -144,31 +172,15 @@ def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_ch
         return [single(cam, pc, pipe, bg_color, scaling_modifier=scaling_modifier, override_color=override_color,
                        override_shape=override_shape, foreground=foreground, world_rotate=world_rotate)
                 for cam in cameras]
-    pts0, common0, call = _prepare(cameras[0], pc, pipe, scaling_modifier, override_color, override_shape, foreground,
-                                   world_rotate)
-    mod = chn_rasterize if variant == "chn" else None
-    settings, points = [], []
-    for i, cam in enumerate(cameras):
-        common = dict(common0, tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5),
-                      viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform, campos=cam.camera_center)
-        if override_shape is None and (int(cam.image_height), int(cam.image_width)) != (common0["image_height"],
-                                                                                        common0["image_width"]):
-            raise ValueError("the views of a batch must share the image size")
-        if variant == "chn":
-            settings.append(mod.GaussianRasterizationSettings(bg=bg_color, debug=bool(getattr(pipe, "debug", False)),
-                                                              num_channels=num_channels, **common))
-        else:
-            settings.append(GaussianRasterizationSettings(bg=bg_color, debug=pipe.debug, **common))
-        if i == 0:
-            points.append(pts0)
-        else:
-            p = torch.zeros_like(pts0, requires_grad=True) + 0
-            try:
-                p.retain_grad()
-            except Exception:
-                pass
-            points.append(p)
-    Rast = mod.GaussianRasterizer if variant == "chn" else GaussianRasterizer
+    if variant == "chn":
+        make_settings = partial(chn_rasterize.GaussianRasterizationSettings, bg=bg_color,
+                                debug=bool(getattr(pipe, "debug", False)), num_channels=num_channels)
+        Rast = chn_rasterize.GaussianRasterizer
+    else:
+        make_settings = partial(GaussianRasterizationSettings, bg=bg_color, debug=pipe.debug)
+        Rast = GaussianRasterizer
+    settings, points, call = _prepare_views(cameras, pc, pipe, scaling_modifier, override_color, override_shape,
+                                            foreground, world_rotate, make_settings)
     outs = Rast.rasterize_batch(call["means3D"], points, call["opacities"], settings, shs=call["shs"],
                                 colors_precomp=call["colors_precomp"], scales=call["scales"],
                                 rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
@@ -226,23 +238,9 @@ def render_with_features_batch(cameras, pc, pipe, bg_color: torch.Tensor, featur
         groups = [cameras]
     res = []
     for group in groups:
-        pts0, common0, call = _prepare(group[0], pc, pipe, scaling_modifier, override_color, override_shape,
-                                       foreground, world_rotate)
-        settings, points = [], []
-        for i, cam in enumerate(group):
-            common = dict(common0, tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5),
-                          viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform,
-                          campos=cam.camera_center)
-            if override_shape is None and (int(cam.image_height), int(cam.image_width)) != (
-                    common0["image_height"], common0["image_width"]):
-                raise ValueError("the views of a batch must share the image size")
-            settings.append(GaussianRasterizationSettings(bg=bg_color, debug=pipe.debug, **common))
-            if i == 0:
-                points.append(pts0)
-            else:
-                p = torch.zeros_like(pts0, requires_grad=True) + 0
-                p.retain_grad()
-                points.append(p)
+        settings, points, call = _prepare_views(group, pc, pipe, scaling_modifier, override_color, override_shape,
+                                                foreground, world_rotate,
+                                                partial(GaussianRasterizationSettings, bg=bg_color, debug=pipe.debug))
         outs = rasterize_joint_batch(call["means3D"], points, call["opacities"], settings, features, bg_features,
                                      shs=call["shs"], colors_precomp=call["colors_precomp"], scales=call["scales"],
                                      rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
