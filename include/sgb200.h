@@ -278,6 +278,51 @@ int sgb_backward_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V,
                              const float* const* dL_dfeature_pix /* [V] (c, H, W) */,
                              float* dL_dfeatures /* (P, c) */, void* stream);
 
+/* ---- camera gradients: what camera pose refinement needs from the backward.
+ *
+ * sgb_backward_batch_cam is sgb_backward_batch_ext, and sgb_backward_joint_batch_cam sgb_backward_joint_batch, that
+ * also write, for every view v with cam_grads non-NULL, the gradient of the loss with respect to that view's camera:
+ * cam_grads[v].dL_dviewmatrix [16], dL_dprojmatrix [16] and dL_dcampos [3], device fp32, in the element order of
+ * sgb_camera's viewmatrix / projmatrix / campos.  The geometry backward of the view forms every visible Gaussian's
+ * contribution (through the view-space centre and the perspective Jacobian, the projected centre, the expected
+ * depth when dL_dexp_depth / dL_dalpha are given, and the SH view direction when shs is given) and sums them:
+ *   - fp64 partials per CTA in ctx scratch, then one fixed-order pass that writes fp32 once: no float atomics, so
+ *     identical calls give bitwise-identical camera gradients;
+ *   - the outputs are overwritten, not accumulated; entries the forward never reads (viewmatrix 3, 7, 11, 15 and
+ *     projmatrix 2, 6, 10, 14) are exactly 0, and so is dL_dcampos without shs; a view with P = 0 or no instance
+ *     gets zeros;
+ *   - focal lengths and tan(fov) are constants (no intrinsics gradient);
+ *   - a joint call's one geometry backward per view carries both images' losses, and so does its camera gradient;
+ *   - every per-Gaussian gradient is bitwise what the same call with cam_grads = NULL writes.
+ * Besides the argument rules of the call it extends, a null pointer in any entry, or one pointer used for two
+ * outputs, returns SGB_E_INVALID before anything is enqueued.  The camera-gradient reduction is timed inside the
+ * geom_bwd profiler stage. */
+typedef struct sgb_camera_grads {
+    float* dL_dviewmatrix;  /* [16] device, element order of sgb_camera.viewmatrix */
+    float* dL_dprojmatrix;  /* [16] device */
+    float* dL_dcampos;      /* [3]  device */
+} sgb_camera_grads;
+
+int sgb_backward_batch_cam(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                           const int64_t* num_rendered, const int32_t* const* radii,
+                           const void* const* geometry_states, const void* const* binning_states,
+                           const void* const* image_states, const float* const* dL_dpix,
+                           const float* const* dL_dexp_depth /* NULL or [V] */,
+                           const float* const* dL_dalpha /* NULL or [V] */,
+                           const sgb_view_grads* grads /* [V] */,
+                           const sgb_camera_grads* cam_grads /* NULL or [V], host array */, void* stream);
+int sgb_backward_joint_batch_cam(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                 const int64_t* num_rendered, const int32_t* const* radii,
+                                 const void* const* geometry_states, const void* const* binning_states,
+                                 const void* const* image_states, const float* const* dL_dpix /* [V] (3, H, W) */,
+                                 const float* const* dL_dexp_depth /* NULL or [V] */,
+                                 const float* const* dL_dalpha /* NULL or [V] */,
+                                 const sgb_view_grads* grads /* [V] */, const float* features /* (P, c) */,
+                                 int32_t c, const float* bg_features /* (c) */,
+                                 const float* const* dL_dfeature_pix /* [V] (c, H, W) */,
+                                 float* dL_dfeatures /* (P, c) */,
+                                 const sgb_camera_grads* cam_grads /* NULL or [V], host array */, void* stream);
+
 /* Identity of the build: "<version> src:<sha256 prefix of csrc/ + include/>" (set by build.py; bench.py prints
  * it so that a stale prebuilt library cannot be mistaken for the sources next to it). */
 const char* sgb_build_id(void);

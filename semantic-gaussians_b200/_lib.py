@@ -46,6 +46,11 @@ class Camera(C.Structure):
                 ("tan_fovx", C.c_float), ("tan_fovy", C.c_float)]
 
 
+class CameraGrads(C.Structure):
+    """sgb_camera_grads: one view's camera-gradient outputs of an sgb_backward_*_cam call."""
+    _fields_ = [("dL_dviewmatrix", C.c_void_p), ("dL_dprojmatrix", C.c_void_p), ("dL_dcampos", C.c_void_p)]
+
+
 MAX_BATCH = 8
 
 
@@ -90,6 +95,7 @@ EXPORTS = (
     "sgb_sparse_conv_half_backward_weight", "sgb_voxel_feature_loss_forward", "sgb_voxel_feature_loss_backward",
     "sgb_nearest", "sgb_decoded_semantic_head", "sgb_decoded_semantic_head_workspace_bytes",
     "sgb_decoded_feature_logits", "sgb_forward_render_joint_batch", "sgb_backward_joint_batch",
+    "sgb_backward_batch_cam", "sgb_backward_joint_batch_cam",
 )
 
 _lib = None
@@ -144,6 +150,9 @@ def load() -> C.CDLL:
         lib.sgb_backward_joint_batch.argtypes = [vp, C.POINTER(ViewInputs), i32, C.POINTER(Camera), C.POINTER(i64),
                                                  pvp, pvp, pvp, pvp, pvp, pvp, pvp, C.POINTER(ViewGrads), vp, i32, vp,
                                                  pvp, vp, vp]
+        lib.sgb_backward_batch_cam.argtypes = lib.sgb_backward_batch_ext.argtypes[:-1] + [C.POINTER(CameraGrads), vp]
+        lib.sgb_backward_joint_batch_cam.argtypes = (lib.sgb_backward_joint_batch.argtypes[:-1] +
+                                                     [C.POINTER(CameraGrads), vp])
         lib.sgb_build_id.restype = C.c_char_p
         lib.sgb_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
         lib.sgb_state_field.argtypes = [C.c_char_p, i32, i64, i32, i32, vp, vp, vp, vp, vp]

@@ -108,6 +108,7 @@ void sgb_ctx_destroy(sgb_ctx* c) {
     if (c->misc.p) cudaFree(c->misc.p);
     if (c->work.p) cudaFree(c->work.p);
     if (c->depth_grad.p) cudaFree(c->depth_grad.p);
+    if (c->cam_partial.p) cudaFree(c->cam_partial.p);
     if (c->lift_state.p) cudaFree(c->lift_state.p);
     if (c->lift_bin.p) cudaFree(c->lift_bin.p);
     delete c->pools;
@@ -160,8 +161,8 @@ uint64_t sgb_ctx_launch_count(const sgb_ctx* c, int library_calls) {
 
 size_t sgb_ctx_scratch_bytes(const sgb_ctx* c) {
     if (!c) return 0;
-    return c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap + c->lift_state.cap +
-           c->lift_bin.cap + c->pools->bytes();
+    return c->geom.cap + c->bin.cap + c->misc.cap + c->work.cap + c->depth_grad.cap + c->cam_partial.cap +
+           c->lift_state.cap + c->lift_bin.cap + c->pools->bytes();
 }
 
 size_t sgb_geometry_bytes(int32_t P) { return GeomView::carve(nullptr, P > 0 ? P : 1).bytes; }
@@ -314,6 +315,27 @@ static int check_backward(const char* what, bool joint, sgb_ctx* ctx, const sgb_
     return SGB_OK;
 }
 
+// The camera-gradient outputs of a _cam backward call (NULL: none): every pointer set, no pointer used twice.
+static int check_camera_grads(const char* what, int32_t V, const sgb_camera_grads* cg) {
+    if (!cg) return SGB_OK;
+    const float* seen[3 * SGB_MAX_BATCH];
+    int n = 0;
+    for (int v = 0; v < V; v++)
+        for (const float* q : {cg[v].dL_dviewmatrix, cg[v].dL_dprojmatrix, cg[v].dL_dcampos}) {
+            if (!q) {
+                set_error("%s: null camera-gradient output of view %d", what, v);
+                return SGB_E_INVALID;
+            }
+            for (int i = 0; i < n; i++)
+                if (seen[i] == q) {
+                    set_error("%s: one camera-gradient buffer is given twice (view %d)", what, v);
+                    return SGB_E_INVALID;
+                }
+            seen[n++] = q;
+        }
+    return SGB_OK;
+}
+
 // Per view: binning once, then the images on its lists.  The POOLED image is the feature image `fin` when given, else
 // the image of `in`.  When its C > 4, its alpha pass builds the weight pool (for a joint call the same walk is the RGB
 // blend of `in`, median depth and expected depth / alpha included), and after the one pool check of the batch the
@@ -377,14 +399,21 @@ static int forward_render_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sg
 // (sgb200.h).  Then per view: the pooled image's chain (or small-C blend) backward, for a joint call the RGB blend
 // backward, and ONE geometry backward with the RGB colour gradient.  The blend that carries the dL_dexp_depth /
 // dL_dalpha terms is the one of `in`.  All blend backwards add into the same dL_dmeans2D / dL_dconic / dL_dopacity.
+// cam_grads (NULL or [V]): the geometry backward of view v also writes view v's camera gradient.
 static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sgb_view_inputs* fin, int V,
                          const sgb_camera* cams, const int64_t* num_rendered, const int32_t* const* radii,
                          const void* const* geometry_states, const void* const* binning_states,
                          const void* const* image_states, const float* const* dL_dpix,
                          const float* const* dL_dexp_depth, const float* const* dL_dalpha, const sgb_view_grads* grads,
-                         const float* const* dL_dfeature_pix, float* dL_dfeatures, cudaStream_t s) {
+                         const float* const* dL_dfeature_pix, float* dL_dfeatures, const sgb_camera_grads* cam_grads,
+                         cudaStream_t s) {
     if (in.P == 0) {
         if (ctx->feature_grad_event) SGB_CUDA(cudaEventRecord(ctx->feature_grad_event, s));
+        for (int v = 0; cam_grads && v < V; v++) {  // no Gaussian: a zero camera gradient
+            SGB_CUDA(cudaMemsetAsync(cam_grads[v].dL_dviewmatrix, 0, 16 * sizeof(float), s));
+            SGB_CUDA(cudaMemsetAsync(cam_grads[v].dL_dprojmatrix, 0, 16 * sizeof(float), s));
+            SGB_CUDA(cudaMemsetAsync(cam_grads[v].dL_dcampos, 0, 3 * sizeof(float), s));
+        }
         return SGB_OK;
     }
     const sgb_view_inputs& pooled = fin ? *fin : in;
@@ -404,6 +433,10 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sgb_view
         rc = ctx->depth_grad.ensure(sizeof(float) * (size_t)in.P);
         if (rc) return rc;
         dL_ddepth = (float*)ctx->depth_grad.p;
+    }
+    if (cam_grads) {
+        rc = ctx->cam_partial.ensure(camera_grad_partial_bytes(in.P));
+        if (rc) return rc;
     }
     // the small-C blend backward of image w of view v; the one of `in` carries the depth terms
     auto blend_backward = [&](const ViewState& w, int v, const float* dL_dout, float* dL_dcolor, bool depth) -> int {
@@ -442,10 +475,10 @@ static int backward_impl(sgb_ctx* ctx, const sgb_view_inputs& in, const sgb_view
         }
         const float* cov3D = in.cov3D_precomp ? in.cov3D_precomp : vw[v].g.cov3D;  // rasterizer_impl.cu:417
         StageTimer t(ctx, ST_GEOM_BWD, s);
-        ctx->launches += 1;
+        ctx->launches += cam_grads ? 2 : 1;
         // a view without instances has no blend and so no depth gradient
         rc = launch_geom_backward(vw[v].in, vw[v].g, radii[v], cov3D, gr.dL_dcolors, gr, vw[v].R > 0 ? dL_ddepth : nullptr,
-                                  s);
+                                  cam_grads ? &cam_grads[v] : nullptr, (double*)ctx->cam_partial.p, s);
         if (rc) return rc;
     }
     return SGB_OK;
@@ -529,12 +562,23 @@ int sgb_backward_batch_ext(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, c
                            const void* const* image_states, const float* const* dL_dpix,
                            const float* const* dL_dexp_depth, const float* const* dL_dalpha,
                            const sgb_view_grads* grads, void* stream) {
+    return sgb_backward_batch_cam(ctx, in, V, cams, num_rendered, radii, geometry_states, binning_states, image_states,
+                                  dL_dpix, dL_dexp_depth, dL_dalpha, grads, nullptr, stream);
+}
+
+int sgb_backward_batch_cam(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                           const int64_t* num_rendered, const int32_t* const* radii,
+                           const void* const* geometry_states, const void* const* binning_states,
+                           const void* const* image_states, const float* const* dL_dpix,
+                           const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                           const sgb_view_grads* grads, const sgb_camera_grads* cam_grads, void* stream) {
     int rc = check_backward("sgb_backward_batch", false, ctx, in, V, cams, num_rendered, radii, geometry_states,
                             binning_states, image_states, dL_dpix, dL_dexp_depth, dL_dalpha, grads, nullptr, 0,
                             nullptr, nullptr, nullptr);
+    if (!rc) rc = check_camera_grads("sgb_backward_batch", V, cam_grads);
     if (rc) return rc;
     return backward_impl(ctx, *in, nullptr, V, cams, num_rendered, radii, geometry_states, binning_states, image_states,
-                         dL_dpix, dL_dexp_depth, dL_dalpha, grads, nullptr, nullptr, (cudaStream_t)stream);
+                         dL_dpix, dL_dexp_depth, dL_dalpha, grads, nullptr, nullptr, cam_grads, (cudaStream_t)stream);
 }
 
 // ---- colour and a feature table through one geometry pass and one binning per view ---------------------------
@@ -561,13 +605,28 @@ int sgb_backward_joint_batch(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V,
                              const float* const* dL_dexp_depth, const float* const* dL_dalpha,
                              const sgb_view_grads* grads, const float* features, int32_t c, const float* bg_features,
                              const float* const* dL_dfeature_pix, float* dL_dfeatures, void* stream) {
+    return sgb_backward_joint_batch_cam(ctx, in, V, cams, num_rendered, radii, geometry_states, binning_states,
+                                        image_states, dL_dpix, dL_dexp_depth, dL_dalpha, grads, features, c,
+                                        bg_features, dL_dfeature_pix, dL_dfeatures, nullptr, stream);
+}
+
+int sgb_backward_joint_batch_cam(sgb_ctx* ctx, const sgb_view_inputs* in, int32_t V, const sgb_camera* cams,
+                                 const int64_t* num_rendered, const int32_t* const* radii,
+                                 const void* const* geometry_states, const void* const* binning_states,
+                                 const void* const* image_states, const float* const* dL_dpix,
+                                 const float* const* dL_dexp_depth, const float* const* dL_dalpha,
+                                 const sgb_view_grads* grads, const float* features, int32_t c,
+                                 const float* bg_features, const float* const* dL_dfeature_pix, float* dL_dfeatures,
+                                 const sgb_camera_grads* cam_grads, void* stream) {
     int rc = check_backward("sgb_backward_joint_batch", true, ctx, in, V, cams, num_rendered, radii, geometry_states,
                             binning_states, image_states, dL_dpix, dL_dexp_depth, dL_dalpha, grads, features, c,
                             bg_features, dL_dfeature_pix, dL_dfeatures);
+    if (!rc) rc = check_camera_grads("sgb_backward_joint_batch", V, cam_grads);
     if (rc) return rc;
     const sgb_view_inputs fin = feature_inputs(*in, features, c, bg_features);
     return backward_impl(ctx, *in, &fin, V, cams, num_rendered, radii, geometry_states, binning_states, image_states,
-                         dL_dpix, dL_dexp_depth, dL_dalpha, grads, dL_dfeature_pix, dL_dfeatures, (cudaStream_t)stream);
+                         dL_dpix, dL_dexp_depth, dL_dalpha, grads, dL_dfeature_pix, dL_dfeatures, cam_grads,
+                         (cudaStream_t)stream);
 }
 
 // ---- lifting feature maps onto the Gaussians by their blend weights ------------------------------------------

@@ -167,6 +167,7 @@ struct sgb_ctx {
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
     sgb::Scratch work;     // work-item counters of the persistent kernels (chn_dfeature.cu)
     sgb::Scratch depth_grad;  // [P] dL/d(view-space z) of the view being differentiated (expected-depth backward)
+    sgb::Scratch cam_partial; // per-CTA fp64 camera-gradient partials of the view being differentiated
     sgb::Scratch lift_state;  // sgb_lift_batch: geometry state, radii and image state of every view of the call
     sgb::Scratch lift_bin;    // sgb_lift_batch: binning states of the views
     // What the ctx carries from one call to the next: the weight rows of the C-channel blend, one pool per view of a
@@ -227,8 +228,12 @@ int launch_blend_backward(const sgb_view_inputs& in, GeomView g, BinView b, ImgV
                           float* dL_dcolors, const float* dL_dexp_depth, const float* dL_dalpha, float* dL_ddepth,
                           cudaStream_t s);
 // C > 4 blend: weight_pool.cuh (the alpha pass and the pools it fills) and chn_blend.cuh (the contraction stages).
+// cam_grads non-NULL: also this view's camera gradient (sgb200.h sgb_camera_grads), through cam_partial, a device
+// buffer of camera_grad_partial_bytes(in.P) that the call's two kernels use in stream order.
 int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* radii, const float* cov3D,
-                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, const float* dL_ddepth, cudaStream_t s);
+                         const float* dL_dcolor_rgb, const sgb_view_grads& gr, const float* dL_ddepth,
+                         const sgb_camera_grads* cam_grads, double* cam_partial, cudaStream_t s);
+size_t camera_grad_partial_bytes(int32_t P);
 
 // ------------------------------------------------------------------ device helpers
 #ifdef __CUDACC__

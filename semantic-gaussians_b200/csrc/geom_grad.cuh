@@ -30,13 +30,24 @@
 namespace sgb {
 namespace geomgrad {
 
+// What project_grad knows on the way that the camera gradient needs (camera_grad below): dL/dt of the view-space
+// centre, dL/dA of A = J W, the Jacobian's scale and clamped evaluation point, and dL/d(homogeneous projected centre).
+struct ProjectTerms {
+    float gt[3];
+    float gA[2][3];
+    float ax, ay, u, v;
+    float g_hom[4];
+};
+
 // ---------------------------------------------------------------- conic / centre -> world mean and covariance
 // view, proj: column-major 4x4 as the reference passes them (element (row i, col j) at [4 j + i]).
 // g_conic = (dL/dK_xx, dL/dK_xy [halved], dL/dK_yy), g_ndc = dL/d(projected centre in NDC units).
 // out_mean[3] = dL/dp (both paths summed), out_cov[6] = dL/d(S_xx, S_xy, S_xz, S_yy, S_yz, S_zz).
+// terms: NULL, or filled for camera_grad.  Filling it only copies values already computed (no value computed for
+// out_mean / out_cov gains a use that could change how it is rounded).
 SGB_HD void project_grad(const float p[3], const float cov6[6], const float* view, const float* proj, float fx, float fy,
                          float tan_x, float tan_y, const float g_conic[3], const float g_ndc[2], float out_mean[3],
-                         float out_cov[6]) {
+                         float out_cov[6], ProjectTerms* terms = nullptr) {
     // view-space centre, frustum clamp of the Jacobian's evaluation point
     float t[3];
 #pragma unroll
@@ -120,6 +131,56 @@ SGB_HD void project_grad(const float p[3], const float cov6[6], const float* vie
         const float via_ndc = iw * (g_ndc[0] * proj[4 * j + 0] + g_ndc[1] * proj[4 * j + 1] - proj[4 * j + 3] * along);
         out_mean[j] = via_cov + via_ndc;
     }
+    if (terms) {
+#pragma unroll
+        for (int i = 0; i < 3; i++) {
+            terms->gt[i] = gt[i];
+            terms->gA[0][i] = gA[0][i];
+            terms->gA[1][i] = gA[1][i];
+        }
+        terms->ax = ax;
+        terms->ay = ay;
+        terms->u = u;
+        terms->v = v;
+        // ndc_k = hom_k iw, iw = 1 / (hom_w + 1e-7)
+        terms->g_hom[0] = g_ndc[0] * iw;
+        terms->g_hom[1] = g_ndc[1] * iw;
+        terms->g_hom[2] = 0.f;
+        terms->g_hom[3] = -along * iw;
+    }
+}
+
+// ---------------------------------------------------------------- one Gaussian's camera gradient
+// ADDS this Gaussian's contribution to dL/dview[16], dL/dproj[16] (element order of view / proj above) and, with
+// g_campos (the SH colour's view-direction term, colour_grad's campos_grad) non-NULL, dL/dcampos[3].  t = W p + t0:
+//     via t:        dL/dW_ij += gt_i p_j,  dL/dt0_i += gt_i
+//     via A = J W:  A_0j = ax (W_0j - u W_2j), A_1j = ay (W_1j - v W_2j) with the clamped u, v held as the forward holds
+//                   them (their dependence on t is gt's)
+//     via z = t_2:  dL/dW_2j += gz p_j, dL/dt0_2 += gz   (expected depth; gz = 0 without it)
+//     via hom = Proj (p, 1):  dL/dProj_kj += dL/dhom_k p_j
+// Entries the forward never reads (view row 3, proj row 2) receive nothing.  Focal lengths and tan(fov) are constants.
+SGB_HD void camera_grad(const float p[3], const ProjectTerms& k, float gz, const float* g_campos, float dview[16],
+                        float dproj[16], float dcampos[3]) {
+    const float ph[4] = {p[0], p[1], p[2], 1.f};
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+#pragma unroll
+        for (int i = 0; i < 3; i++) dview[4 * j + i] += k.gt[i] * ph[j];
+        dview[4 * j + 2] += gz * ph[j];
+        dproj[4 * j + 0] += k.g_hom[0] * ph[j];
+        dproj[4 * j + 1] += k.g_hom[1] * ph[j];
+        dproj[4 * j + 3] += k.g_hom[3] * ph[j];
+    }
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+        dview[4 * j + 0] += k.ax * k.gA[0][j];
+        dview[4 * j + 1] += k.ay * k.gA[1][j];
+        dview[4 * j + 2] -= k.ax * k.u * k.gA[0][j] + k.ay * k.v * k.gA[1][j];
+    }
+    if (g_campos) {
+#pragma unroll
+        for (int i = 0; i < 3; i++) dcampos[i] += g_campos[i];
+    }
 }
 
 // ---------------------------------------------------------------- world covariance -> scale, rotation
@@ -191,9 +252,11 @@ SGB_HD void sh_basis(int deg, float x, float y, float z, float Y[16], float dY[1
 }
 
 // sh: the Gaussian's [max_coeffs][3] coefficients; g_rgb: dL/d(colour), already zeroed where the forward clamped.
-// Writes out_sh[(deg+1)^2][3]; ADDS the view-direction path to mean_grad[3].
+// Writes out_sh[(deg+1)^2][3]; ADDS the view-direction path to mean_grad[3].  campos_grad: NULL, or receives the same
+// path for the camera centre, v = p - campos: -(what mean_grad gains), written as d <d, g> / |v| - g / |v| so that the
+// product added to mean_grad keeps its single use (and so its rounding).
 SGB_HD void colour_grad(int deg, const float p[3], const float* campos, const float* sh, const float g_rgb[3],
-                        float* out_sh, float mean_grad[3]) {
+                        float* out_sh, float mean_grad[3], float* campos_grad = nullptr) {
     const float v[3] = {p[0] - campos[0], p[1] - campos[1], p[2] - campos[2]};
     const float len2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
     const float ilen = 1.f / sqrtf(len2);
@@ -218,6 +281,11 @@ SGB_HD void colour_grad(int deg, const float p[3], const float* campos, const fl
     const float radial = d[0] * gd[0] + d[1] * gd[1] + d[2] * gd[2];
 #pragma unroll
     for (int i = 0; i < 3; i++) mean_grad[i] += (gd[i] - d[i] * radial) * ilen;
+    if (campos_grad) {
+        const float radial_ilen = radial * ilen;
+#pragma unroll
+        for (int i = 0; i < 3; i++) campos_grad[i] = d[i] * radial_ilen - gd[i] * ilen;
+    }
 }
 
 }  // namespace geomgrad

@@ -178,7 +178,7 @@ def _forward_joint(what: str, cams, background, means3D, colors, opacity, scales
 
 
 def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_depth=None, dL_dalpha=None,
-              joint=None):
+              joint=None, cam_grad=False):
     """sgb_backward_batch_ext over the views of one forward: ``native`` is what _make_inputs returned for it, the other
     arguments are per-view lists of its states and of dL/dout (dL/d expected depth and dL/d alpha: per-view lists of
     (1, H, W) planes, or None when absent).  Returns (the per-view list of dL_dmeans2D, then the
@@ -186,7 +186,9 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_
     features accumulate over the views in ONE (P, C) buffer inside the kernels; on the SH path the per-view RGB
     gradient is an input of that view's SH backward (backward.cu:385-386), so every view gets its own (P, 3).
     ``joint`` = (features, bg_features, per-view dL/d feature image) runs sgb_backward_joint_batch instead (the forward
-    was _forward with ``features``) and appends the (P, c) feature gradient to the result."""
+    was _forward with ``features``) and appends the (P, c) feature gradient to the result.  ``cam_grad`` runs the
+    ``_cam`` entry point of the same call and appends the (V, 35) camera gradients: per view dL/dviewmatrix (16),
+    dL/dprojmatrix (16) and dL/dcampos (3) in the element order of the marshalled (contiguous) camera tensors."""
     lib = _lib.load()
     inp, cameras, _, dev = native
     V, P, M, Cn = len(dL_dout), inp.P, inp.M, inp.C
@@ -201,6 +203,7 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_
     gouts = [_f32(g, dev, "dL_dout_color") for g in dL_dout]
     planes = lambda gs, name: None if gs is None else [_f32(g, dev, name).reshape(inp.H, inp.W) for g in gs]
     g_exp, g_alpha = planes(dL_dexp_depth, "dL_dexp_depth"), planes(dL_dalpha, "dL_dalpha")
+    g_cam = torch.zeros((V, 35), **z) if cam_grad else None   # an empty scene has a zero camera gradient
     if P != 0:
         # view v's slice of every buffer, by address; the shared colour buffer is the same for all views
         base = [t.data_ptr() for t in bufs]
@@ -214,18 +217,25 @@ def _backward(what: str, native, radii, dL_dout, geom, R, binning, img, dL_dexp_
             common = (ctx, C.byref(inp), V, cameras, num_rendered, _ptrs(radii), _ptrs(geom), _ptrs(binning),
                       _ptrs(img), _ptrs(gouts), None if g_exp is None else _ptrs(g_exp),
                       None if g_alpha is None else _ptrs(g_alpha), grads)
+            cams = ()
+            if cam_grad:
+                b = g_cam.data_ptr()
+                cams = (_per_view(_lib.CameraGrads, [_lib.CameraGrads(b + 140 * v, b + 140 * v + 64, b + 140 * v + 128)
+                                                     for v in range(V)]),)
             if joint is None:
-                _lib.check(lib.sgb_backward_batch_ext(*common, stream), what)
+                fn = lib.sgb_backward_batch_cam if cam_grad else lib.sgb_backward_batch_ext
+                _lib.check(fn(*common, *cams, stream), what)
             else:
                 feats, bg_feats, gfeat = joint
                 g_features = torch.zeros(feats.shape, **z)
                 gfeat = [_f32(g, dev, "dL_dfeatures_image") for g in gfeat]
-                _lib.check(lib.sgb_backward_joint_batch(*common, feats.data_ptr(), feats.size(1), bg_feats.data_ptr(),
-                                                        _ptrs(gfeat), g_features.data_ptr(), stream), what)
+                fn = lib.sgb_backward_joint_batch_cam if cam_grad else lib.sgb_backward_joint_batch
+                _lib.check(fn(*common, feats.data_ptr(), feats.size(1), bg_feats.data_ptr(), _ptrs(gfeat),
+                              g_features.data_ptr(), *cams, stream), what)
     elif joint is not None:
         g_features = torch.zeros(joint[0].shape, **z)
     summed = [g_colors, g_opacity, g_means3D, g_cov3D, g_sh, g_scales, g_rot]
-    tail = () if joint is None else (g_features,)
+    tail = (() if joint is None else (g_features,)) + (() if g_cam is None else (g_cam,))
     if V == 1:
         return ([g_means2D], *summed, *tail)
     # the shared colour buffer already holds the sum over the views
@@ -384,9 +394,16 @@ def _views_forward(ctx, is_chn, what, settings_list, means3D, sh, colors_precomp
     return outs + (*exp_depth, *alpha) if expected_depth else outs
 
 
-def _views_backward(ctx, what, saved, grad_outputs):
+def _camera_tensors(settings_list):
+    """The camera tensors of the views, passed to the autograd functions as inputs so that they can receive
+    gradients: viewmatrix, projmatrix, campos of each view in turn."""
+    return [t for rs in settings_list for t in (rs.viewmatrix, rs.projmatrix, rs.campos)]
+
+
+def _views_backward(ctx, what, saved, grad_outputs, cam_grad=False):
     """(per-view list of dL_dmeans2D, then the gradients of means3D, sh, colors_precomp, opacities, scales,
-    rotations, cov3Ds_precomp[, features] summed over the views; None for an absent optional input).  ``saved`` is
+    rotations, cov3Ds_precomp[, features] summed over the views; None for an absent optional input), followed by the
+    gradients of _camera_tensors(ctx.settings_list): computed with ``cam_grad``, else None.  ``saved`` is
     ctx.saved_tensors, ``grad_outputs`` the gradients of _views_forward's outputs."""
     V = len(ctx.settings_list)
     colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features, *states = saved
@@ -412,13 +429,22 @@ def _views_backward(ctx, what, saved, grad_outputs):
     if features is not None:  # the table and background as the forward marshalled them (as given: empty scene)
         keep = native[2]
         joint = (keep.get("features", features), keep.get("bg_features", bg_features), g_feat)
-    g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot, *g_features = _backward(
-        what, native, radii, grad_colors, geom, ctx.R, binning, img, g_exp, g_alpha, joint)
+    g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot, *tail = _backward(
+        what, native, radii, grad_colors, geom, ctx.R, binning, img, g_exp, g_alpha, joint, cam_grad)
+    g_features = tail[:1] if features is not None else []
+    cams = _camera_tensors(ctx.settings_list)
+    if cam_grad:
+        # buffer order is the contiguous copy's, i.e. the tensor's own logical order (see _f32)
+        g_cam = tail[-1]
+        g_cams = [g_cam[i // 3, (0, 16, 32)[i % 3]:(16, 32, 35)[i % 3]].reshape(t.shape) for i, t in enumerate(cams)]
+    else:
+        g_cams = [None] * len(cams)
 
     def present(t, g):  # absent optional inputs were empty tensors; they get no gradient
         return g if t.numel() != 0 else None
     return (g_means2D, g_means3D, present(sh, g_sh), present(colors_precomp, g_colors), g_opac,
-            present(scales, g_scales), present(rotations, g_rot), present(cov3Ds_precomp, g_cov3D), *g_features)
+            present(scales, g_scales), present(rotations, g_rot), present(cov3Ds_precomp, g_cov3D), *g_features,
+            *g_cams)
 
 
 def make_module(variant: str):
@@ -461,7 +487,8 @@ def make_module(variant: str):
     class _RasterizeGaussians(torch.autograd.Function):
         @staticmethod
         def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                    raster_settings, expected_depth=False):
+                    raster_settings, expected_depth=False, *camera):
+            # camera: _camera_tensors([raster_settings]), inputs only so that they can receive gradients
             rs = raster_settings
             try:
                 return _views_forward(ctx, is_chn, "rasterize_gaussians", [rs], means3D, sh, colors_precomp, opacities,
@@ -480,7 +507,7 @@ def make_module(variant: str):
             saved = ctx.saved_tensors
             try:
                 g_means2D, g_means3D, *grads = _views_backward(ctx, "rasterize_gaussians_backward", saved,
-                                                               grad_outputs)
+                                                               grad_outputs, any(ctx.needs_input_grad[10:]))
             except Exception:
                 rs = ctx.settings_list[0]
                 if rs.debug:
@@ -492,14 +519,16 @@ def make_module(variant: str):
                     _dump(args + [rs.debug] if is_chn else args, "snapshot_bw.dump")
                     print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
                 raise
-            return (g_means3D, g_means2D[0], *grads, None, None)
+            *grads, g_view, g_proj, g_campos = grads
+            return (g_means3D, g_means2D[0], *grads, None, None, g_view, g_proj, g_campos)
 
     def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                             raster_settings, *, expected_depth=False):
         """The reference's rasterize_gaussians; with ``expected_depth`` the outputs gain the expected depth
         E = sum_i w_i z_i and the accumulated opacity A = sum_i w_i, (1, H, W) each and differentiable (C <= 4)."""
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                         cov3Ds_precomp, raster_settings, expected_depth)
+                                         cov3Ds_precomp, raster_settings, expected_depth,
+                                         *_camera_tensors([raster_settings]))
 
     class _RasterizeGaussiansBatch(torch.autograd.Function):
         """V views of the same Gaussians in one native call each way (the reference loops over
@@ -509,16 +538,18 @@ def make_module(variant: str):
 
         @staticmethod
         def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings_list,
-                    expected_depth, *means2D):
+                    expected_depth, *means2D_camera):
+            # means2D_camera: the V screen-space tensors, then _camera_tensors(settings_list)
             _check_batch_settings(settings_list)
             return _views_forward(ctx, is_chn, "rasterize_gaussians_batch", settings_list, means3D, sh, colors_precomp,
                                   opacities, scales, rotations, cov3Ds_precomp, expected_depth)
 
         @staticmethod
         def backward(ctx, *grad_outputs):
+            V = len(ctx.settings_list)
             g_means2D, *grads = _views_backward(ctx, "rasterize_gaussians_backward_batch", ctx.saved_tensors,
-                                                grad_outputs)
-            return (*grads, None, None, *g_means2D)
+                                                grad_outputs, any(ctx.needs_input_grad[9 + V:]))
+            return (*grads[:-3 * V], None, None, *g_means2D, *grads[-3 * V:])
 
     def rasterize_gaussians_batch(means3D, means2D_list, opacities, settings_list, shs=None, colors_precomp=None,
                                   scales=None, rotations=None, cov3D_precomp=None, expected_depth=False):
@@ -534,7 +565,7 @@ def make_module(variant: str):
             sl = list(settings_list[lo:lo + _lib.MAX_BATCH])
             m2 = list(means2D_list[lo:lo + _lib.MAX_BATCH])
             out = _RasterizeGaussiansBatch.apply(means3D, shs, colors_precomp, opacities, scales, rotations,
-                                                 cov3D_precomp, sl, expected_depth, *m2)
+                                                 cov3D_precomp, sl, expected_depth, *m2, *_camera_tensors(sl))
             V = len(sl)
             per_view = 2 if is_chn else 3
             if expected_depth:
@@ -582,15 +613,18 @@ class _RasterizeJointBatch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, features, bg_features,
-                settings_list, expected_depth, *means2D):
+                settings_list, expected_depth, *means2D_camera):
+        # means2D_camera: the V screen-space tensors, then _camera_tensors(settings_list)
         _check_batch_settings(settings_list)
         return _views_forward(ctx, False, "rasterize_joint_batch", settings_list, means3D, sh, colors_precomp,
                               opacities, scales, rotations, cov3Ds_precomp, expected_depth, features, bg_features)
 
     @staticmethod
     def backward(ctx, *grad_outputs):
-        g_means2D, *grads = _views_backward(ctx, "rasterize_joint_backward_batch", ctx.saved_tensors, grad_outputs)
-        return (*grads, None, None, None, *g_means2D)
+        V = len(ctx.settings_list)
+        g_means2D, *grads = _views_backward(ctx, "rasterize_joint_backward_batch", ctx.saved_tensors, grad_outputs,
+                                            any(ctx.needs_input_grad[11 + V:]))
+        return (*grads[:-3 * V], None, None, None, *g_means2D, *grads[-3 * V:])
 
 
 def rasterize_joint_batch(means3D, means2D_list, opacities, settings_list, features, bg_features, shs=None,
@@ -608,7 +642,7 @@ def rasterize_joint_batch(means3D, means2D_list, opacities, settings_list, featu
         sl = list(settings_list[lo:lo + _lib.MAX_BATCH])
         m2 = list(means2D_list[lo:lo + _lib.MAX_BATCH])
         out = _RasterizeJointBatch.apply(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                         features, bg_features, sl, expected_depth, *m2)
+                                         features, bg_features, sl, expected_depth, *m2, *_camera_tensors(sl))
         V = len(sl)
         for v in range(V):
             results.append(tuple(out[i * V + v] for i in range(per_view)))
