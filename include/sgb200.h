@@ -84,6 +84,15 @@ typedef struct sgb_view_inputs {
     float tan_fovx, tan_fovy;
     int32_t prefiltered;         /* trap if a Gaussian fails the near cull (auxiliary.h:156-160) */
     int32_t debug;               /* synchronise + check after every stage (auxiliary.h:166-173) */
+    /* Anti-aliasing (3DGS's PipelineParams.antialiasing, Mip-Splatting's screen-space filter): 0 = off, 1 = on; any
+     * other value returns SGB_E_INVALID before anything is enqueued.  With C0 the screen covariance before the fixed
+     * 0.3 px^2 dilation and C = C0 + 0.3 I, every blend reads the opacity o h, h = sqrt(max(2.5e-5, det C0 / det C)):
+     * a Gaussian keeps the integral of its undilated footprint at every image size.  Conics, radii, tiles, binning
+     * and depth order are unchanged; the geometry backward carries dL/do = h dL/d(o h) and the covariance term of h
+     * (to means3D, cov3D, scales / rotations and the camera).  Honoured by every call that takes sgb_view_inputs,
+     * sgb_lift_batch included; the backward must be given the forward's value.  This field grew the struct by 4 bytes
+     * (no padding change before it); a zero-initialised struct keeps the behaviour without it. */
+    int32_t antialiasing;
 } sgb_view_inputs;
 
 /* Gradients of one view (all caller-zero-filled, as rasterize_points.cu:157-165 does). */

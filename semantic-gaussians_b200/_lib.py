@@ -30,7 +30,7 @@ class ViewInputs(C.Structure):
         ("rotations", C.c_void_p), ("cov3D_precomp", C.c_void_p), ("viewmatrix", C.c_void_p),
         ("projmatrix", C.c_void_p), ("campos", C.c_void_p),
         ("tan_fovx", C.c_float), ("tan_fovy", C.c_float),
-        ("prefiltered", C.c_int32), ("debug", C.c_int32),
+        ("prefiltered", C.c_int32), ("debug", C.c_int32), ("antialiasing", C.c_int32),
     ]
 
 

@@ -52,6 +52,10 @@ int check_inputs(const sgb_view_inputs& in) {
         set_error("null required input pointer");
         return SGB_E_INVALID;
     }
+    if (in.antialiasing != 0 && in.antialiasing != 1) {
+        set_error("antialiasing must be 0 or 1, got %d", in.antialiasing);
+        return SGB_E_INVALID;
+    }
     return SGB_OK;
 }
 

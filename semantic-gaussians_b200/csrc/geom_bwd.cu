@@ -24,7 +24,10 @@ __host__ __device__ constexpr int cam_slot_entry(int k) {  // index into view (1
 // CAM = false: the per-Gaussian gradients only.  CAM = true: the same per-Gaussian outputs (the same statements), and
 // each CTA also sums its Gaussians' camera terms (geom_grad.cuh camera_grad) in fp64 - over the warp by shuffles in a
 // fixed order, then over the warps in order - and writes one partial per reduction slot to cam_partial[k][blockIdx.x].
-template <bool CAM>
+// AA: anti-aliasing (geom_grad.cuh).  dL_dopacity holds dL/d(o h), the blend backwards' sum; it is overwritten with
+// dL/do = h dL/d(o h), and dL/dr = o dL/d(o h) / (2 h) joins the covariance gradient.  h and its branch are the
+// forward's, read from the record (SplatRec::pad).
+template <bool CAM, bool AA>
 __global__ void __launch_bounds__(256) geom_backward_kernel(
     int P, int D, int M, const float* __restrict__ means, const int* __restrict__ radii,
     const float* __restrict__ shs, const uint8_t* __restrict__ clamped, const float* __restrict__ scales,
@@ -33,7 +36,8 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
     const float tan_fovx, const float tan_fovy, const float* __restrict__ campos, const float* __restrict__ dL_dmean2D,
     const float* __restrict__ dL_dconics, float* __restrict__ dL_dmeans, const float* __restrict__ dL_dcolor,
     float* __restrict__ dL_dcov, float* __restrict__ dL_dsh, float* __restrict__ dL_dscale,
-    float* __restrict__ dL_drot, const float* __restrict__ dL_ddepth, double* __restrict__ cam_partial) {
+    float* __restrict__ dL_drot, const float* __restrict__ dL_ddepth, double* __restrict__ cam_partial,
+    const SplatRec* __restrict__ rec, const float* __restrict__ opacities, float* __restrict__ dL_dopacity) {
     __shared__ float cam[35];  // view (16) | proj (16) | campos (3): read by every thread, staged once per CTA
     if (threadIdx.x < 16) {
         cam[threadIdx.x] = view_matrix[threadIdx.x];
@@ -52,10 +56,18 @@ __global__ void __launch_bounds__(256) geom_backward_kernel(
         const float g_conic[3] = {dL_dconics[4 * g], dL_dconics[4 * g + 1], dL_dconics[4 * g + 3]};
         const float g_ndc[2] = {dL_dmean2D[3 * g], dL_dmean2D[3 * g + 1]};
 
+        float g_r = 0.f;
+        if constexpr (AA) {
+            const float hs = rec[g].pad, h = fabsf(hs);
+            const float g_op = dL_dopacity[g];
+            dL_dopacity[g] = h * g_op;
+            if (hs > 0.f) g_r = opacities[g] * g_op / (2.f * h);
+        }
+
         float g_mean[3], g_cov[6];
         geomgrad::ProjectTerms terms;
         geomgrad::project_grad(p, cov6, cam, cam + 16, focal_x, focal_y, tan_fovx, tan_fovy, g_conic, g_ndc, g_mean,
-                               g_cov, CAM ? &terms : nullptr);
+                               g_cov, CAM ? &terms : nullptr, AA ? &g_r : nullptr);
 #pragma unroll
         for (int i = 0; i < 6; i++) dL_dcov[6 * g + i] = g_cov[i];
 
@@ -154,12 +166,14 @@ int launch_geom_backward(const sgb_view_inputs& in, GeomView g, const int32_t* r
     const float focal_y = in.H / (2.0f * in.tan_fovy);
     const float focal_x = in.W / (2.0f * in.tan_fovx);
     const int blocks = (in.P + 255) / 256;
-    auto kernel = cam_grads ? geom_backward_kernel<true> : geom_backward_kernel<false>;
+    auto kernel = cam_grads ? (in.antialiasing ? geom_backward_kernel<true, true> : geom_backward_kernel<true, false>)
+                            : (in.antialiasing ? geom_backward_kernel<false, true> : geom_backward_kernel<false, false>);
     kernel<<<blocks, 256, 0, s>>>(
         in.P, in.D, in.M, in.means3D, radii, in.shs, g.clamped, in.scales,
         in.rotations, in.scale_modifier, cov3D, in.viewmatrix, in.projmatrix, focal_x, focal_y,
         in.tan_fovx, in.tan_fovy, in.campos, gr.dL_dmeans2D, gr.dL_dconic, gr.dL_dmeans3D, dL_dcolor_rgb,
-        gr.dL_dcov3D, gr.dL_dsh, gr.dL_dscales, gr.dL_drotations, dL_ddepth, cam_partial);
+        gr.dL_dcov3D, gr.dL_dsh, gr.dL_dscales, gr.dL_drotations, dL_ddepth, cam_partial, g.rec, in.opacities,
+        gr.dL_dopacity);
     SGB_LAUNCH_CHECK("geom_backward_kernel", in.debug, s);
     if (!cam_grads) return SGB_OK;
     camera_grad_finalize_kernel<<<1, 1024, 0, s>>>(blocks, cam_partial, cam_grads->dL_dviewmatrix,

@@ -39,15 +39,44 @@ struct ProjectTerms {
     float g_hom[4];
 };
 
+// ---------------------------------------------------------------- anti-aliasing: opacity-compensated 0.3 px² dilation
+// The screen-space filter of Mip-Splatting as 3DGS ships it: with C0 = (a0, b; b, c0) the screen covariance before
+// the dilation and C = C0 + s I (s = 0.3, the conic's matrix), the blend reads the opacity o h with
+//     r = det C0 / det C,   h = sqrt(max(eps, r)),   eps = 2.5e-5
+// so a Gaussian keeps the integral o 2 pi sqrt(det C0) of its undilated footprint at every image size.  The floor keeps
+// degenerate and flat Gaussians finite (det C0 can round negative) and has zero gradient.
+constexpr float kAADilation = 0.3f;
+constexpr float kAAFloor = 2.5e-5f;
+
+// h of one Gaussian from C0 and the det C the conic inversion uses, signed: negative on the floor branch (r <= eps),
+// where the backward adds no covariance term.  The geometry state keeps it for the backward.
+SGB_HD float aa_scale(float a0, float b, float c0, float det) {
+    const float r = (a0 * c0 - b * b) / det;
+    return r > kAAFloor ? sqrtf(r) : -sqrtf(kAAFloor);
+}
+
+// dL/d(a0, b, c0) = g_r dr/d(a0, b, c0) with D = det C:
+//     dr/da0 = s (c0^2 + s c0 + b^2) / D^2,  dr/dc0 = s (a0^2 + s a0 + b^2) / D^2,  dr/db = -2 s b (a0 + c0 + s) / D^2
+// b is the off-diagonal VALUE (one variable, appearing twice in C), so out[1] is the full dL/db.
+SGB_HD void aa_cov_grad(float a0, float b, float c0, float D, float g_r, float out[3]) {
+    const float s = kAADilation;
+    const float k = g_r * s / (D * D);
+    out[0] = k * (c0 * c0 + s * c0 + b * b);
+    out[1] = -2.f * k * b * (a0 + c0 + s);
+    out[2] = k * (a0 * a0 + s * a0 + b * b);
+}
+
 // ---------------------------------------------------------------- conic / centre -> world mean and covariance
 // view, proj: column-major 4x4 as the reference passes them (element (row i, col j) at [4 j + i]).
 // g_conic = (dL/dK_xx, dL/dK_xy [halved], dL/dK_yy), g_ndc = dL/d(projected centre in NDC units).
 // out_mean[3] = dL/dp (both paths summed), out_cov[6] = dL/d(S_xx, S_xy, S_xz, S_yy, S_yz, S_zz).
 // terms: NULL, or filled for camera_grad.  Filling it only copies values already computed (no value computed for
 // out_mean / out_cov gains a use that could change how it is rounded).
+// aa_g_r: NULL without anti-aliasing, else dL/dr of the opacity factor above (0 on its floor branch); its covariance
+// term joins dL/dC before anything is formed from it, so it reaches the mean, covariance and camera gradients.
 SGB_HD void project_grad(const float p[3], const float cov6[6], const float* view, const float* proj, float fx, float fy,
                          float tan_x, float tan_y, const float g_conic[3], const float g_ndc[2], float out_mean[3],
-                         float out_cov[6], ProjectTerms* terms = nullptr) {
+                         float out_cov[6], ProjectTerms* terms = nullptr, const float* aa_g_r = nullptr) {
     // view-space centre, frustum clamp of the Jacobian's evaluation point
     float t[3];
 #pragma unroll
@@ -88,6 +117,16 @@ SGB_HD void project_grad(const float p[3], const float cov6[6], const float* vie
         m00 = -scale * (h00 * cc - h01 * cb);
         m01 = -scale * (h01 * ca - h00 * cb);
         m11 = -scale * (h11 * ca - h10 * cb);
+    }
+    if (aa_g_r && *aa_g_r != 0.f) {
+        // M is dL/dC as a symmetric matrix (dL/dA = 2 M B): the off-diagonal entry takes half of dL/db
+        const float a0 = B[0][0] * A[0][0] + B[0][1] * A[0][1] + B[0][2] * A[0][2];
+        const float c0 = B[1][0] * A[1][0] + B[1][1] * A[1][1] + B[1][2] * A[1][2];
+        float g[3];
+        aa_cov_grad(a0, cb, c0, det, *aa_g_r, g);
+        m00 += g[0];
+        m01 += 0.5f * g[1];
+        m11 += g[2];
     }
 
     // dL/dS = A^T M A (symmetric; off-diagonal outputs doubled), dL/dA = 2 M B

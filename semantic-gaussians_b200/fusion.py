@@ -241,7 +241,7 @@ def lift_views(gaussians, views, feature_maps, pipe, feat_sum: torch.Tensor, wei
     views         cameras (FoVx, FoVy, world_view_transform, full_proj_transform, camera_center)
     feature_maps  sequence, or callable idx -> map, of (C, h, w) float16 / float32 tensors on the Gaussians' device;
                   views are rendered at the map size (render()'s override_shape), which all maps of a call share
-    pipe          compute_cov3d_python and debug are honoured as in render_chn_batch
+    pipe          compute_cov3d_python, debug and antialiasing are honoured as in render_chn_batch
     feat_sum      (P, C) and weight_sum (P,) or (P, 1): contiguous float32 on the Gaussians' device, added into
 
     The views go to the native call in batches of at most 8 consecutive views whose maps share a dtype.  A sequence
@@ -250,7 +250,7 @@ def lift_views(gaussians, views, feature_maps, pipe, feat_sum: torch.Tensor, wei
     map size that differs from the call's first map.  Returns the number of views lifted."""
     from . import channel_rasterization as chn
     from .rasterizer import _cameras, _make_inputs, _ptrs, _stream_ctx
-    from .renderer import _prepare
+    from .renderer import _antialiasing, _prepare
     views = list(views)
     xyz = gaussians.get_xyz
     dev, P = xyz.device, xyz.shape[0]
@@ -307,7 +307,8 @@ def lift_views(gaussians, views, feature_maps, pipe, feat_sum: torch.Tensor, wei
                        campos=cam.camera_center)) for cam in batch]
             inp, cameras, keep, _ = _make_inputs(_cameras(settings), bg, call["means3D"], None,
                                                  call["opacities"], call["scales"], call["rotations"], scaling_modifier,
-                                                 call["cov3D_precomp"], h, w, None, 0, False, debug, Cn)
+                                                 call["cov3D_precomp"], h, w, None, 0, False, debug, Cn,
+                                                 antialiasing=_antialiasing(pipe))
             inp.background = None
             stream, ctx = _stream_ctx(dev)
             dt = _lib.FEAT_F16 if maps[0].dtype == torch.float16 else _lib.FEAT_F32

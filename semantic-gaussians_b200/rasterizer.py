@@ -58,9 +58,10 @@ def _stream_ctx(device):
 
 
 def _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                 H, W, sh, degree, prefiltered, debug, num_channels):
+                 H, W, sh, degree, prefiltered, debug, num_channels, antialiasing=False):
     """``cams`` holds one (viewmatrix, projmatrix, campos, tan_fovx, tan_fovy) per view.  Returns the shared inputs
-    (carrying view 0's camera), the sgb_camera array, the tensors both point into, and the device."""
+    (carrying view 0's camera), the sgb_camera array, the tensors both point into, and the device.  ``antialiasing``:
+    the opacity-compensated screen-space filter (sgb_view_inputs.antialiasing)."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:61-64
     if not means3D.is_cuda:
@@ -86,7 +87,7 @@ def _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, 
         scale_modifier=float(scale_modifier), rotations=_ptr(keep["rotations"]),
         cov3D_precomp=_ptr(keep["cov3D"]), viewmatrix=_ptr(keep["view"]), projmatrix=_ptr(keep["proj"]),
         campos=_ptr(keep["campos"]), tan_fovx=float(tan_fovx), tan_fovy=float(tan_fovy),
-        prefiltered=int(bool(prefiltered)), debug=int(bool(debug)))
+        prefiltered=int(bool(prefiltered)), debug=int(bool(debug)), antialiasing=int(bool(antialiasing)))
     # view 0 is the camera of the shared inputs, checked above in the reference's argument order
     cameras = [_lib.Camera(inp.viewmatrix, inp.projmatrix, inp.campos, inp.tan_fovx, inp.tan_fovy)]
     for v, (viewmatrix, projmatrix, campos, tan_fovx, tan_fovy) in enumerate(cams[1:], 1):
@@ -98,7 +99,7 @@ def _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, 
 
 def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opacity, scales, rotations,
              scale_modifier, cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, num_channels,
-             want_exp_alpha=False, features=None, bg_features=None):
+             want_exp_alpha=False, features=None, bg_features=None, antialiasing=False):
     """V = len(cams) views of the same Gaussians through sgb_forward_geometry_batch / sgb_forward_render_batch_ext:
     one stream sync for all instance counts, one for all weight-pool checks.  With ``features`` (P, c) over
     ``bg_features`` (c), the render call is sgb_forward_render_joint_batch, which also renders that table from the same
@@ -123,7 +124,7 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
                       z(1, image_height, image_width) if want_exp_alpha else None,
                       z(1, image_height, image_width) if want_exp_alpha else None, *feat)
     native = _make_inputs(cams, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                          image_height, image_width, sh, degree, prefiltered, debug, num_channels)
+                          image_height, image_width, sh, degree, prefiltered, debug, num_channels, antialiasing)
     inp, cameras, keep, dev = native
     P, H, W, Cn = inp.P, inp.H, inp.W, inp.C
     if features is not None:
@@ -168,12 +169,12 @@ def _forward(want_depth: bool, what: str, cams, background, means3D, colors, opa
 
 def _forward_joint(what: str, cams, background, means3D, colors, opacity, scales, rotations, scale_modifier,
                    cov3D_precomp, image_height, image_width, sh, degree, prefiltered, debug, features, bg_features,
-                   want_exp_alpha=False):
+                   want_exp_alpha=False, antialiasing=False):
     """_forward of the RGB render (median depth always) with ``features``: (native, per-view lists as _forward's
     without features, per-view feature images, the marshalled (features, bg_features) or None for an empty scene)."""
     native, (*lists, feat) = _forward(True, what, cams, background, means3D, colors, opacity, scales, rotations,
                                       scale_modifier, cov3D_precomp, image_height, image_width, sh, degree,
-                                      prefiltered, debug, 3, want_exp_alpha, features, bg_features)
+                                      prefiltered, debug, 3, want_exp_alpha, features, bg_features, antialiasing)
     return native, tuple(lists), feat, None if native is None else (native[2]["features"], native[2]["bg_features"])
 
 
@@ -364,7 +365,7 @@ def _native_args(is_chn, joint, settings_list, means3D, sh, colors_precomp, opac
 
 
 def _views_forward(ctx, is_chn, what, settings_list, means3D, sh, colors_precomp, opacities, scales, rotations,
-                   cov3Ds_precomp, expected_depth, features=None, bg_features=None):
+                   cov3Ds_precomp, expected_depth, antialiasing, features=None, bg_features=None):
     """Forward of _RasterizeGaussians (one view), _RasterizeGaussiansBatch and, with ``features``, _RasterizeJointBatch:
     (*colors, *radii[, *depths][, *feature images][, *expected depths, *alphas]), the depths for the rgbd variant (not
     ``is_chn``), the feature images with ``features``, the last two when ``expected_depth``."""
@@ -372,10 +373,10 @@ def _views_forward(ctx, is_chn, what, settings_list, means3D, sh, colors_precomp
     native, (R, color, radii, geom, binning, img, depth, exp_depth, alpha, *feat) = _forward(
         not is_chn, what, *_native_args(is_chn, joint, settings_list, means3D, sh, colors_precomp, opacities, scales,
                                         rotations, cov3Ds_precomp),
-        want_exp_alpha=expected_depth, features=features, bg_features=bg_features)
+        want_exp_alpha=expected_depth, features=features, bg_features=bg_features, antialiasing=antialiasing)
     # the backward reuses the marshalled inputs; they also hold any contiguous copies their pointers refer to
     ctx.settings_list, ctx.R, ctx.native, ctx.expected_depth = settings_list, R, native, expected_depth
-    ctx.is_chn = is_chn
+    ctx.is_chn, ctx.antialiasing = is_chn, antialiasing
     ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, sh, features, bg_features, *radii,
                           *geom, *binning, *img)
     ctx.mark_non_differentiable(*radii)
@@ -424,7 +425,8 @@ def _views_backward(ctx, what, saved, grad_outputs, cam_grad=False):
     native = ctx.native
     if native is None:  # empty scene: the forward marshalled nothing
         native = _make_inputs(*_native_args(ctx.is_chn, features is not None, ctx.settings_list, means3D, sh,
-                                            colors_precomp, means3D, scales, rotations, cov3Ds_precomp))
+                                            colors_precomp, means3D, scales, rotations, cov3Ds_precomp),
+                              antialiasing=ctx.antialiasing)
     joint = None
     if features is not None:  # the table and background as the forward marshalled them (as given: empty scene)
         keep = native[2]
@@ -487,12 +489,12 @@ def make_module(variant: str):
     class _RasterizeGaussians(torch.autograd.Function):
         @staticmethod
         def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                    raster_settings, expected_depth=False, *camera):
+                    raster_settings, expected_depth=False, antialiasing=False, *camera):
             # camera: _camera_tensors([raster_settings]), inputs only so that they can receive gradients
             rs = raster_settings
             try:
                 return _views_forward(ctx, is_chn, "rasterize_gaussians", [rs], means3D, sh, colors_precomp, opacities,
-                                      scales, rotations, cov3Ds_precomp, expected_depth)
+                                      scales, rotations, cov3Ds_precomp, expected_depth, antialiasing)
             except Exception:
                 if rs.debug:
                     args = [rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
@@ -507,7 +509,7 @@ def make_module(variant: str):
             saved = ctx.saved_tensors
             try:
                 g_means2D, g_means3D, *grads = _views_backward(ctx, "rasterize_gaussians_backward", saved,
-                                                               grad_outputs, any(ctx.needs_input_grad[10:]))
+                                                               grad_outputs, any(ctx.needs_input_grad[11:]))
             except Exception:
                 rs = ctx.settings_list[0]
                 if rs.debug:
@@ -520,14 +522,15 @@ def make_module(variant: str):
                     print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
                 raise
             *grads, g_view, g_proj, g_campos = grads
-            return (g_means3D, g_means2D[0], *grads, None, None, g_view, g_proj, g_campos)
+            return (g_means3D, g_means2D[0], *grads, None, None, None, g_view, g_proj, g_campos)
 
     def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                            raster_settings, *, expected_depth=False):
+                            raster_settings, *, expected_depth=False, antialiasing=False):
         """The reference's rasterize_gaussians; with ``expected_depth`` the outputs gain the expected depth
-        E = sum_i w_i z_i and the accumulated opacity A = sum_i w_i, (1, H, W) each and differentiable (C <= 4)."""
+        E = sum_i w_i z_i and the accumulated opacity A = sum_i w_i, (1, H, W) each and differentiable (C <= 4).
+        ``antialiasing``: 3DGS's opacity-compensated screen-space filter (INTEGRATION.md, "Anti-aliasing")."""
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                         cov3Ds_precomp, raster_settings, expected_depth,
+                                         cov3Ds_precomp, raster_settings, expected_depth, bool(antialiasing),
                                          *_camera_tensors([raster_settings]))
 
     class _RasterizeGaussiansBatch(torch.autograd.Function):
@@ -538,26 +541,27 @@ def make_module(variant: str):
 
         @staticmethod
         def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings_list,
-                    expected_depth, *means2D_camera):
+                    expected_depth, antialiasing, *means2D_camera):
             # means2D_camera: the V screen-space tensors, then _camera_tensors(settings_list)
             _check_batch_settings(settings_list)
             return _views_forward(ctx, is_chn, "rasterize_gaussians_batch", settings_list, means3D, sh, colors_precomp,
-                                  opacities, scales, rotations, cov3Ds_precomp, expected_depth)
+                                  opacities, scales, rotations, cov3Ds_precomp, expected_depth, antialiasing)
 
         @staticmethod
         def backward(ctx, *grad_outputs):
             V = len(ctx.settings_list)
             g_means2D, *grads = _views_backward(ctx, "rasterize_gaussians_backward_batch", ctx.saved_tensors,
-                                                grad_outputs, any(ctx.needs_input_grad[9 + V:]))
-            return (*grads[:-3 * V], None, None, *g_means2D, *grads[-3 * V:])
+                                                grad_outputs, any(ctx.needs_input_grad[10 + V:]))
+            return (*grads[:-3 * V], None, None, None, *g_means2D, *grads[-3 * V:])
 
     def rasterize_gaussians_batch(means3D, means2D_list, opacities, settings_list, shs=None, colors_precomp=None,
-                                  scales=None, rotations=None, cov3D_precomp=None, expected_depth=False):
+                                  scales=None, rotations=None, cov3D_precomp=None, expected_depth=False,
+                                  antialiasing=False):
         """Batched counterpart of GaussianRasterizer.forward: ``settings_list`` holds one
         GaussianRasterizationSettings per view (same image size / background tensor / channel count; only the
         cameras differ), ``means2D_list`` one screen-space tensor per view.  Returns a list of per-view tuples
         (color, radii[, depth][, expected depth, alpha]), the last two with ``expected_depth`` (see
-        rasterize_gaussians).  Batches larger than the native limit are split."""
+        rasterize_gaussians, also for ``antialiasing``).  Batches larger than the native limit are split."""
         shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
                                                                                  rotations, cov3D_precomp)
         results = []
@@ -565,7 +569,8 @@ def make_module(variant: str):
             sl = list(settings_list[lo:lo + _lib.MAX_BATCH])
             m2 = list(means2D_list[lo:lo + _lib.MAX_BATCH])
             out = _RasterizeGaussiansBatch.apply(means3D, shs, colors_precomp, opacities, scales, rotations,
-                                                 cov3D_precomp, sl, expected_depth, *m2, *_camera_tensors(sl))
+                                                 cov3D_precomp, sl, expected_depth, bool(antialiasing), *m2,
+                                                 *_camera_tensors(sl))
             V = len(sl)
             per_view = 2 if is_chn else 3
             if expected_depth:
@@ -575,9 +580,12 @@ def make_module(variant: str):
         return results
 
     class GaussianRasterizer(nn.Module):  # channel_rasterization/__init__.py:232-289
-        def __init__(self, raster_settings):
+        def __init__(self, raster_settings, antialiasing=False):
+            """``antialiasing``: 3DGS's opacity-compensated screen-space filter for every render of this rasterizer
+            (INTEGRATION.md, "Anti-aliasing"); not a settings field, whose layout is the reference's."""
             super().__init__()
             self.raster_settings = raster_settings
+            self.antialiasing = bool(antialiasing)
 
         def markVisible(self, positions):
             with torch.no_grad():
@@ -589,7 +597,7 @@ def make_module(variant: str):
             shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
                                                                                      rotations, cov3D_precomp)
             return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, self.raster_settings)
+                                       cov3D_precomp, self.raster_settings, antialiasing=self.antialiasing)
 
         def forward_expected_depth(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                                    rotations=None, cov3D_precomp=None):
@@ -597,7 +605,8 @@ def make_module(variant: str):
             shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales,
                                                                                      rotations, cov3D_precomp)
             return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, self.raster_settings, expected_depth=True)
+                                       cov3D_precomp, self.raster_settings, expected_depth=True,
+                                       antialiasing=self.antialiasing)
 
     GaussianRasterizationSettings.__qualname__ = "GaussianRasterizationSettings"
     GaussianRasterizer.__qualname__ = "GaussianRasterizer"
@@ -613,27 +622,29 @@ class _RasterizeJointBatch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, features, bg_features,
-                settings_list, expected_depth, *means2D_camera):
+                settings_list, expected_depth, antialiasing, *means2D_camera):
         # means2D_camera: the V screen-space tensors, then _camera_tensors(settings_list)
         _check_batch_settings(settings_list)
         return _views_forward(ctx, False, "rasterize_joint_batch", settings_list, means3D, sh, colors_precomp,
-                              opacities, scales, rotations, cov3Ds_precomp, expected_depth, features, bg_features)
+                              opacities, scales, rotations, cov3Ds_precomp, expected_depth, antialiasing, features,
+                              bg_features)
 
     @staticmethod
     def backward(ctx, *grad_outputs):
         V = len(ctx.settings_list)
         g_means2D, *grads = _views_backward(ctx, "rasterize_joint_backward_batch", ctx.saved_tensors, grad_outputs,
-                                            any(ctx.needs_input_grad[11 + V:]))
-        return (*grads[:-3 * V], None, None, None, *g_means2D, *grads[-3 * V:])
+                                            any(ctx.needs_input_grad[12 + V:]))
+        return (*grads[:-3 * V], None, None, None, None, *g_means2D, *grads[-3 * V:])
 
 
 def rasterize_joint_batch(means3D, means2D_list, opacities, settings_list, features, bg_features, shs=None,
-                          colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, expected_depth=False):
+                          colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, expected_depth=False,
+                          antialiasing=False):
     """The RGB-D rasterizer's rasterize_batch (``settings_list`` of rgbd GaussianRasterizationSettings, RGB colours
     from ``shs`` or ``colors_precomp``) that also renders ``features`` (P, c) over ``bg_features`` (c) from the same
     geometry and binning.  Returns a list of per-view tuples (rgb, radii, depth, feature image[, expected depth,
     alpha]).  ``means2D_list[v].grad`` receives the sum of both images' dL/dmean2D.  Batches larger than the native
-    limit are split."""
+    limit are split.  ``antialiasing`` as for rasterize_gaussians."""
     shs, colors_precomp, scales, rotations, cov3D_precomp = _optional_inputs(shs, colors_precomp, scales, rotations,
                                                                              cov3D_precomp)
     results = []
@@ -642,7 +653,8 @@ def rasterize_joint_batch(means3D, means2D_list, opacities, settings_list, featu
         sl = list(settings_list[lo:lo + _lib.MAX_BATCH])
         m2 = list(means2D_list[lo:lo + _lib.MAX_BATCH])
         out = _RasterizeJointBatch.apply(means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                         features, bg_features, sl, expected_depth, *m2, *_camera_tensors(sl))
+                                         features, bg_features, sl, expected_depth, bool(antialiasing), *m2,
+                                         *_camera_tensors(sl))
         V = len(sl)
         for v in range(V):
             results.append(tuple(out[i * V + v] for i in range(per_view)))

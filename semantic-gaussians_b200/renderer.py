@@ -17,6 +17,11 @@ with gradients (to means3D through z and through the blend weights, to opacity, 
 the screen-space points).  No background term: the normalised depth is E / A.clamp_min(eps).  "depth" stays the
 reference's non-differentiable median depth.
 
+Addition: ``pipe.antialiasing`` (3DGS's PipelineParams attribute; absent means False) turns on the opacity-compensated
+screen-space filter in every render here: each Gaussian's opacity is scaled by sqrt(det C0 / det C), C0 its screen
+covariance before the fixed 0.3 px² dilation and C after it, so a Gaussian covers the same area at every image size.
+Radii, tiles and binning are unchanged.  Train and render a model with the same setting (INTEGRATION.md).
+
 Addition: render_with_features() / render_with_features_batch() train colour and a per-Gaussian feature field
 together: one geometry pass and one binning per view produce render()'s dict (plus "expected_depth" / "alpha" under
 ``differentiable_depth``) and "features" (c, H, W), the image of a (P, c) table over its background, bitwise what
@@ -32,6 +37,10 @@ from . import channel_rasterization as chn_rasterize
 from .rasterizer import rasterize_joint_batch
 from .rgbd_rasterization import GaussianRasterizationSettings, GaussianRasterizer
 from .sh_utils import eval_sh
+
+
+def _antialiasing(pipe) -> bool:
+    return bool(getattr(pipe, "antialiasing", False))
 
 
 def _prepare(viewpoint_camera, pc, pipe, scaling_modifier, override_color, override_shape, foreground, world_rotate):
@@ -133,7 +142,7 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
     screenspace_points, common, call = _prepare(viewpoint_camera, pc, pipe, scaling_modifier, override_color,
                                                 override_shape, foreground, world_rotate)
     raster_settings = GaussianRasterizationSettings(bg=bg_color, debug=pipe.debug, **common)
-    rasterizer = GaussianRasterizer(raster_settings=raster_settings)
+    rasterizer = GaussianRasterizer(raster_settings=raster_settings, antialiasing=_antialiasing(pipe))
     if differentiable_depth:
         rendered_image, radii, depth, exp_depth, alpha = rasterizer.forward_expected_depth(**call)
     else:
@@ -152,7 +161,7 @@ def render_chn(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modif
                                                 override_shape, foreground, world_rotate)
     raster_settings = chn_rasterize.GaussianRasterizationSettings(
         bg=bg_color, debug=bool(getattr(pipe, "debug", False)), num_channels=num_channels, **common)
-    rasterizer = chn_rasterize.GaussianRasterizer(raster_settings=raster_settings)
+    rasterizer = chn_rasterize.GaussianRasterizer(raster_settings=raster_settings, antialiasing=_antialiasing(pipe))
     rendered_image, radii = rasterizer.forward(**call)
     return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
             "radii": radii}
@@ -184,7 +193,7 @@ def _render_batch(variant, cameras, pc, pipe, bg_color, scaling_modifier, num_ch
     outs = Rast.rasterize_batch(call["means3D"], points, call["opacities"], settings, shs=call["shs"],
                                 colors_precomp=call["colors_precomp"], scales=call["scales"],
                                 rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
-                                expected_depth=differentiable_depth)
+                                expected_depth=differentiable_depth, antialiasing=_antialiasing(pipe))
     res = []
     for pts, o in zip(points, outs):
         d = {"render": o[0], "viewspace_points": pts, "visibility_filter": o[1] > 0, "radii": o[1]}
@@ -244,7 +253,7 @@ def render_with_features_batch(cameras, pc, pipe, bg_color: torch.Tensor, featur
         outs = rasterize_joint_batch(call["means3D"], points, call["opacities"], settings, features, bg_features,
                                      shs=call["shs"], colors_precomp=call["colors_precomp"], scales=call["scales"],
                                      rotations=call["rotations"], cov3D_precomp=call["cov3D_precomp"],
-                                     expected_depth=differentiable_depth)
+                                     expected_depth=differentiable_depth, antialiasing=_antialiasing(pipe))
         for pts, o in zip(points, outs):
             d = {"render": o[0], "viewspace_points": pts, "visibility_filter": o[1] > 0, "radii": o[1],
                  "depth": o[2], "features": o[3]}
