@@ -20,10 +20,11 @@
 //                     Gaussian) for all channels over the strip's own entries (register
 //                     micro-tiles), then the reference's back-to-front chain (backward.cu:477-550)
 //                     in dot-product form -> dL/dmean2D, dL/dconic, dL/dopacity.
-//   dfeature          persistent CTAs claim (tile, 64-channel chunk) items: dL/dfeature[g][ch] = sum_px
-//                     w * dL/dout, a producer warp streams dL tiles and weight slabs by TMA, every
-//                     compute warp owns 8 channels of all the tile's entries, one 16-byte reduction
-//                     per (Gaussian, tile, 4 channels).
+//   dfeature          persistent CTAs claim (tile, up to 256 channels) items: dL/dfeature[g][ch] =
+//                     sum_px w * dL/dout, a producer warp streams 32-pixel weight and dL slabs by TMA
+//                     through one ring, every compute warp owns 32 channels of all the tile's entries
+//                     (setmaxnreg moves the producer group's registers to them), one 16-byte
+//                     reduction per (Gaussian, tile, 4 channels).
 //
 // Results are unchanged: the integer outputs come from the verbatim chain; every accumulator still
 // adds its Gaussians in depth order.
@@ -51,7 +52,7 @@ int chn_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float*
 //     forward   out[256 px][64 ch]  = W^T[256 px][G]  . F[G][64 ch]      K = G      lane tile 8 px x 8 ch
 //     s-pass    S[32 px][32]        = dL[32 px][C]    . F^T[C][32]       K = C      lane tile 8 px x 4 entries
 //               (per warp: its strip and a 32-entry segment of the strip's entries)
-//     dfeature  dF[G][64 ch]        = W[G][256 px]    . dL[256 px][64]   K = 256 px lane tile <= 8 entries x 4 ch
+//     dfeature  dF[G][256 ch]       = W[G][256 px]    . dL[256 px][256]  K = 256 px lane tile <= 8 entries x 16 ch
 // Register tiles give every shared-memory load several FMAs and need no cross-lane reductions (a
 // shuffle-reduce formulation spends its issue slots on SHFL/FSEL/FADD instead).
 
