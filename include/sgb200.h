@@ -343,7 +343,9 @@ int sgb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,
 /* Named read-only views into the opaque state, for tests and diagnostics.  Copies the field
  * into dst (device) and returns the byte count, or a negative error.  Fields: "depths",
  * "means2D", "conic_opacity", "cov3D", "rgb", "clamped", "tiles_touched", "point_list",
- * "ranges", "n_contrib", "final_T". */
+ * "ranges", "n_contrib", "final_T", and "aa_h" (float [P]): with antialiasing the signed opacity factor h of
+ * each Gaussian (conic_opacity's opacity is o |h|; h < 0 on the floor branch, where the backward adds no
+ * covariance term), 0 without it.  Per-Gaussian fields are defined where radii > 0. */
 int64_t sgb_state_field(const char* name, int32_t P, int64_t num_rendered, int32_t W, int32_t H,
                         const void* geometry_state, const void* binning_state,
                         const void* image_state, void* dst, void* stream);

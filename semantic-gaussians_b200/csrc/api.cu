@@ -65,6 +65,7 @@ __global__ void extract_rec_kernel(int P, const SplatRec* __restrict__ rec, int 
     const SplatRec r = rec[i];
     if (what == 0) dst[i] = r.depth;
     else if (what == 1) { dst[2 * i] = r.mx; dst[2 * i + 1] = r.my; }
+    else if (what == 3) dst[i] = r.pad;
     else { dst[4 * i] = r.cx; dst[4 * i + 1] = r.cy; dst[4 * i + 2] = r.cz; dst[4 * i + 3] = r.op; }
 }
 
@@ -757,11 +758,12 @@ int64_t sgb_state_field(const char* name, int32_t P, int64_t R, int32_t W, int32
     size_t n = 0;
     if (geometry_state && P > 0) {
         GeomView g = GeomView::carve(const_cast<void*>(geometry_state), P);
-        int what = !strcmp(name, "depths") ? 0 : !strcmp(name, "means2D") ? 1 : !strcmp(name, "conic_opacity") ? 2 : -1;
+        int what = !strcmp(name, "depths") ? 0 : !strcmp(name, "means2D") ? 1 : !strcmp(name, "conic_opacity") ? 2
+                 : !strcmp(name, "aa_h") ? 3 : -1;
         if (what >= 0) {
             extract_rec_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, g.rec, what, (float*)dst);
             SGB_LAUNCH_CHECK("extract_rec_kernel", 0, s);
-            return (int64_t)P * (what == 0 ? 4 : what == 1 ? 8 : 16);
+            return (int64_t)P * (what == 0 || what == 3 ? 4 : what == 1 ? 8 : 16);
         }
         if (!strcmp(name, "cov3D")) { src = g.cov3D; n = (size_t)P * 24; }
         else if (!strcmp(name, "rgb")) { src = g.rgb; n = (size_t)P * 12; }

@@ -13,16 +13,24 @@ gradient of the conic K = C^-1 scaled by det^2 / (det^2 + 1e-7), the reference's
 Conventions held as the forward holds them: where the Jacobian's evaluation point is clamped sideways, the clamped
 t_x (t_y) is a constant; focal lengths are fp32 constants.
 
-Magnitude: per Gaussian and entry, mag = kappa |c_cov| + |c_ndc| + |c_z| + |c_rgb| from four separate backwards (one
-per path), kappa the screen covariance's conditioning (geom_ref).  A per-view camera gradient passes when
-|got - sum_i c_i| <= RTOL * sum_i mag_i entry by entry.
+With antialiasing a fifth path is the opacity factor: L_aa = sum_i g_i o_i h_i(C0_i) with g = dL/d(o h) the blend's
+opacity gradient (what the geometry kernel reads before it overwrites dL_dopacity with h g), o the raw opacity and
+h = sqrt(max(2.5e-5, det C0 / det C)) of the undilated screen covariance C0 = C - 0.3 I; on the floor h is constant.
+Which side of the floor a Gaussian is on is the kernel's fp32 decision (the sign of the h it stored, aa_active), not
+a float64 one: where det C0 / det C lies within rounding of the floor the two could differ, and the whole term of
+that Gaussian would count as error (geom_ref's comparison checks that decision, leaving out its fragile band).
+
+Magnitude: per Gaussian and entry, mag = kappa |c_cov| + |c_ndc| + |c_z| + |c_rgb| (+ kappa0 |c_aa|) from separate
+backwards (one per path), kappa the screen covariance's conditioning (geom_ref) and kappa0 that of C0, whose
+determinant h is formed from.  A per-view camera gradient passes when |got - sum_i c_i| <= RTOL * sum_i mag_i entry
+by entry.
 """
 from __future__ import annotations
 
 import numpy as np
 import torch
 
-from geom_ref import DET_REG, EPS32, LOWPASS, W_EPS, _c
+from geom_ref import AA_FLOOR, DET_REG, EPS32, LOWPASS, W_EPS, _c
 
 from semantic_gaussians_b200.sh_utils import eval_sh
 
@@ -40,10 +48,13 @@ def _f64(a, dev):
 
 
 def camera_terms(means3D, radii, cov3D, view, proj, campos, W, H, tan_fovx, tan_fovy, dL_dmeans2D, dL_dconic, *,
-                 shs=None, D=0, clamped=None, dL_dcolors=None, dL_ddepth=None, dev="cpu"):
+                 shs=None, D=0, clamped=None, dL_dcolors=None, dL_ddepth=None, antialiasing=False, opacities=None,
+                 dL_dopacity=None, aa_active=None, dev="cpu"):
     """Per-Gaussian camera-gradient contributions (P, 35) = [dview 16 | dproj 16 | dcampos 3] (element order of the
     flattened fp32 camera arrays the kernel reads) and their magnitudes (P, 35), both float64; culled Gaussians
-    (radii <= 0) get zeros."""
+    (radii <= 0) get zeros.  antialiasing: opacities (P,) the raw o, dL_dopacity (P,) the blend's g = dL/d(o h),
+    aa_active (P,) the branch the kernel took (h > 0: above the floor)."""
+    assert not antialiasing or all(x is not None for x in (opacities, dL_dopacity, aa_active))
     P = int(np.asarray(radii.cpu() if isinstance(radii, torch.Tensor) else radii).shape[0])
     keep = torch.as_tensor(np.asarray(radii.cpu() if isinstance(radii, torch.Tensor) else radii)).reshape(-1) > 0
     idx = torch.nonzero(keep).reshape(-1).to(dev)
@@ -102,7 +113,15 @@ def camera_terms(means3D, radii, cov3D, view, proj, campos, W, H, tan_fovx, tan_
             l_rgb = (g * rgb).sum()
         else:
             l_rgb = tz.sum() * 0.0
-        return l_cov, l_ndc, l_z, l_rgb, Cm.detach()
+        l_aa = tz.sum() * 0.0
+        if antialiasing:
+            C0 = Cm - LOWPASS * torch.eye(2, dtype=torch.float64, device=dev)
+            r = torch.linalg.det(C0) / torch.linalg.det(Cm)
+            active = pick(aa_active, 1)[:, 0] > 0
+            # the floor branch is constant: no camera gradient
+            h = torch.where(active, r.clamp(min=1e-300).sqrt(), torch.full_like(r, AA_FLOOR ** 0.5))
+            l_aa = (pick(opacities, 1)[:, 0] * pick(dL_dopacity, 1)[:, 0] * h).sum()
+        return l_cov, l_ndc, l_z, l_rgb, l_aa, Cm.detach()
 
     vm = view0.expand(n, 16).clone().requires_grad_(True)
     pm = proj0.expand(n, 16).clone().requires_grad_(True)
@@ -110,16 +129,19 @@ def camera_terms(means3D, radii, cov3D, view, proj, campos, W, H, tan_fovx, tan_
     with torch.enable_grad():
         losses = forward(vm, pm, cp)
         parts = []
-        for loss in losses[:4]:
+        for loss in losses[:5]:
             gs = (torch.autograd.grad(loss, (vm, pm, cp), retain_graph=True, allow_unused=True) if loss.requires_grad
                   else (None, None, None))   # SH degree 0: the colour does not depend on the camera
             parts.append(torch.cat([torch.zeros((n, w), dtype=torch.float64, device=dev) if g is None else g
                                     for g, w in zip(gs, (16, 16, 3))], 1))
-    Cm = losses[4]
+    Cm = losses[5]
     a, b, c = Cm[:, 0, 0], Cm[:, 0, 1], Cm[:, 1, 1]
     kappa = ((a * c).abs() + b * b) / (a * c - b * b).abs()
-    contrib = parts[0] + parts[1] + parts[2] + parts[3]
-    mag = kappa[:, None] * parts[0].abs() + parts[1].abs() + parts[2].abs() + parts[3].abs()
+    a0, c0 = a - LOWPASS, c - LOWPASS
+    kappa0 = ((a0 * c0).abs() + b * b) / (a0 * c0 - b * b).abs()
+    contrib = parts[0] + parts[1] + parts[2] + parts[3] + parts[4]
+    mag = (kappa[:, None] * parts[0].abs() + parts[1].abs() + parts[2].abs() + parts[3].abs()
+           + torch.where(parts[4] == 0, torch.zeros_like(parts[4]), kappa0[:, None] * parts[4].abs()))
     full = torch.zeros((P, 35), dtype=torch.float64, device=dev)
     fmag = torch.zeros((P, 35), dtype=torch.float64, device=dev)
     full[idx], fmag[idx] = contrib, mag

@@ -241,12 +241,49 @@ def _rect_edge(e: AV, gmax, dev):
     return val, _near(e, k) & (k >= 1) & (k <= gmax)
 
 
+AA_DILATION = LOWPASS        # the 0.3 px^2 the anti-aliasing filter compensates for
+AA_FLOOR = _c(2.5e-5)       # the floor of det C0 / det C
+
+
+def _aa_factor(a0, b, c0):
+    """3DGS's anti-aliasing opacity factor (forward.cu of the 3DGS rasterizer with antialiasing) in scalar form:
+        det C0 = a0 c0 - b^2,  det C = (a0 + 0.3) (c0 + 0.3) - b^2,  h = sqrt(max(2.5e-5, det C0 / det C)).
+    Returns (h as AV, active = r above the floor, fragile band of that decision).  det C0 cancels for needles and
+    sub-pixel Gaussians, and its magnitude (|a0 c0| + b^2) carries that into r, h and everything formed from them.
+    On the floor branch h is the constant sqrt(2.5e-5), whose fp32 rounding its own magnitude covers."""
+    det0 = a0 * c0 - b * b
+    detc = (a0 + AA_DILATION) * (c0 + AA_DILATION) - b * b
+    r = det0 / detc
+    active = r.v > AA_FLOOR
+    floor = AV(torch.full_like(r.v, AA_FLOOR ** 0.5))
+    h = _where(active, AV(r.v.clamp(min=AA_FLOOR), r.m).sqrt(), floor)
+    return h, active, _near(r, AA_FLOOR)
+
+
+def _aa_dr(a0, b, c0, mutation=None):
+    """dr/d(a0, b, c0) of r = det C0 / det C, b the off-diagonal value (one variable that appears twice in C): 3DGS's
+    backward.cu expression with x = a0, y = c0, z = b, w = 0.3:
+        dr/dx = w (w y + y^2 + z^2) / den^2,  dr/dy = w (w x + x^2 + z^2) / den^2,  dr/dz = -2 w z (w + x + y) / den^2,
+    den = w^2 + w (x + y) + x y - z^2 = det C."""
+    w, x, y, z = AA_DILATION, a0, c0, b
+    den = w * w + w * (x + y) + x * y - z * z
+    if mutation == "aa_det_swapped":    # det C0 where det C belongs
+        den = x * y - z * z
+    den2 = den * den
+    dz = -2.0 * w * z * (w + x + y) / den2
+    if mutation == "aa_offdiag_not_halved":   # the symmetric-matrix entry given the whole dr/db
+        dz = 2.0 * dz
+    return w * (w * y + y * y + z * z) / den2, dz, w * (w * x + x * x + z * z) / den2
+
+
 def geom_forward(means3D, opacities, view, proj, campos, W, H, tan_fovx, tan_fovy, *, scales=None, rotations=None,
-                 scale_modifier=1.0, cov3D_precomp=None, shs=None, D=0):
+                 scale_modifier=1.0, cov3D_precomp=None, shs=None, D=0, antialiasing=False):
     """forward.cu:155-256 for every Gaussian.  Inputs are the fp32 arrays the kernel read.  Returns AV outputs
     depth (P,), means2D (P, 2), conic (P, 3), cov3D (P, 6) (from scale / rotation only), rgb (P, 3) (SH only),
     the integers radii, tiles_touched, rect (P, 4) = (xmin, ymin, xmax, ymax), clamped (P, 3), the masks near
-    (culled by the near plane) and visible (radius > 0), kappa, and fragile (P,)."""
+    (culled by the near plane) and visible (radius > 0), kappa, and fragile (P,).  With antialiasing also AV aa_h
+    (the opacity factor h, unsigned), aa_opacity (o h) and aa_cov0 (P, 3) = (a0, b, c0), the mask aa_active (r above
+    the floor), and r within the fragile band of the floor makes a Gaussian fragile (see _aa_factor)."""
     dev = torch.as_tensor(means3D).device
     cam = _camera(view, proj, campos, W, H, tan_fovx, tan_fovy)
     P = means3D.shape[0]
@@ -268,9 +305,10 @@ def geom_forward(means3D, opacities, view, proj, campos, W, H, tan_fovx, tan_fov
     T = _T(t, tcl, cam)
     V = _sym(cov6)
     TV = [[T[i][0] * V[0][j] + T[i][1] * V[1][j] + T[i][2] * V[2][j] for j in range(3)] for i in range(2)]
-    a = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2] + LOWPASS
+    a0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2]
     b = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2]
-    c = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2] + LOWPASS
+    c0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2]
+    a, c = a0 + LOWPASS, c0 + LOWPASS
     det = a * c - b * b                                                  # forward.cu:219-223
     det_inv = 1.0 / det
     conic = [c * det_inv, -b * det_inv, a * det_inv]
@@ -304,6 +342,11 @@ def geom_forward(means3D, opacities, view, proj, campos, W, H, tan_fovx, tan_fov
                opacity=_f64(opacities, dev).reshape(-1))
     if cov3D_precomp is None:
         out["cov3D"] = stack(cov6)
+    if antialiasing:
+        h, active, band = _aa_factor(a0, b, c0)
+        fragile |= band & visible
+        out.update(aa_h=h, aa_active=active, aa_cov0=stack([a0, b, c0]),
+                   aa_opacity=_exact(out["opacity"], dev) * h)
     if shs is not None:
         # computeColorFromSH (forward.cu:20-71)
         _, d = _sh_dir(means3D, cam["campos"], dev)
@@ -320,21 +363,28 @@ def geom_forward(means3D, opacities, view, proj, campos, W, H, tan_fovx, tan_fov
     return out
 
 
-# mutations of the backward, each a plausible kernel bug (tests/test_geom_ref_cpu.py shows the comparison rejects them)
+# mutations of the backward, each a plausible kernel bug (tests/test_geom_ref_cpu.py and
+# tests/test_antialias_ref_cpu.py show the comparison rejects them)
+AA_MUTATIONS = ("aa_offdiag_not_halved", "aa_cov_on_floor", "aa_dopacity_not_scaled", "aa_det_swapped",
+                "aa_h_squared")
 MUTATIONS = ("no_clamp_mask", "conic_xy_not_halved", "cov_offdiag_not_doubled", "scale_times_modifier",
              "quat_xyzw", "no_sh_direction", "clamped_not_zeroed", "y1_sign")
 
 
 def geom_backward(means3D, radii, view, proj, campos, W, H, tan_fovx, tan_fovy, cov3D, dL_dmeans2D, dL_dconic, *,
                   scales=None, rotations=None, scale_modifier=1.0, shs=None, D=0, clamped=None, dL_dcolors=None,
-                  det_reg=True, mutation=None):
+                  det_reg=True, mutation=None, antialiasing=False, opacities=None, dL_dopacity=None):
     """backward.cu:20-391 for every Gaussian with radii > 0, on the inputs the geometry kernel reads: the fp32 cov3D
     of the forward state (or cov3D_precomp), clamped flags, and the blend's dL_dmeans2D (P, 3) (NDC units),
     dL_dconic (P, 4) (x, y, _, w, with y halved as the blend writes it) and dL_dcolors (P, 3).  Returns AV
     dL_dmeans3D (P, 3), dL_dcov3D (P, 6), and with scale / rotation dL_dscales (P, 3), dL_drotations (P, 4), with
     SH dL_dsh (P, M, 3); Gaussians with radii == 0 get exact zeros.  det_reg=False drops the 1e-7 of
-    backward.cu:200 (for finite differences of geom_forward).  mutation: one of MUTATIONS."""
-    assert mutation is None or mutation in MUTATIONS, mutation
+    backward.cu:200 (for finite differences of geom_forward).  mutation: one of MUTATIONS or AA_MUTATIONS.
+    antialiasing: dL_dopacity (P,) is g = dL/d(o h), the blend's gradient of the opacity it read, and opacities (P,)
+    the raw o.  Returns also AV dL_dopacity = h g, and on the branch above the floor (o g / (2 h)) dr/d(a0, b, c0)
+    joins dL/d(a, b, c) before the covariance -> means3D / cov3D / scale / rotation chain (nothing on the floor)."""
+    assert mutation is None or mutation in MUTATIONS + AA_MUTATIONS, mutation
+    assert not antialiasing or (opacities is not None and dL_dopacity is not None)
     dev = torch.as_tensor(means3D).device
     cam = _camera(view, proj, campos, W, H, tan_fovx, tan_fovy)
     vm, pm, fx, fy = cam["view"], cam["proj"], cam["fx"], cam["fy"]
@@ -356,9 +406,10 @@ def geom_backward(means3D, radii, view, proj, campos, W, H, tan_fovx, tan_fovy, 
     T = _T(t, tcl, cam)
     V = _sym(cov6)
     TV = [[T[i][0] * V[0][j] + T[i][1] * V[1][j] + T[i][2] * V[2][j] for j in range(3)] for i in range(2)]
-    a = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2] + LOWPASS
+    a0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2]
     b = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2]
-    c = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2] + LOWPASS
+    c0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2]
+    a, c = a0 + LOWPASS, c0 + LOWPASS
     denom = a * c - b * b
     d2 = denom * denom
     # det^2 + 1e-7: the reference's regulariser, visible in its outputs (:200)
@@ -367,6 +418,20 @@ def geom_backward(means3D, radii, view, proj, campos, W, H, tan_fovx, tan_fovy, 
     dL_da = inv * (-1.0 * c * c * gx + 2.0 * b * c * gy + (denom - a * c) * gz)
     dL_dc = inv * (-1.0 * a * a * gz + 2.0 * a * b * gy + (denom - a * c) * gx)
     dL_db = inv * 2.0 * (b * c * gx - (denom + 2.0 * b * b) * gy + a * b * gz)
+    out = {}
+    if antialiasing:
+        # 3DGS backward.cu with antialiasing: dL/do = h g, and dL/dr = o g / (2 h) above the floor
+        h, active, _ = _aa_factor(a0, b, c0)
+        if mutation == "aa_h_squared":
+            h = h * h
+        g = _exact(_f64(dL_dopacity, dev).reshape(P), dev)
+        og = _exact(_f64(opacities, dev).reshape(P), dev) * g
+        out["dL_dopacity"] = g if mutation == "aa_dopacity_not_scaled" else h * g
+        g_r = og / (2.0 * h)
+        on = active | (mutation == "aa_cov_on_floor")
+        g_r = _where(on, g_r, AV(torch.zeros_like(g_r.v)))
+        dx, dz, dy = _aa_dr(a0, b, c0, mutation)
+        dL_da, dL_db, dL_dc = dL_da + g_r * dx, dL_db + g_r * dz, dL_dc + g_r * dy
     # :214-224: the diagonal entries once, the off-diagonal ones doubled (each appears twice in Vrk)
     off = 1.0 if mutation == "cov_offdiag_not_doubled" else 2.0
     T0, T1 = T
@@ -407,7 +472,6 @@ def geom_backward(means3D, radii, view, proj, campos, W, H, tan_fovx, tan_fovy, 
     for j in range(3):
         g_mean[j] = g_mean[j] + ((pm[4 * j] * m_w - pm[4 * j + 3] * mul1) * gmx
                                  + (pm[4 * j + 1] * m_w - pm[4 * j + 3] * mul2) * gmy)
-    out = {}
 
     # ---- SH colour (backward.cu:20-136)
     if shs is not None:

@@ -83,9 +83,11 @@ def _gen(seed):
 
 
 # ---------------------------------------------------------------- 1. against float64, per view (C ABI driver)
-def _native(scene, cams, *, C=3, sh_degree=None, cov=False, joint_c=0, seed=0):
+def _native(scene, cams, *, C=3, sh_degree=None, cov=False, joint_c=0, seed=0, antialiasing=False):
     """Forward through rasterizer._forward and backward through sgb_backward_[joint_]batch_cam with per-view gradient
-    buffers the test owns; returns per view the camera gradient (35) and the inputs of camera_ref.camera_terms."""
+    buffers the test owns; returns per view the camera gradient (35) and the inputs of camera_ref.camera_terms (with
+    antialiasing also the raw opacities, the blends' dL/d(o h), recovered as dL_dopacity / |h|, and the branch the
+    kernel took, the sign of h)."""
     lib = _lib.load()
     P = scene.P
     t = lambda a: torch.as_tensor(a, device=DEV).contiguous()  # noqa: E731
@@ -106,7 +108,7 @@ def _native(scene, cams, *, C=3, sh_degree=None, cov=False, joint_c=0, seed=0):
            math.tan(c.FoVy * 0.5)) for c in cams]
     native, (R, color, radii, geom, binning, img, depth, _, _, *feat) = rasterizer._forward(
         bool(joint_c), "test", cl, bg, xyz, colors, opac, scales, rots, 1.0, cov3D, H, W, sh,
-        sh_degree or 0, False, False, C, features=feats, bg_features=bgf)
+        sh_degree or 0, False, False, C, features=feats, bg_features=bgf, antialiasing=antialiasing)
     inp, cameras, _, _ = native
     V = len(cams)
     z = lambda *s: torch.zeros(s, device=DEV)  # noqa: E731
@@ -135,14 +137,19 @@ def _native(scene, cams, *, C=3, sh_degree=None, cov=False, joint_c=0, seed=0):
     torch.cuda.synchronize()
     out = []
     for v in range(V):
-        st = read_state(lib, P, R[v], W, H, geom[v], binning[v], img[v], ("cov3D", "clamped"))
+        st = read_state(lib, P, R[v], W, H, geom[v], binning[v], img[v], ("cov3D", "clamped", "aa_h"))
         c = cams[v]
+        kw = dict(shs=sh, D=sh_degree or 0, clamped=st["clamped"], dL_dcolors=grads[v]["col"])
+        if antialiasing:
+            live = radii[v] > 0
+            g_oh = torch.where(live, grads[v]["opac"].double() / st["aa_h"].abs().double().clamp(min=1e-30),
+                               torch.zeros_like(grads[v]["opac"].double()))
+            kw.update(antialiasing=True, opacities=opac.reshape(-1), dL_dopacity=g_oh, aa_active=st["aa_h"] > 0)
         out.append(dict(cam=cam_out[v].cpu(), args=(xyz, radii[v], cov3D if cov else st["cov3D"],
                                                     np.asarray(c.world_view_transform), np.asarray(c.full_proj_transform),
                                                     np.asarray(c.camera_center), W, H, math.tan(c.FoVx * 0.5),
                                                     math.tan(c.FoVy * 0.5), grads[v]["m2"], grads[v]["conic"]),
-                        kw=dict(shs=sh, D=sh_degree or 0, clamped=st["clamped"], dL_dcolors=grads[v]["col"]),
-                        grads=grads[v]))
+                        kw=kw, grads=grads[v]))
     return out
 
 

@@ -40,28 +40,29 @@ def _placed(t, offset_bytes):
     return v
 
 
-def _native(sc, cams, W, H, Cn):
+def _native(sc, cams, W, H, Cn, antialiasing=False):
     """(ViewInputs of the Gaussians without colours, sgb_camera array, the tensors they point into)."""
     cms = [dev_cam(c, DEV) for c in cams]
     inp = _lib.ViewInputs(P=sc["means3D"].shape[0], D=0, M=0, W=W, H=H, C=Cn, background=None,
                           means3D=sc["means3D"].data_ptr(), shs=None, colors_precomp=None,
                           opacities=sc["opacities"].data_ptr(), scales=sc["scales"].data_ptr(), scale_modifier=1.0,
                           rotations=sc["rotations"].data_ptr(), cov3D_precomp=None, viewmatrix=None, projmatrix=None,
-                          campos=None, tan_fovx=0.0, tan_fovy=0.0, prefiltered=0, debug=0)
+                          campos=None, tan_fovx=0.0, tan_fovy=0.0, prefiltered=0, debug=0,
+                          antialiasing=int(bool(antialiasing)))
     cam_arr = (_lib.Camera * len(cams))(*[_lib.Camera(c["viewmatrix"].data_ptr(), c["projmatrix"].data_ptr(),
                                                       c["campos"].data_ptr(), c["tanfovx"], c["tanfovy"]) for c in cms])
     return inp, cam_arr, cms
 
 
-def forward_states(sc, cams, W, H):
+def forward_states(sc, cams, W, H, antialiasing=False):
     """Every view's kernel state (means2D, conic_opacity, point_list, ranges, final_T) from C = 8 forwards of at most
     8 views on a fresh ctx; None for a view without instances."""
     if len(cams) > _lib.MAX_BATCH:
         return [st for lo in range(0, len(cams), _lib.MAX_BATCH)
-                for st in forward_states(sc, cams[lo:lo + _lib.MAX_BATCH], W, H)]
+                for st in forward_states(sc, cams[lo:lo + _lib.MAX_BATCH], W, H, antialiasing)]
     lib = _lib.load()
     V, P = len(cams), sc["means3D"].shape[0]
-    inp, cam_arr, keep = _native(sc, cams, W, H, 8)
+    inp, cam_arr, keep = _native(sc, cams, W, H, 8, antialiasing)
     feats, bg = torch.zeros((P, 8), device=DEV), torch.zeros(8, device=DEV)
     inp.colors_precomp, inp.background = feats.data_ptr(), bg.data_ptr()
     ptrs = lambda ts: (Ct.c_void_p * V)(*[t.data_ptr() for t in ts])
@@ -86,12 +87,12 @@ def forward_states(sc, cams, W, H):
         lib.sgb_ctx_destroy(ctx)
 
 
-def lift_native(sc, cams, W, H, maps, ctx=None):
+def lift_native(sc, cams, W, H, maps, ctx=None, antialiasing=False):
     """sgb_lift_batch of len(cams) views (maps: (C, H, W) tensors of one dtype) on a fresh ctx or the one given.
     Returns (feat_sum, weight_sum, weight-pool chunks of the last view)."""
     lib = _lib.load()
     V, P, Cn = len(cams), sc["means3D"].shape[0], maps[0].shape[0]
-    inp, cam_arr, keep = _native(sc, cams, W, H, Cn)
+    inp, cam_arr, keep = _native(sc, cams, W, H, Cn, antialiasing)
     fs, ws = torch.zeros((P, Cn), device=DEV), torch.zeros(P, device=DEV)
     dt = _lib.FEAT_F16 if maps[0].dtype == F16 else _lib.FEAT_F32
     own = ctx is None
@@ -110,12 +111,13 @@ def lift_native(sc, cams, W, H, maps, ctx=None):
     return fs, ws, chunks
 
 
-def check_lift(scene, cams, Cn, dtype, *, map_offset=0, seed=0):
+def check_lift(scene, cams, Cn, dtype, *, map_offset=0, seed=0, antialiasing=False):
     """Lift random maps (zero at each view's fragile pixels) of len(cams) views natively and compare feat_sum and
-    weight_sum with the sum of the views' float64 restatements.  Returns the errors and statistics."""
+    weight_sum with the sum of the views' float64 restatements (on the kernels' state: with antialiasing the
+    record's opacity is o h).  Returns the errors and statistics."""
     W, H = cams[0].image_width, cams[0].image_height
     sc = dev_scene(scene, DEV)
-    states = forward_states(sc, cams, W, H)
+    states = forward_states(sc, cams, W, H, antialiasing)
     g = torch.Generator(device=DEV).manual_seed(seed)
     P = scene.P
     want_f = torch.zeros((P, Cn), dtype=torch.float64, device=DEV)
@@ -138,7 +140,7 @@ def check_lift(scene, cams, Cn, dtype, *, map_offset=0, seed=0):
             rg = st["ranges"].long()
             lens.append(rg[:, 1] - rg[:, 0])
         maps.append(_placed(m, map_offset))
-    fs, ws, chunks = lift_native(sc, cams, W, H, maps)
+    fs, ws, chunks = lift_native(sc, cams, W, H, maps, antialiasing=antialiasing)
     seen = want_w > 0
     assert int(seen.sum()) > 0 and int((ok & seen).sum()) > 0
     errs = dict(feat_sum=br.compare(fs, want_f), weight_sum=br.compare(ws[ok], want_w[ok]))
