@@ -12,10 +12,13 @@
 //                     (forward.cu:326-363) -> final_T, n_contrib, and for every Gaussian that
 //                     touches the tile a 1 KB row of weights w[pixel] = alpha * T (0 where the
 //                     pixel skips it) appended to a per-tile linked list of 16-entry chunks.
-//   blend_forward     CTA = (tile, 64-channel chunk): the tile's weight rows and feature slices
-//                     stream through a TMA-fed shared-memory ring (plain loads from L2 when the
-//                     feature rows are not 16-byte aligned slices) and every lane accumulates an
-//                     8 px x 8 ch register micro-tile (outer product, paired FMAs).
+//   blend_forward     persistent CTAs claim (tile, up to 128 channels) items: a producer warp
+//                     streams the tile's 16-entry pool chunks (weight rows and the item's feature
+//                     slices, by bulk copy, or staged with cp.async when the feature rows are not
+//                     16-byte aligned slices) through one ring, every compute warp owns a 32-pixel
+//                     strip and all the item's channels, every lane an 8 px x 16 ch register tile
+//                     (setmaxnreg moves the producer group's registers to the compute groups); the
+//                     output leaves through shared memory as TMA tensor stores.
 //   chain_backward    CTA = tile, warp = 32-pixel strip: s = <feature, dL/dout> per (pixel,
 //                     Gaussian) for all channels over the strip's own entries (register
 //                     micro-tiles), then the reference's back-to-front chain (backward.cu:477-550)
@@ -49,7 +52,7 @@ int chn_chain(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const float*
 // With the weights materialised per tile, the three C-wide contractions are small dense GEMMs over the
 // tile's touching Gaussians (G ~ 115 on K3), done in fp32 on the CUDA cores (north_star: no tensor cores;
 // the 1e-4 fp32 bar rules out TF32 anyway):
-//     forward   out[256 px][64 ch]  = W^T[256 px][G]  . F[G][64 ch]      K = G      lane tile 8 px x 8 ch
+//     forward   out[256 px][128 ch] = W^T[256 px][G]  . F[G][128 ch]     K = G      lane tile 8 px x 16 ch
 //     s-pass    S[32 px][32]        = dL[32 px][C]    . F^T[C][32]       K = C      lane tile 8 px x 4 entries
 //               (per warp: its strip and a 32-entry segment of the strip's entries)
 //     dfeature  dF[G][256 ch]       = W[G][256 px]    . dL[256 px][256]  K = 256 px lane tile <= 8 entries x 16 ch

@@ -89,15 +89,6 @@ __device__ __forceinline__ float4 df_dl4(const __half* dl, int q, int k, int swz
     return make_float4(a.x, a.y, b.x, b.y);
 }
 
-__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src, int src_bytes) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes)
-                 : "memory");
-}
-// Arrives on `bar` once every cp.async this thread issued so far has landed (the arrival is part of the init count).
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // One 32-pixel slab of a pass: acc[j][4g + k] += sum over the slab of w[eg + 16j][px] * dL[px][cl + 8g + k], g < 4.
 // dl points at channel cl of the stage's dL slab, ws at its weight rows; swz = df_swz<T>(cl), rs the dL row pitch.
 template <int R, typename T>

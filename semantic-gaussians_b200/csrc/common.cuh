@@ -165,7 +165,7 @@ struct sgb_ctx {
     sgb::Scratch geom;     // depth-sort keys, iota values, CUB temp, 64-bit instance total (shared by a batch's views)
     sgb::Scratch bin;      // unsorted / sorted tile keys, unsorted values, CUB temp
     sgb::Scratch misc;     // fusion: pixel-sorted visible list, z-buffer
-    sgb::Scratch work;     // work-item counters of the persistent kernels (chn_dfeature.cu)
+    sgb::Scratch work;     // work-item counter of the persistent kernels (chn_forward.cu, chn_dfeature.cu)
     sgb::Scratch depth_grad;  // [P] dL/d(view-space z) of the view being differentiated (expected-depth backward)
     sgb::Scratch cam_partial; // per-CTA fp64 camera-gradient partials of the view being differentiated
     sgb::Scratch lift_state;  // sgb_lift_batch: geometry state, radii and image state of every view of the call

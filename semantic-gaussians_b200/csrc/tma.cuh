@@ -94,6 +94,29 @@ __device__ __forceinline__ void tma_tile3d_g2s(void* dst_smem, const CUtensorMap
         "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar))
         : "memory");
 }
+// 3-D tensor tile shared -> global through the TMA engine (SASS: UTMASTG), committed to this thread's bulk group: box
+// corner (x, y, z) in elements, elements outside the tensor are not written.  src 16-byte aligned; the generic-proxy
+// writes that filled it must be ordered before by fence_proxy_async_smem.
+__device__ __forceinline__ void tma_store3d_s2g(const CUtensorMap* map, int x, int y, int z, const void* src_smem) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(
+                     reinterpret_cast<uint64_t>(map)),
+                 "r"(x), "r"(y), "r"(z), "r"(smem_u32(src_smem))
+                 : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+// Waits until this thread's committed bulk stores have read their shared-memory sources (the buffer may be rewritten).
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// Waits until this thread's committed bulk stores have completed.
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// 4-byte cp.async global -> shared; src_bytes 0 writes a zero instead of reading src.
+__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src, int src_bytes) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes)
+                 : "memory");
+}
+// Arrives on `bar` once every cp.async this thread issued so far has landed (the arrival is part of the init count).
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 // Orders this thread's earlier generic-proxy shared-memory accesses before later async-proxy (TMA) writes.
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
