@@ -2,7 +2,7 @@
 #include <cstddef>
 #include <cstring>
 #include "chn_blend.cuh"
-#include "tma.cuh"
+#include "persistent.cuh"
 
 namespace sgb {
 
@@ -24,9 +24,9 @@ namespace {
 //     channels 32w + 4h + 8g + {0..3}, g < 4, in 128 scalar registers, R = ceil(entries / 16) <= 8: per 4-pixel K step
 //     64R FMAs for R + 16 LDS.128 (512 per 24 at R = 8).  (16 warps of 16 channels, 64 accumulators each, would leave
 //     a compute thread at most 120 registers, and ptxas spills the slab loop at that limit.)
-// Every hand-off is a full/empty mbarrier pair; there is no CTA-wide barrier after the set-up.  Each accumulator adds
-// the pixels of the tile in order 0..255, and each (Gaussian, tile, 4 channels) is one 16-byte reduction.  The TMA
-// swizzles keep every operand load at 2 shared-memory wavefronts or less, 1 for dL (see lane_group8):
+// Each accumulator adds the pixels of the tile in order 0..255, and each (Gaussian, tile, 4 channels) is one 16-byte
+// reduction.  The TMA swizzles keep every operand load at 2 shared-memory wavefronts or less, 1 for dL (see
+// lane_group8):
 //   * weights, SWIZZLE_128B: quad q of the 128-byte row e sits at q ^ (e & 7); each 4-lane group reads 2 rows and each
 //     half-warp 8 consecutive rows -> 8 distinct bank groups;
 //   * dL, SWIZZLE_64B over a [row][ch][16 px] box: quad p of channel c sits at p ^ ((c >> 1) & 3), so channels c and
@@ -39,7 +39,7 @@ constexpr int kDfSlabs = SGB_TILE_PIX / kDfSlabPix;
 constexpr int kDfComputeWarps = kDfCH / 32;                // 2 warp groups, 32 channels per warp
 constexpr int kDfThreads = 128 + 32 * kDfComputeWarps;  // producer warp group + 2 compute warp groups
 constexpr uint32_t kDfProducerRegs = 56, kDfComputeRegs = 224;
-static_assert(128 * kDfProducerRegs + 32 * kDfComputeWarps * kDfComputeRegs <= 65536,
+static_assert(warp_group_regs_fit(kDfProducerRegs, kDfComputeWarps, kDfComputeRegs),
               "dL/dfeature: the warp groups' register limits exceed the register file");
 
 struct DfHdr {  // one ring stage's description, written by the producer before the stage is armed
@@ -55,19 +55,11 @@ template <typename T>
 struct DfSmem {  // at a 1024-byte aligned offset of the dynamic shared memory (TMA swizzle atoms)
     float w[kDfStages][kDfPass * kDfSlabPix];
     T dl[kDfStages][kDfSlabPix * kDfCH];
-    DfHdr hdr[kDfStages];
-    uint64_t full[kDfStages], empty[kDfStages];
+    MbarRing<kDfStages, DfHdr> ring;
 };
 template <typename T>
 constexpr size_t kDfSmemBytes = sizeof(DfSmem<T>) + 1024;
 static_assert(kDfSmemBytes<float> <= 227 * 1024, "dL/dfeature shared memory exceeds the sm_90 opt-in limit");
-
-__device__ __forceinline__ void df_setmaxnreg_dec() {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kDfProducerRegs));
-}
-__device__ __forceinline__ void df_setmaxnreg_inc() {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kDfComputeRegs));
-}
 
 // Pixels 4 (q & 3) .. 4 (q & 3) + 3 of slab row q >> 2, channel cl + k, of a stage's dL slab; dl points at channel cl
 // (a multiple of 4) of row 0, rs is the row pitch in elements (16 x the item's channels) and swz = df_swz<T>(cl).  The
@@ -122,18 +114,11 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
     extern __shared__ __align__(128) unsigned char smem_raw[];
     DfSmem<T>& sm = *reinterpret_cast<DfSmem<T>*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) {
-        for (int i = 0; i < kDfStages; i++) {
-            // the producer lane 0's arrive.expect_tx, and without TMA one arrival per producer lane for its dL copies
-            mbar_init(&sm.full[i], use_tma ? 1 : 33);
-            mbar_init(&sm.empty[i], kDfComputeWarps);
-        }
-        mbar_fence_init();
-    }
+    if (tid == 0) sm.ring.init(!use_tma, kDfComputeWarps);
     __syncthreads();
 
     if (warp >= 4) {
-        df_setmaxnreg_inc();
+        setmaxnreg_inc<kDfComputeRegs>();
         const int cw = warp - 4;
         const int eg = lane >> 1;
         const int cl = cw * 32 + (lane & 1) * 4;  // channel (within the item) of k = 0; k = 4g..4g+3 are cl + 8g + {0..3}
@@ -142,9 +127,8 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
         const bool red16 = ((C & 3) == 0) && ((reinterpret_cast<uintptr_t>(dL_dcolors) & 15) == 0);
         float acc[8][16];
         for (uint32_t step = 0;; step++) {
-            const int st = (int)(step % kDfStages);
-            mbar_wait(&sm.full[st], (step / kDfStages) & 1u);
-            const DfHdr& h = sm.hdr[st];
+            const int st = sm.ring.wait(step);
+            const DfHdr& h = sm.ring.hdr[st];
             if (h.end) break;
             const int slab = h.slab, cnt = h.cnt, nch = h.nch;
             const int R = (cnt + 15) >> 4;
@@ -189,14 +173,13 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
                     }
                 }
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.empty[st]);
+            sm.ring.release(st, lane);
         }
         return;
     }
 
     // ---- producer warp group: warp 0 streams, warps 1-3 only hand their registers back
-    df_setmaxnreg_dec();
+    setmaxnreg_dec<kDfProducerRegs>();
     if (warp != 0) return;
     const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
     const int tiles = tiles_x * ((H + SGB_TILE - 1) / SGB_TILE);
@@ -205,15 +188,8 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
     const size_t plane = (size_t)H * W;
     const uint32_t dl_bytes = use_tma ? (uint32_t)(kDfSlabPix * CW * sizeof(T)) : 0u;
     uint32_t step = 0;  // ring stages armed so far
-    auto acquire = [&]() -> int {  // next ring stage, once the compute warps released its previous use
-        const int st = (int)(step % kDfStages);
-        if (step >= kDfStages) mbar_wait(&sm.empty[st], ((step / kDfStages) - 1) & 1u);
-        return st;
-    };
     for (;;) {
-        int k = 0;
-        if (lane == 0) k = atomicAdd(work_counter, 1);
-        k = __shfl_sync(0xffffffffu, k, 0);
+        const int k = claim_item(work_counter, lane);
         if (k >= total) break;
         const int tile = k / nitems, ch0 = (k % nitems) * CW;
         const uint32_t n = pool.count[tile];
@@ -233,8 +209,8 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
                 gid[i] = e < cnt ? pool.chunks[c].meta[e & (kChunkEntries - 1)].x : 0u;
             }
             for (int s = 0; s < kDfSlabs; s++) {
-                const int st = acquire();
-                DfHdr& h = sm.hdr[st];
+                const int st = sm.ring.acquire(step);
+                DfHdr& h = sm.ring.hdr[st];
                 if (lane == 0) {
                     h.end = 0;
                     h.cnt = cnt;
@@ -247,11 +223,11 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
                     for (int i = 0; i < kDfPass / 32; i++) h.gid[lane + 32 * i] = gid[i];
                 }
                 if (lane < nck)
-                    tma_tile3d_g2s(&sm.w[st][lane * kChunkEntries * 32], &w_map, 32 * s, 0, (int)cid, &sm.full[st]);
+                    tma_tile3d_g2s(&sm.w[st][lane * kChunkEntries * 32], &w_map, 32 * s, 0, (int)cid, &sm.ring.full[st]);
                 const int ys = y0 + 2 * s;  // first tile row of the slab
                 T* dst = sm.dl[st];
                 if (use_tma) {
-                    if (lane == 0) tma_tile3d_g2s(dst, &dl_map, x0, ch0, ys, &sm.full[st]);
+                    if (lane == 0) tma_tile3d_g2s(dst, &dl_map, x0, ch0, ys, &sm.ring.full[st]);
                 } else if constexpr (sizeof(T) == 2) {
                     // cp.async has no 2-byte size: plain loads into the TMA layout, then one release-arrive per lane
 #pragma unroll 1
@@ -262,7 +238,7 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
                         dst[r * CW * 16 + c * 16 + ((((x >> 3) ^ ((c >> 2) & 1)) << 3) | (x & 7))] =
                             ok ? dL_dpixels[(size_t)(ch0 + c) * plane + (size_t)W * gy + gx] : T(0.f);
                     }
-                    mbar_arrive(&sm.full[st]);
+                    mbar_arrive(&sm.ring.full[st]);
                 } else {
 #pragma unroll 1
                     for (int idx = lane; idx < 2 * 16 * CW; idx += 32) {
@@ -273,20 +249,16 @@ __global__ void __launch_bounds__(kDfThreads, 1) dfeature_persistent_kernel(
                         cp_async4(dst + r * CW * 16 + c * 16 + ((((x >> 2) ^ ((c >> 1) & 3)) << 2) | (x & 3)), src,
                                   ok ? 4 : 0);
                     }
-                    cp_async_mbar_arrive_noinc(&sm.full[st]);
+                    cp_async_mbar_arrive_noinc(&sm.ring.full[st]);
                 }
                 __syncwarp();
                 if (lane == 0)
-                    mbar_arrive_expect_tx(&sm.full[st], (uint32_t)nck * (kChunkEntries * 32 * 4) + dl_bytes);
+                    mbar_arrive_expect_tx(&sm.ring.full[st], (uint32_t)nck * (kChunkEntries * 32 * 4) + dl_bytes);
                 step++;
             }
         }
     }
-    const int st = acquire();
-    if (lane == 0) sm.hdr[st].end = 1;
-    __syncwarp();
-    if (!use_tma) mbar_arrive(&sm.full[st]);
-    if (lane == 0) mbar_arrive(&sm.full[st]);
+    sm.ring.finish(step, !use_tma, lane);
 }
 
 }  // namespace
@@ -324,10 +296,9 @@ template <typename T>
 static int launch_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, const T* dL_dpix, float* dL_dcolors,
                            cudaStream_t s) {
     const sgb_view_inputs& in = w.in;
-    // items of equal width per tile: one at C <= 256, two at C = 512
-    const int nitems = (in.C + kDfCH - 1) / kDfCH;
-    const int CW = ((in.C + nitems - 1) / nitems + 15) / 16 * 16;
-    const int items = num_tiles(in) * nitems;
+    const ItemSplit sp = split_channels(in.C, kDfCH);  // one item at C <= 256, two at C = 512
+    const int CW = sp.CW;
+    const int items = num_tiles(in) * sp.nitems;
     if (items == 0) return SGB_OK;
     CUtensorMap dl_map, w_map;
     const int use_tma = encode_dfeature_dl_map(&dl_map, dL_dpix, in.W, in.H, in.C, CW) ? 1 : 0;
@@ -335,29 +306,13 @@ static int launch_dfeature(sgb_ctx* ctx, const ViewState& w, const PoolView& pv,
         set_error("dL/dfeature: cuTensorMapEncodeTiled is unavailable or rejected the weight pool");
         return SGB_E_CUDA;
     }
-    int rc = ctx->work.ensure(sizeof(int));
-    if (rc) return rc;
-    // persistent grid: as many CTAs as are co-resident on the device
-    static DeviceOnce attr_set;
-    static int grid_of_device[64];
-    int dev = 0;
-    SGB_CUDA(cudaGetDevice(&dev));
-    int& grid = grid_of_device[dev < 64 ? dev : 63];
-    if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(dfeature_persistent_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)kDfSmemBytes<T>));
-        int per_sm = 0, sms = 0;
-        SGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dfeature_persistent_kernel<T>, kDfThreads,
-                                                               kDfSmemBytes<T>));
-        SGB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        grid = per_sm * sms > 0 ? per_sm * sms : 1;
-    }
-    int* counter = static_cast<int*>(ctx->work.p);
     StageTimer t(ctx, ST_DFEATURE, s);
-    SGB_CUDA(cudaMemsetAsync(counter, 0, sizeof(int), s));
+    int grid = 0;
+    const int rc = persistent_grid<dfeature_persistent_kernel<T>>(ctx, kDfThreads, kDfSmemBytes<T>, items, s, &grid);
+    if (rc) return rc;
     ctx->launches += 1;
-    dfeature_persistent_kernel<T><<<grid < items ? grid : items, kDfThreads, kDfSmemBytes<T>, s>>>(
-        in.W, in.H, in.C, CW, dL_dpix, pv, dL_dcolors, counter, dl_map, w_map, use_tma);
+    dfeature_persistent_kernel<T><<<grid, kDfThreads, kDfSmemBytes<T>, s>>>(
+        in.W, in.H, in.C, CW, dL_dpix, pv, dL_dcolors, static_cast<int*>(ctx->work.p), dl_map, w_map, use_tma);
     SGB_LAUNCH_CHECK("dfeature_persistent_kernel", in.debug, s);
     return SGB_OK;
 }

@@ -1,7 +1,7 @@
 // Forward contraction of the C-channel blend (chn_blend.cuh): out[px][ch] = sum over the tile's weight rows.
 #include <cstring>
 #include "chn_blend.cuh"
-#include "tma.cuh"
+#include "persistent.cuh"
 
 namespace sgb {
 
@@ -30,14 +30,13 @@ namespace {
 // together and stall on the store queue: about 0.57 of 3.24 ms at K3 (H100 80GB HBM3, 700 W).  The output boxes
 // (128 KB) leave room for a ring of 4 stages.  Plain stores remain for rows that are not 16-byte multiples
 // (W % 4 != 0) or an unaligned output.
-// Every hand-off is a full/empty mbarrier pair; there is no CTA-wide barrier after the set-up.
 // Each accumulator starts at 0 and adds the tile's entries 0 .. n-1 in order with fmaf.
 constexpr int kFwCH = 128;                   // widest work item (channels)
 constexpr int kFwStages = 4;                 // ring depth (one 16-entry pool chunk per stage)
 constexpr int kFwComputeWarps = SGB_TILE_PIX / 32;     // 2 warp groups, one 32-pixel strip per warp
 constexpr int kFwThreads = 128 + 32 * kFwComputeWarps;  // producer warp group + 2 compute warp groups
 constexpr uint32_t kFwProducerRegs = 56, kFwComputeRegs = 224;
-static_assert(128 * kFwProducerRegs + 32 * kFwComputeWarps * kFwComputeRegs <= 65536,
+static_assert(warp_group_regs_fit(kFwProducerRegs, kFwComputeWarps, kFwComputeRegs),
               "forward: the warp groups' register limits exceed the register file");
 
 struct FwHdr {  // one ring stage's description, written by the producer before the stage is armed
@@ -54,18 +53,10 @@ struct FwStage {
 struct FwSmem {
     FwStage stg[kFwStages];
     float out[kFwComputeWarps][kFwCH][2][SGB_TILE];  // each compute warp's output box [channel][tile row][16 px]
-    FwHdr hdr[kFwStages];
-    uint64_t full[kFwStages], empty[kFwStages];
+    MbarRing<kFwStages, FwHdr> ring;
 };
 constexpr size_t kFwSmemBytes = sizeof(FwSmem);
 static_assert(kFwSmemBytes <= 227 * 1024, "forward shared memory exceeds the sm_90 opt-in limit");
-
-__device__ __forceinline__ void fw_setmaxnreg_dec() {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kFwProducerRegs));
-}
-__device__ __forceinline__ void fw_setmaxnreg_inc() {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kFwComputeRegs));
-}
 
 // Channel (within the item) of accumulator column k of lane group cg.
 __device__ __forceinline__ int fw_channel(int k, int cg) { return (k >> 2) * 32 + cg * 4 + (k & 3); }
@@ -173,18 +164,11 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
     FwSmem& sm = *reinterpret_cast<FwSmem*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tiles_x = (W + SGB_TILE - 1) / SGB_TILE;
-    if (tid == 0) {
-        for (int i = 0; i < kFwStages; i++) {
-            // the producer lane 0's arrive.expect_tx, and when staging one arrival per producer lane for its copies
-            mbar_init(&sm.full[i], use_bulk ? 1 : 33);
-            mbar_init(&sm.empty[i], kFwComputeWarps);
-        }
-        mbar_fence_init();
-    }
+    if (tid == 0) sm.ring.init(!use_bulk, kFwComputeWarps);
     __syncthreads();
 
     if (warp >= 4) {
-        fw_setmaxnreg_inc();
+        setmaxnreg_inc<kFwComputeRegs>();
         const int strip = warp - 4;
         const int pg = lane_group4(lane), cg = lane_group8(lane);
         const int woff = strip * 32 + pg * 8;  // this lane's 8 pixels (tile-local)
@@ -192,9 +176,8 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
         float acc[8][16];
         float Tl = 0.f, bgl[4] = {0.f, 0.f, 0.f, 0.f};  // final_T of strip pixel `lane`, bg of item channel lane + 32q
         for (uint32_t step = 0;; step++) {
-            const int st = (int)(step % kFwStages);
-            mbar_wait(&sm.full[st], (step / kFwStages) & 1u);
-            const FwHdr& h = sm.hdr[st];
+            const int st = sm.ring.wait(step);
+            const FwHdr& h = sm.ring.hdr[st];
             if (h.end) break;
             const int cnt = h.cnt, last = h.last, tile = h.tile, ch0 = h.ch0, nch = h.nch;
             const uint32_t n = h.n, dbase = h.dbase;
@@ -226,8 +209,7 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
                     }
                 }
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.empty[st]);
+            sm.ring.release(st, lane);
             if (!last) continue;
 
             // ---- epilogue: out = acc + T * bg (forward.cu:372-373)
@@ -283,21 +265,14 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
     }
 
     // ---- producer warp group: warp 0 streams, warps 1-3 only hand their registers back
-    fw_setmaxnreg_dec();
+    setmaxnreg_dec<kFwProducerRegs>();
     if (warp != 0) return;
     const int tiles = tiles_x * ((H + SGB_TILE - 1) / SGB_TILE);
     const int nitems = (C + CW - 1) / CW;
     const int total = tiles * nitems;
     uint32_t step = 0;  // ring stages armed so far
-    auto acquire = [&]() -> int {  // next ring stage, once the compute warps released its previous use
-        const int st = (int)(step % kFwStages);
-        if (step >= kFwStages) mbar_wait(&sm.empty[st], ((step / kFwStages) - 1) & 1u);
-        return st;
-    };
     for (;;) {
-        int k = 0;
-        if (lane == 0) k = atomicAdd(work_counter, 1);
-        k = __shfl_sync(0xffffffffu, k, 0);
+        const int k = claim_item(work_counter, lane);
         if (k >= total) break;
         const int tile = k / nitems, ch0 = (k % nitems) * CW;
         const int nch = min(CW, C - ch0);
@@ -328,8 +303,8 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
                 c_next = chunk_id(j + 1);
                 g_next = gid_of(c_next, j + 1);
             }
-            const int st = acquire();
-            FwHdr& h = sm.hdr[st];
+            const int st = sm.ring.acquire(step);
+            FwHdr& h = sm.ring.hdr[st];
             if (lane == 0) {
                 h.end = 0;
                 h.cnt = cnt;
@@ -343,31 +318,27 @@ __global__ void __launch_bounds__(kFwThreads, 1) blend_forward_persistent_kernel
             }
             FwStage& sg = sm.stg[st];
             if (cnt > 0 && lane == 0)
-                bulk_g2s(&sg.w[0][0], &pool.chunks[c_cur].w[0][0], (uint32_t)cnt * (SGB_TILE_PIX * 4u), &sm.full[st]);
+                bulk_g2s(&sg.w[0][0], &pool.chunks[c_cur].w[0][0], (uint32_t)cnt * (SGB_TILE_PIX * 4u), &sm.ring.full[st]);
             if (use_bulk) {
                 if (lane < cnt)
-                    bulk_g2s(&sg.f[lane][0], features + (size_t)g_cur * C + ch0, (uint32_t)nch * 4u, &sm.full[st]);
+                    bulk_g2s(&sg.f[lane][0], features + (size_t)g_cur * C + ch0, (uint32_t)nch * 4u, &sm.ring.full[st]);
             } else {
 #pragma unroll 1
                 for (int e = 0; e < cnt; e++) {
                     const float* src = features + (size_t)__shfl_sync(0xffffffffu, g_cur, e) * C + ch0;
                     for (int c = lane; c < nch4; c += 32) cp_async4(&sg.f[e][c], c < nch ? src + c : src, c < nch ? 4 : 0);
                 }
-                cp_async_mbar_arrive_noinc(&sm.full[st]);
+                cp_async_mbar_arrive_noinc(&sm.ring.full[st]);
             }
             __syncwarp();
             if (lane == 0)
-                mbar_arrive_expect_tx(&sm.full[st], (uint32_t)cnt * (SGB_TILE_PIX * 4u + (use_bulk ? (uint32_t)nch * 4u : 0u)));
+                mbar_arrive_expect_tx(&sm.ring.full[st], (uint32_t)cnt * (SGB_TILE_PIX * 4u + (use_bulk ? (uint32_t)nch * 4u : 0u)));
             step++;
             c_cur = c_next;
             g_cur = g_next;
         }
     }
-    const int st = acquire();
-    if (lane == 0) sm.hdr[st].end = 1;
-    __syncwarp();
-    if (!use_bulk) mbar_arrive(&sm.full[st]);
-    if (lane == 0) mbar_arrive(&sm.full[st]);
+    sm.ring.finish(step, !use_bulk, lane);
 }
 
 }  // namespace
@@ -389,38 +360,21 @@ static bool encode_forward_out_map(CUtensorMap* map, float* out, int W, int H, i
 // its step while the GEMM runs.
 int chn_forward(sgb_ctx* ctx, const ViewState& w, const PoolView& pv, float* out_color, cudaStream_t s) {
     const sgb_view_inputs& in = w.in;
-    // items of equal width per tile, a multiple of 16: one at C <= 128, two at C = 256, four at C = 512
-    const int nitems = (in.C + kFwCH - 1) / kFwCH;
-    const int CW = ((in.C + nitems - 1) / nitems + 15) / 16 * 16;
-    const int items = num_tiles(in) * nitems;
+    const ItemSplit sp = split_channels(in.C, kFwCH);  // one item at C <= 128, two at C = 256, four at C = 512
+    const int CW = sp.CW;
+    const int items = num_tiles(in) * sp.nitems;
     if (items == 0) return SGB_OK;
     const int use_bulk = (in.C % 4 == 0) && ((reinterpret_cast<uintptr_t>(w.colors) & 15) == 0);
     CUtensorMap out_map;
     const int use_tma_store = encode_forward_out_map(&out_map, out_color, in.W, in.H, in.C, CW) ? 1 : 0;
-    int rc = ctx->work.ensure(sizeof(int));
-    if (rc) return rc;
-    // persistent grid: as many CTAs as are co-resident on the device
-    static DeviceOnce attr_set;
-    static int grid_of_device[64];
-    int dev = 0;
-    SGB_CUDA(cudaGetDevice(&dev));
-    int& grid = grid_of_device[dev < 64 ? dev : 63];
-    if (attr_set.first_use_on_device()) {
-        SGB_CUDA(cudaFuncSetAttribute(blend_forward_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)kFwSmemBytes));
-        int per_sm = 0, sms = 0;
-        SGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blend_forward_persistent_kernel, kFwThreads,
-                                                               kFwSmemBytes));
-        SGB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        grid = per_sm * sms > 0 ? per_sm * sms : 1;
-    }
-    int* counter = static_cast<int*>(ctx->work.p);
     StageTimer t(ctx, ST_BLEND_FWD, s);
-    SGB_CUDA(cudaMemsetAsync(counter, 0, sizeof(int), s));
+    int grid = 0;
+    const int rc = persistent_grid<blend_forward_persistent_kernel>(ctx, kFwThreads, kFwSmemBytes, items, s, &grid);
+    if (rc) return rc;
     ctx->launches += 1;
-    blend_forward_persistent_kernel<<<grid < items ? grid : items, kFwThreads, kFwSmemBytes, s>>>(
-        in.W, in.H, in.C, CW, w.colors, in.background, w.im.final_T, pv, out_color, counter, use_bulk, out_map,
-        use_tma_store);
+    blend_forward_persistent_kernel<<<grid, kFwThreads, kFwSmemBytes, s>>>(
+        in.W, in.H, in.C, CW, w.colors, in.background, w.im.final_T, pv, out_color, static_cast<int*>(ctx->work.p),
+        use_bulk, out_map, use_tma_store);
     SGB_LAUNCH_CHECK("blend_forward_persistent_kernel", in.debug, s);
     return SGB_OK;
 }
